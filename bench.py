@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- recommend() users/sec of the B200 score + top-K engine on BASELINE.json's configurations.
+"""bench.py -- recommend() users/sec of the H100 score + top-K engine on BASELINE.json's configurations.
 
-    python bench.py --gpus N --steps K --warmup W [--config c2|c3|c4|c5] [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--config c2|c3|c4|c5] [--impl reference] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path (score every user against the catalogue, mask viewed items, keep the K best)
 over one batch of synthetic users (SURVEY.md section 8d synthetic inputs: N(0,1)/sqrt(d) factors, fixed seeds, ~100 viewed
@@ -22,6 +22,10 @@ items per user).  Named workloads (BASELINE.json `configs[1..4]`; the default is
            `rectools_b200.install()`, users/sec incl. the host code around the ranker (N = 1, when the package is staged)
   --impl reference : the reference's CPU path (restatement of implicit.cpu.topk: BLAS sgemm + OpenMP select, all host
            threads) on a bounded sample of the same workload, rank 0 only.
+  --dump-outputs DIR : after the timed steps, rank 0 writes what the last timed step returned for a fixed, seeded sample of
+           the users (at most 64 MB in all) as DIR/rows.npy (user rows), DIR/ids.npy, DIR/scores.npy ([rows, K] float64 ids,
+           float32 scores) and, on one GPU, DIR/counts.npy: two builds run with the same arguments can be compared output for
+           output.
 """
 from __future__ import annotations
 
@@ -230,7 +234,7 @@ def model_recommend_leg(a, items, users, indptr, indices, dev_index):
     from oracle import stage_reference
 
     if not stage_reference.available():
-        return {"unavailable": "reference package not staged (oracle/_ref is made by __graft_entry__.build() in the build container)"}
+        return {"unavailable": "reference package not staged (oracle/_ref is made by __graft_entry__.build() when a reference checkout is found)"}
     added = stage_reference.add_to_path()
     try:
         import pandas as pd
@@ -278,6 +282,22 @@ def model_recommend_leg(a, items, users, indptr, indices, dev_index):
         stage_reference.remove_from_path(added)
 
 
+def dump_outputs(out_dir, result, k):
+    """The last timed step's (ids, scores[, counts]) for a seeded sample of at most ~60 MB of rows (float64 ids: exact)."""
+    ids = result["ids"].cpu().numpy()
+    sc = result["sc"].cpu().numpy()
+    n = ids.shape[0]
+    per_row = k * (8 + 4) + 8 + 8
+    n_keep = min(n, max(1, 60_000_000 // per_row))
+    rows = np.sort(np.random.default_rng(12345).choice(n, n_keep, replace=False)) if n_keep < n else np.arange(n)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "rows.npy"), rows.astype(np.float64))
+    np.save(os.path.join(out_dir, "ids.npy"), ids[rows].astype(np.float64))
+    np.save(os.path.join(out_dir, "scores.npy"), sc[rows].astype(np.float32))
+    if result.get("cnt") is not None:
+        np.save(os.path.join(out_dir, "counts.npy"), result["cnt"].cpu().numpy()[rows].astype(np.float64))
+
+
 # --------------------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -299,6 +319,7 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-model", action="store_true", help="skip the model.recommend() leg")
     ap.add_argument("--no-share", action="store_true", help="N > 1: no threshold sharing between the item shards")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's results (a seeded sample) here")
     ap.add_argument("--item-shards", type=int, default=0,
                     help="N > 1: item shards I (a divisor of N); the ranks form I item shards x N/I user groups.  0 = N (the north-star "
                          "scheme: every rank ranks all users against 1/N of the catalogue); 1 = plain user sharding")
@@ -378,7 +399,7 @@ def main():
                 subjects=d_users.data_ptr(), indptr=d_indptr.data_ptr(), indices=d_indices.data_ptr(),
                 stream=torch.cuda.current_stream().cuda_stream,
             )
-            result["ids"], result["sc"] = o_ids, o_sc
+            result["ids"], result["sc"], result["cnt"] = o_ids, o_sc, o_cnt
         else:
             result["ids"], result["sc"], result["cnt"] = sharded.rank_device(d_users, k, d_indptr, d_indices)
             st = dict(sharded.last_stats)
@@ -455,6 +476,8 @@ def main():
     timed_launches = launches[0]
     timed_stats = list(stats_log)
     value = n_users_all * a.steps / (total_ms / 1e3)  # whole job: all user groups
+    if a.dump_outputs and rank == 0 and a.steps > 0:
+        dump_outputs(a.dump_outputs, result, k)
 
     e2e = None
     if not a.no_e2e:
@@ -493,27 +516,17 @@ def main():
         peak = peaks.get("bf16_tflops_sustained")
         peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (the kernel runs ~all of a long step)"
         if peak is None:
-            peak, peak_src = 1400.0, "fallback 1.4 PFLOP/s sustained (B200_PROFILING.md; MEASURED_PEAKS.json absent)"
+            peak, peak_src = 989.0, "H100 SXM data sheet, dense FP16 / BF16 at 700 W (not a measured rate; MEASURED_PEAKS.json absent)"
         achieved = flops / (ms_main * 1e-3) / 1e12
-        # dram__bytes_read + write of one launch of this kernel from the committed `ncu --set full` capture, when that
-        # capture was taken on exactly this workload; otherwise null
         traffic = None
-        for cap_name in ("r02_ncu_fused_kernel.json", "r01_ncu_tc_kernel.json"):
-            try:
-                cap = json.load(open(os.path.join(ROOT, "profiles", cap_name)))
-                if world == 1 and (cap["users"], cap["items"], cap["dim"]) == (n_loc_users, a.items, a.dim) and cap.get("k", 10) == k:
-                    traffic = cap["dram_bytes_per_launch"]
-                    break
-            except (OSError, ValueError, KeyError):
-                pass
         shard_bytes = int(n_loc * info["d_pad"] * 2)
         n_waves = -(-(-(-n_loc_users // 256)) // (info["sm_count"] // 2))  # waves of subject tiles = HBM passes over the shard
         roof = {
-            "kernel": f"fused_topk_kernel<{st0.get('epi_warps', 8)}> (TMA -> tcgen05.mma.cta_group::2 256x256x16 -> TMEM -> fused streaming "
-                      "top-K' selection" + (", wide mode: frozen threshold + global append" if st0.get("wide") else "") + ")",
+            "kernel": f"fused_topk_kernel<{st0.get('epi_warps', 8)}> (TMA -> wgmma 64x64x16 -> accumulators staged in shared memory -> "
+                      "fused streaming top-K' selection" + (", wide mode: frozen threshold + global append" if st0.get("wide") else "") + ")",
             "bound": "tensor",
             "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
-            "frac": achieved / peak, "traffic": traffic, "traffic_unit": "bytes per launch (ncu dram read+write)", "peak_source": peak_src,
+            "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
             "algorithmic": f"2*U*N_g*d = 2*{n_loc_users}*{n_loc}*{a.dim} FLOP per step",
             "ms_per_launch": ms_main, "launches_per_step": st0.get("n_tc_launches"),
             "ms_select_per_step": ms_select,
@@ -521,7 +534,7 @@ def main():
             "frac_of_burst": achieved / peaks["bf16_tflops"] if peaks.get("bf16_tflops") else None,
             "item_stream": {
                 "note": "item-factor HBM stream: the carousel keeps the CTA pairs on the same object tiles, so the 16-bit shard is read "
-                        "from HBM about once per wave of subject tiles (the other 73 of 74 reads are L2 hits); the path is tensor-bound",
+                        "from HBM about once per wave of subject tiles (the other reads are meant to be L2 hits)",
                 "shard_bytes": shard_bytes, "hbm_passes_per_step": n_waves,
                 "achieved_gbs": shard_bytes * n_waves / (ms_main * 1e-3) / 1e9,
                 "hbm_gbs_peak": peaks.get("hbm_gbs"),

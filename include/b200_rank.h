@@ -1,5 +1,5 @@
 /*
- * b200_rank.h -- C ABI of the B200-native score + top-K engine (libb200rank.so).
+ * b200_rank.h -- C ABI of the H100-native (sm_90a) score + top-K engine (libb200rank.so).
  *
  * This is the drop-in boundary for RecTools' vector-ranking hot path.  Paths below are relative to the reference
  * checkout (RecTools 0.17.0).  Plain pointers and sizes only; no Python / torch types cross this boundary.
@@ -35,7 +35,7 @@
  *
  * Error convention: every function returns 0 on success or a negative B200_E_* code; a human-readable message for the
  * last failure on the calling thread is available from b200_rank_last_error().  There is NO CPU fallback: if no
- * sm_100 device is present b200_rank_create fails with B200_E_CUDA.
+ * sm_90 device is present b200_rank_create fails with B200_E_CUDA.
  *
  * Threading: calls on one engine are serialised by an internal mutex; distinct engines are independent.
  */
@@ -53,7 +53,7 @@ extern "C" {
 /* error codes */
 #define B200_OK 0
 #define B200_E_INVALID (-1) /* contract violation (bad shape / pointer / k) */
-#define B200_E_CUDA (-2)    /* CUDA runtime / driver failure, or no sm_100 device */
+#define B200_E_CUDA (-2)    /* CUDA runtime / driver failure, or no sm_90 device */
 #define B200_E_NOMEM (-3)
 #define B200_E_UNSUPPORTED (-4)
 

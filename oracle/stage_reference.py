@@ -1,8 +1,10 @@
 """Stage the unmodified reference package where the GPU box can import it (test / measurement infrastructure only).
 
-`/root/reference` exists in the build container only.  `stage()` -- called by `__graft_entry__.build()` there -- copies the
-reference's pure-Python package `rectools/` as it lies into the git-ignored `oracle/_ref/` (never into the history), from
-where it travels to the GPU box with the repo snapshot exactly like the built `.so` files.  Together with
+The reference is a RecTools source checkout: the directory named by the RECTOOLS_REFERENCE environment variable, else
+the build environment's checkout at /root/reference.  `stage()` -- called by `__graft_entry__.build()` -- copies its
+pure-Python package `rectools/` as it lies into the git-ignored `oracle/_ref/` (never into the history), from where it
+can travel with the working tree exactly like the built `.so` files.  Without a checkout nothing is staged and the tests
+that run the reference package skip.  Together with
 `oracle/implicit_stub` (import-only placeholders for the third-party `implicit` package + the oracle's restatement of its
 top-k) the UNMODIFIED `rectools.models.*` then run on the GPU box: `rectools_b200.install()` is exercised against the real
 `VectorModel` / `ModelBase.recommend` / `DistanceSimilarityModule`, and `bench.py` can time `model.recommend()`.
@@ -16,7 +18,7 @@ import sys
 import typing as tp
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = "/root/reference"
+SRC = os.environ.get("RECTOOLS_REFERENCE") or "/root/reference"
 DST = os.path.join(HERE, "_ref")
 STUB = os.path.join(HERE, "implicit_stub")
 
@@ -32,9 +34,9 @@ def _tree_stamp(root: str) -> tp.Tuple[int, int]:
 
 
 def stage() -> tp.Optional[str]:
-    """Copy `/root/reference/rectools` to `oracle/_ref/rectools` (no-op without the checkout or when up to date)."""
+    """Copy `<checkout>/rectools` to `oracle/_ref/rectools` (no-op without the checkout or when up to date)."""
     src = os.path.join(SRC, "rectools")
-    if not os.path.isdir(src):
+    if not SRC or not os.path.isdir(src):
         return None
     dst = os.path.join(DST, "rectools")
     if os.path.isdir(dst) and _tree_stamp(dst) == _tree_stamp(src):
@@ -48,7 +50,7 @@ def stage() -> tp.Optional[str]:
 def reference_root() -> tp.Optional[str]:
     """Directory to put on sys.path for `import rectools`: the staged copy, else the checkout, else None."""
     for root in (DST, SRC):
-        if os.path.isfile(os.path.join(root, "rectools", "__init__.py")):
+        if root and os.path.isfile(os.path.join(root, "rectools", "__init__.py")):
             return root
     return None
 
@@ -61,7 +63,7 @@ def add_to_path() -> tp.List[str]:
     """Prepend the reference package and the `implicit` stub to sys.path; returns the entries added."""
     root = reference_root()
     if root is None:
-        raise ImportError("the reference package is neither staged (oracle/_ref) nor checked out (/root/reference)")
+        raise ImportError("the reference package is neither staged (oracle/_ref) nor checked out ($RECTOOLS_REFERENCE or /root/reference)")
     added = []
     for p in (os.path.abspath(STUB), os.path.abspath(root)):
         if p not in sys.path:

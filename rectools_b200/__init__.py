@@ -1,4 +1,4 @@
-"""rectools_b200: a B200-native (sm_100a) scoring + top-K engine for RecTools' vector-ranking path.
+"""rectools_b200: an H100-native (sm_90a) scoring + top-K engine for RecTools' vector-ranking path.
 
 Public surface (host-side mirror of `rectools.models.rank`):
   * `Distance`, `B200Ranker`              -- drop-in for `ImplicitRanker` / the `Ranker` protocol

@@ -120,7 +120,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise B200RankError(
             f"{LIB_PATH} is missing: build it with `python -m rectools_b200.build` "
-            "(nvcc, sm_100a).  rectools_b200 has no CPU fallback."
+            "(nvcc, sm_90a).  rectools_b200 has no CPU fallback."
         )
     lib = C.CDLL(LIB_PATH)
     vp, i32, i64 = C.c_void_p, C.c_int32, C.c_int64

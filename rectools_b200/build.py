@@ -1,4 +1,4 @@
-"""Build libb200rank.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libb200rank.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m rectools_b200.build [--force] [--verbose]
 """
@@ -17,7 +17,7 @@ SOURCES = ["engine.cu"]
 HEADERS = ["common.cuh", "prep.cuh", "select.cuh", "sparse.cuh", "tc_common.cuh", "fused_topk.cuh", os.path.join("..", "..", "include", "b200_rank.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-Wno-format-truncation",
     "-shared",

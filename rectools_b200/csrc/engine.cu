@@ -1,4 +1,4 @@
-// libb200rank.so -- host side of the B200 score + top-K engine behind the C ABI of include/b200_rank.h.
+// libb200rank.so -- host side of the H100 (sm_90a) score + top-K engine behind the C ABI of include/b200_rank.h.
 //
 // Reference seams (RecTools 0.17.0): `ImplicitRanker.rank` (rectools/models/rank/rank_implicit.py:187-280),
 // `ImplicitRanker._rank_on_gpu` (:148-185) and `TorchRanker.rank` (rectools/models/rank/rank_torch.py:77-177).
@@ -89,13 +89,13 @@ PFN_encodeTiled get_encode_tiled() {
     return fn;
 }
 
-// Row-major [rows, d_pad] 16-bit matrix, boxes of [128 rows x 64 cols] (128-byte rows, SWIZZLE_128B).
-bool make_tensor_map(CUtensorMap* tm, const void* base, int64_t rows, int d_pad, bool is_bf16) {
+// Row-major [rows, d_pad] 16-bit matrix, boxes of [box_rows x 64 cols] (128-byte rows, SWIZZLE_128B).
+bool make_tensor_map(CUtensorMap* tm, const void* base, int64_t rows, int d_pad, bool is_bf16, int box_rows) {
     PFN_encodeTiled enc = get_encode_tiled();
     if (!enc) return false;
     cuuint64_t dims[2] = {(cuuint64_t)d_pad, (cuuint64_t)rows};
     cuuint64_t strides[1] = {(cuuint64_t)d_pad * 2};
-    cuuint32_t box[2] = {(cuuint32_t)b200::tc::KBLK, 128u};
+    cuuint32_t box[2] = {(cuuint32_t)b200::tc::KBLK, (cuuint32_t)box_rows};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = enc(tm, is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
                      const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -216,7 +216,7 @@ void prepare_objects(b200_rank_engine* E, int tc_mode) {
     memcpy(&maxnorm, &h[1], 4);
     E->max_obj_norm = maxnorm;
 
-    if (tc_mode == B200_TC_OFF || E->cc_major != 10 || E->sm_count % 2 != 0) {
+    if (tc_mode == B200_TC_OFF || E->cc_major != 9 || E->sm_count % 2 != 0) {
         E->tc_dtype = B200_TC_OFF;
         return;
     }
@@ -247,23 +247,12 @@ TcPlan plan_fused(int d_pad) {
     TcPlan pl{};
     pl.kblocks = d_pad / tc::KBLK;
     const int fixed = pl.kblocks * tc::BLK_BYTES + tc::FusedCfg<NW>::FIXED_BYTES;
-    int stages = (tc::SMEM_LIMIT - fixed) / tc::BLK_BYTES;
+    int stages = (tc::SMEM_LIMIT - fixed) / tc::OBJ_BLK_BYTES;
     if (stages > tc::MAX_STAGES) stages = tc::MAX_STAGES;
     pl.ok = stages >= 2;
     pl.n_stages = stages;
-    pl.smem_bytes = fixed + stages * tc::BLK_BYTES;
+    pl.smem_bytes = fixed + stages * tc::OBJ_BLK_BYTES;
     return pl;
-}
-
-uint32_t make_idesc(bool bf16) {
-    uint32_t d = 0;
-    d |= 1u << 4;                       // accumulator format: F32
-    d |= (bf16 ? 1u : 0u) << 7;         // A format
-    d |= (bf16 ? 1u : 0u) << 10;        // B format
-    // bits 13/14: no negate; bits 15/16: both operands K-major
-    d |= (uint32_t)(tc::TILE_N >> 3) << 17;
-    d |= (uint32_t)(256 >> 4) << 24;    // M = 256 across the CTA pair
-    return d;
 }
 
 int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int64_t n_objects, int32_t d, int32_t distance,
@@ -294,9 +283,9 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
         E->cc_major = prop.major;
         E->cc_minor = prop.minor;
         snprintf(E->dev_name, sizeof(E->dev_name), "%.127s", prop.name);
-        if (prop.major != 10) {
+        if (prop.major != 9 || prop.minor != 0) {
             delete E;
-            return fail(B200_E_CUDA, "b200_rank_create: device %d is sm_%d%d; this library contains sm_100a code only",
+            return fail(B200_E_CUDA, "b200_rank_create: device %d is sm_%d%d; this library contains sm_90a code only",
                         device, prop.major, prop.minor);
         }
         E->distance = distance;
@@ -333,12 +322,17 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
             if (!p8.ok || !p16.ok) {
                 E->tc_dtype = B200_TC_OFF;
             } else {
-                CK(cudaFuncSetAttribute(tc::fused_topk_kernel<8, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, p8.smem_bytes));
-                CK(cudaFuncSetAttribute(tc::fused_topk_kernel<8, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, p8.smem_bytes));
-                CK(cudaFuncSetAttribute(tc::fused_topk_kernel<8, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, p8.smem_bytes));
-                CK(cudaFuncSetAttribute(tc::fused_topk_kernel<16, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, p16.smem_bytes));
-                CK(cudaFuncSetAttribute(tc::fused_topk_kernel<16, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, p16.smem_bytes));
-                CK(cudaFuncSetAttribute(tc::fused_topk_kernel<16, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, p16.smem_bytes));
+                auto allow = [](const void* f, int bytes) { CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)); };
+#define B200_ALLOW(NW_, PL_)                                                                                        \
+    allow((const void*)tc::fused_topk_kernel<NW_, false, false, false>, PL_.smem_bytes);                            \
+    allow((const void*)tc::fused_topk_kernel<NW_, true, false, false>, PL_.smem_bytes);                             \
+    allow((const void*)tc::fused_topk_kernel<NW_, false, true, false>, PL_.smem_bytes);                             \
+    allow((const void*)tc::fused_topk_kernel<NW_, false, false, true>, PL_.smem_bytes);                             \
+    allow((const void*)tc::fused_topk_kernel<NW_, true, false, true>, PL_.smem_bytes);                              \
+    allow((const void*)tc::fused_topk_kernel<NW_, false, true, true>, PL_.smem_bytes)
+                B200_ALLOW(8, p8);
+                B200_ALLOW(16, p16);
+#undef B200_ALLOW
             }
         }
         CK(cudaFuncSetAttribute(rescore_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
@@ -533,7 +527,8 @@ void run_tc(Call& c, const TcPass& t) {
         obj_rows = npad;
     }
     CUtensorMap tm_obj, tm_sub;
-    if (!make_tensor_map(&tm_obj, obj_base, obj_rows, E->d_pad, bf16) || !make_tensor_map(&tm_sub, E->sub16.p, rows_pad, E->d_pad, bf16))
+    if (!make_tensor_map(&tm_obj, obj_base, obj_rows, E->d_pad, bf16, tc::QUART_N) ||
+        !make_tensor_map(&tm_sub, E->sub16.p, rows_pad, E->d_pad, bf16, tc::TILE_M))
         throw CudaError{cudaErrorUnknown, "cuTensorMapEncodeTiled", __LINE__};
 
     tc::TcParams tp{};
@@ -564,7 +559,6 @@ void run_tc(Call& c, const TcPass& t) {
     }
     tp.n_splits = best_splits;
     tp.tiles_per_split = (tp.n_obj_tiles + best_splits - 1) / best_splits;
-    tp.idesc = make_idesc(bf16);
     tp.pos2obj = c.wl;
     tp.indptr = t.indptr;
     tp.indices = c.indices;
@@ -629,8 +623,13 @@ void run_tc(Call& c, const TcPass& t) {
     const int grid = 2 * std::min(n_work, n_units);
     c.time_begin(0);
     const bool use_peers = t.peers && tp.n_peers > 0;  // (wide mode and threshold sharing never meet: sharing needs k <= 24)
-#define B200_LAUNCH(NW_, WIDE_, PEERS_) \
-    tc::fused_topk_kernel<NW_, WIDE_, PEERS_><<<grid, tc::FusedCfg<NW_>::THREADS, pl.smem_bytes, st>>>(tm_sub, tm_obj, tp)
+#define B200_LAUNCH(NW_, WIDE_, PEERS_)                                                                                              \
+    do {                                                                                                                       \
+        if (bf16)                                                                                                              \
+            tc::fused_topk_kernel<NW_, WIDE_, PEERS_, true><<<grid, tc::FusedCfg<NW_>::threads(PEERS_), pl.smem_bytes, st>>>(tm_sub, tm_obj, tp); \
+        else                                                                                                                   \
+            tc::fused_topk_kernel<NW_, WIDE_, PEERS_, false><<<grid, tc::FusedCfg<NW_>::threads(PEERS_), pl.smem_bytes, st>>>(tm_sub, tm_obj, tp); \
+    } while (0)
     if (t.nw == 8) {
         if (t.wide) B200_LAUNCH(8, true, false);
         else if (use_peers) B200_LAUNCH(8, false, true);
@@ -1065,9 +1064,8 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
         // certificate and take the second-chance pass.  Inserts, the dominant epilogue cost, scale with K'.
         c.bf16 = E->tc_dtype == B200_TC_BF16;
         const bool wide = k_out > 24 && k_out <= 128 && env_int("B200_WIDE", 1) != 0;
-        // 16 epilogue warps (B200_EPI_WARPS=16) measured 5 % slower at N = 1M, 5 % faster on a 125 K-object shard, equal at
-        // d = 256 (profiles/r02_ab_fused.txt): opt-in.  The wide mode always runs the 8-warp geometry: four lists per row
-        // freeze at a weaker, noisier rank and 10 % of the rows miss their candidate count.
+        // 16 epilogue warps (B200_EPI_WARPS=16) are opt-in: next to the MMA warp group they get 96 registers a thread and
+        // spill.  The wide mode always runs the 8-warp geometry: four lists per row freeze at a weaker, noisier rank.
         c.nw = (!wide && env_int("B200_EPI_WARPS", 8) == 16) ? 16 : 8;
         int k_cand = 0;
         if (k_out <= 24) {

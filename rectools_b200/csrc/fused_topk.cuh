@@ -1,19 +1,20 @@
-// The fused scoring + candidate-selection kernel: one persistent CTA pair per two SMs.
+// The fused scoring + candidate-selection kernel: one persistent CTA per SM, two CTAs (a "pair") per 256 subject rows.
 //
-//   TMA (own 128 subject rows once per work item; own half of every 256-object tile through a ring of 16 KiB blocks)
-//   -> tcgen05.mma.cta_group::2 256 x 256 x 16 (fp16 / bf16 -> fp32), two 256-column accumulators per CTA in TMEM
-//   -> tcgen05.ld of a [32 rows x COLS columns] slice per epilogue warp into registers, accumulator handed back at once
-//   -> threshold scan (3-input max tree, ONE vote per tile), hits extracted into per-thread ring FIFOs in shared memory
+//   TMA (own 128 subject rows once per work item; every 256-object tile as four quarters of 64 objects, streamed through a
+//   ring of 8 KiB blocks) -> wgmma 64 x 64 x 16 (fp16 / bf16 -> fp32) into the registers of the MMA warp group
+//   -> each finished quarter [128 rows x 64 columns] is staged in shared memory and read back by the epilogue warps, one
+//   row per thread; the staging buffer is handed back as soon as the rows are in registers
+//   -> threshold scan (3-input max tree), hits extracted into per-thread ring FIFOs in shared memory
 //   -> deferred, bounded steps: filter_pairs_csr lookup through a prefetched 4-entry window, candidate-list insertion.
 // Score rows never reach HBM: only the K' best (score, id) pairs per row and column group are written.
 //
-// NW = epilogue warps per CTA:
-//   8  : 32 rows x 128 columns per warp, two candidate lists per row (32 slots each), 232 registers per epilogue thread
-//   16 : 32 rows x  64 columns per warp, four lists per row (16 slots each), 120 registers; four warps per scheduler
-//        hide each other's latencies and a warp is hit by half as many candidates.
-// Warp group 0: warp 0 = TMA producer, warp 1 = MMA issuer + TMEM allocator (leader CTA issues), warps 2-3 = peer-threshold
-// helpers (multi-GPU: they poll the other ranks' published thresholds over NVLink and publish this rank's; idle otherwise).
-// `setmaxnreg` moves the registers warp group 0 does not need to the epilogue warps.
+// NW = epilogue warps per CTA; column group g of a tile is made of the quarters g, g + NW / 4, ...:
+//   8  : two quarters (128 columns) per warp and tile, two candidate lists per row (32 slots each)
+//   16 : one quarter (64 columns) per warp and tile, four lists per row (16 slots each)
+// Warps 0-3: the MMA warp group (thread 0 also issues every TMA load); warps 4 .. 4 + NW - 1: epilogue; with PEERS two
+// more warps poll the other ranks' published thresholds over NVLink and publish this rank's.
+// The two CTAs of a pair work on the same object tiles in the same order; the odd CTA waits for the start tile the even
+// one publishes through global memory, so the pair is launched as a cluster of two (co-scheduled by the hardware).
 //
 // Three selection modes share the epilogue:
 //   * adaptive lists (k <= 24): replace-minimum lists of K' slots, the list minimum is the running threshold;
@@ -35,24 +36,21 @@ constexpr uint32_t TAG_NONE = 0xffffffffu, TAG_DONE = 0xfffffffeu;  // exchange-
 template <int NW>
 struct FusedCfg {
     static_assert(NW == 8 || NW == 16, "8 or 16 epilogue warps");
-    static constexpr int EPI0 = 4;                    // first epilogue warp; (warp & 3) is its TMEM lane quarter
-    static constexpr int THREADS = (EPI0 + NW) * 32;
+    static constexpr int EPI0 = 4;                    // first epilogue warp; (warp & 3) is its row quarter
+    static constexpr int HELPERS = 2;                 // peer-threshold warps behind the epilogue (PEERS kernels only)
+    static constexpr int threads(bool peers) { return (EPI0 + NW + (peers ? HELPERS : 0)) * 32; }
     static constexpr int COLS = 1024 / NW;            // accumulator columns per epilogue thread and tile
     static constexpr int NLIST = NW / 4;              // column groups = candidate lists per row
+    static constexpr int NQ = COLS / QUART_N;         // staged quarters per epilogue thread and tile
     static constexpr int SLOTS = 64 / NLIST;          // list capacity (K' <= SLOTS)
-    // setmaxnreg moves registers inside the CTA's LAUNCH allocation (168 x 384 = 64512, 96 x 640 = 61440), not the whole file:
-    // 4 * REGS_LOW + NW * REGS_EPI <= launch registers * (4 + NW).  (120 for the 16-warp geometry over-subscribes the pool: the
-    // last epilogue warps wait for ever in setmaxnreg.inc -- the first hardware run of round 2.)
-    static constexpr int REGS_LOW = NW == 8 ? 40 : 32;
-    static constexpr int REGS_EPI = NW == 8 ? 232 : 112;
-    static constexpr int Q = NW == 8 ? 8 : 4;         // deferred hits per thread (ring FIFO), measured with the step period
+    static constexpr int Q = NW == 8 ? 8 : 4;         // deferred hits per thread (ring FIFO)
     static constexpr int QSTRIDE = NW * 32 * 8;       // bytes between FIFO slots: [slot][epilogue thread] x (score, position)
     static constexpr int QBYTES = Q * QSTRIDE;
     static constexpr int BACKLOG = NW == 8 ? 4 : 2;   // a row with this many pending hits gets a step at once
     static constexpr int PERIOD = 16;                 // otherwise deferred work runs every PERIOD-th tile (power of two)
     static constexpr int LIST_BYTES = NLIST * TILE_M * SLOTS * 4;  // one of the two arrays (scores / ids): 32 KiB
     static constexpr int THR_BYTES = (NLIST + 1) * TILE_M * 8;     // (tag, threshold) per list + one slot for the peers' maximum
-    static constexpr int FIXED_BYTES = 2 * LIST_BYTES + QBYTES + THR_BYTES + 1024 /*alignment slack*/ + 512 /*barriers*/;
+    static constexpr int FIXED_BYTES = STG_BYTES + 2 * LIST_BYTES + QBYTES + THR_BYTES + 1024 /*alignment slack*/ + 512 /*barriers*/;
 };
 
 // Move this thread's pending hits of chunk OFF (ascending column order) into its FIFO (a ring of QN slots).  Returns
@@ -136,205 +134,175 @@ __device__ __forceinline__ void fifo_step(const TcParams& p, RowState& rs, CsrWi
     }
 }
 
-// Shared-memory map (dynamic, 1 KiB aligned): [KB] subject blocks | [NS] object blocks (16 KiB each: this CTA's half of a
-// 256-object tile) | candidate lists [NLIST][128 rows][SLOTS] scores + ids | FIFOs | thresholds [NLIST + 1][128] | barriers.
+// Shared-memory map (dynamic, 1 KiB aligned): [KB] subject blocks (16 KiB each) | [NS] object blocks (8 KiB each: 64
+// objects of a tile quarter) | accumulator staging [128 rows][STG_STRIDE] fp32 | candidate lists [NLIST][128 rows][SLOTS]
+// scores + ids | FIFOs | thresholds [NLIST + 1][128] | barriers.
 // WIDE / PEERS compile the wide mode (threshold freeze + global append) and the peer-threshold exchange in; the plain
-// instantiation carries neither in its tile loop (measured: the run-time switches cost the 8-warp kernel ~6 %).
-template <int NW, bool WIDE, bool PEERS>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(FusedCfg<NW>::THREADS, 1)
+// instantiation carries neither in its tile loop.  BF16 selects the MMA operand type.
+template <int NW, bool WIDE, bool PEERS, bool BF16>
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(FusedCfg<NW>::threads(PEERS), 1)
 fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_constant__ CUtensorMap tm_obj, const TcParams p) {
     using Cfg = FusedCfg<NW>;
-    constexpr int NBUF = 2;
-    constexpr int COLS = Cfg::COLS, NLIST = Cfg::NLIST, SLOTS = Cfg::SLOTS, QN = Cfg::Q, QS = Cfg::QSTRIDE;
+    constexpr int NLIST = Cfg::NLIST, SLOTS = Cfg::SLOTS, NQ = Cfg::NQ, QN = Cfg::Q, QS = Cfg::QSTRIDE;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
 
     const int KB = p.kblocks, NS = p.n_stages;
     uint8_t* sA = smem;
     uint8_t* sB = sA + (size_t)KB * BLK_BYTES;
-    uint8_t* sLs = sB + (size_t)NS * BLK_BYTES;  // per warp [slot][lane] arrays
+    uint8_t* sStg = sB + (size_t)NS * OBJ_BLK_BYTES;
+    uint8_t* sLs = sStg + STG_BYTES;  // per warp [slot][lane] arrays
     uint8_t* sLi = sLs + Cfg::LIST_BYTES;
     uint8_t* sQ = sLi + Cfg::LIST_BYTES;
     unsigned long long* sThr = reinterpret_cast<unsigned long long*>(sQ + Cfg::QBYTES);  // [NLIST + 1][128]
     uint64_t* bars = reinterpret_cast<uint64_t*>(sThr + (NLIST + 1) * TILE_M);
-    const uint32_t bar_full = smem_u32(bars);
-    const uint32_t bar_empty = smem_u32(bars + MAX_STAGES);
-    const uint32_t bar_afull = smem_u32(bars + 2 * MAX_STAGES);
-    const uint32_t bar_aempty = smem_u32(bars + 2 * MAX_STAGES + 1);
-    const uint32_t bar_tfull = smem_u32(bars + 2 * MAX_STAGES + 2);
-    const uint32_t bar_tempty = smem_u32(bars + 2 * MAX_STAGES + 2 + NBUF);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * MAX_STAGES + 2 + 2 * NBUF);
+    const uint32_t bar_full = smem_u32(bars);                     // [NS] object block landed
+    const uint32_t bar_afull = smem_u32(bars + MAX_STAGES);       // subject blocks landed
+    const uint32_t bar_qfull = smem_u32(bars + MAX_STAGES + 1);   // [4] quarter q of the current tile staged
+    const uint32_t bar_qempty = smem_u32(bars + MAX_STAGES + 5);  // staged quarter read by its four epilogue warps
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();  // 0 = leader
+    const int rank = blockIdx.x & 1;  // which 128 rows of the pair's 256 (== the CTA's rank in its cluster)
     const int n_pairs = gridDim.x >> 1, pair = blockIdx.x >> 1;
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < NS; ++i) {
-            mbar_init(bar_full + 8 * i, 1);   // leader's copy is the one that counts
-            mbar_init(bar_empty + 8 * i, 1);  // one multicast commit per use
-        }
+        for (int i = 0; i < NS; ++i) mbar_init(bar_full + 8 * i, 1);
         mbar_init(bar_afull, 1);
-        mbar_init(bar_aempty, 1);
-        for (int b = 0; b < NBUF; ++b) {
-            mbar_init(bar_tfull + 8 * b, 1);
-            mbar_init(bar_tempty + 8 * b, 2 * NW);  // the epilogue warps of both CTAs arrive on the leader's copy
-        }
+        for (int q = 0; q < 4; ++q) mbar_init(bar_qfull + 8 * q, 128);  // every thread of the MMA warp group
+        mbar_init(bar_qempty, 4);
         fence_barrier_init();
         tma_prefetch_desc(&tm_sub);
         tma_prefetch_desc(&tm_obj);
     }
     for (int i = threadIdx.x; i < (NLIST + 1) * TILE_M; i += blockDim.x) sts_thr(smem_u32(sThr + i), TAG_NONE, INFINITY);
-    if (warp == 1) {
-        tmem_alloc_2sm(smem_u32(tmem_slot), TMEM_COLS);
-        tmem_relinquish_2sm();
-    }
-    tc_fence_before();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    if (tmem_base != 0) __trap();  // all 512 columns are ours
+    __syncthreads();
 
     const int n_work = p.n_row_tiles * p.n_splits;
-    constexpr uint32_t BLK16 = BLK_BYTES >> 4;  // a 16 KiB block in descriptor address units
+    constexpr uint32_t BLK16 = BLK_BYTES >> 4, OBJ16 = OBJ_BLK_BYTES >> 4;  // blocks in descriptor address units
 
-    if (warp < Cfg::EPI0) reg_dealloc<Cfg::REGS_LOW>();  // all four warps of warp group 0
-    if (warp == 0) {
-        // ===================================================================== TMA producer (both CTAs, one elected thread)
-        if (elect_one()) {
-            uint32_t stage = 0, ph = 0, work_it = 0;
-            const uint32_t sA_u = smem_u32(sA), sB_u = smem_u32(sB);
-            for (int w = pair; w < n_work; w += n_pairs, ++work_it) {
-                const int split = w / p.n_row_tiles, rt = w - split * p.n_row_tiles;
-                const int t0 = split * p.tiles_per_split;
-                const int t1 = min(t0 + p.tiles_per_split, p.n_obj_tiles);
-                if (work_it > 0) mbar_wait(bar_aempty, (work_it - 1) & 1);
-                if (rank == 0) mbar_arrive_expect_tx(bar_afull, (uint32_t)(2 * KB * BLK_BYTES));
-                for (int kb = 0; kb < KB; ++kb)
-                    tma_load_2d_2sm(sA_u + (uint32_t)kb * BLK_BYTES, &tm_sub, bar_afull, kb * KBLK, (rt * 2 + (int)rank) * TILE_M);
-                const int nt = t1 - t0;
-                const int ts = carousel_start(p, pair, work_it, split, t0, t1, rank == 0);
-                for (int i = 0; i < nt; ++i) {
-                    const int t = ts + i < t1 ? ts + i : ts + i - nt;
-                    // the front is the position of the reference pair (pair 0 of each split's work items); measured: letting
-                    // every pair overwrite it does not re-align pairs that drifted apart (333 GB of DRAM reads instead of 15)
-                    if (rank == 0 && p.front && (i & 15) == 0 && pair == 0)
-                        *reinterpret_cast<volatile int32_t*>(p.front + split) = t;
-                    for (int kb = 0; kb < KB; ++kb) {
-                        mbar_wait(bar_empty + 8 * stage, ph ^ 1);
-                        if (rank == 0) mbar_arrive_expect_tx(bar_full + 8 * stage, 2 * BLK_BYTES);
-                        tma_load_2d_2sm(sB_u + stage * BLK_BYTES, &tm_obj, bar_full + 8 * stage, kb * KBLK,
-                                        t * TILE_N + (int)rank * HALF_N);
-                        if (++stage == (uint32_t)NS) {
-                            stage = 0;
-                            ph ^= 1;
-                        }
+    if (warp < Cfg::EPI0) {
+        // ===================================================================== MMA warp group (+ TMA issue by thread 0)
+        const bool issuer = threadIdx.x == 0;
+        const uint32_t sA_u = smem_u32(sA), sB_u = smem_u32(sB);
+        // Object blocks are issued in consumption order (work item, tile, quarter, k block) up to NS blocks ahead of the
+        // MMAs; a ring slot is refilled once the wgmmas that read it have retired in every thread of the warp group
+        // (wgmma.wait_group waits for the executing thread's groups only, hence the warp-group barrier before the refill).
+        int lw = pair, li = 0, lq = 0, lkb = 0, lnt = 0, lts = 0, lt0 = 0, lt1 = 0, lsplit = 0;
+        uint32_t lwork = 0, lstage = 0;
+        bool lnew = true;
+        int64_t issued = 0, done = 0;
+        auto issue_next = [&]() -> bool {
+            if (lw >= n_work) return false;
+            if (lnew) {
+                lsplit = lw / p.n_row_tiles;
+                lt0 = lsplit * p.tiles_per_split;
+                lt1 = min(lt0 + p.tiles_per_split, p.n_obj_tiles);
+                lnt = lt1 - lt0;
+                lts = carousel_start(p, pair, lwork, lsplit, lt0, lt1, rank == 0);
+                lnew = false;
+            }
+            const int t = lts + li < lt1 ? lts + li : lts + li - lnt;
+            // the front is the position of the reference pair (pair 0 of each split's work items)
+            if (rank == 0 && p.front && pair == 0 && lq == 0 && lkb == 0 && (li & 15) == 0)
+                *reinterpret_cast<volatile int32_t*>(p.front + lsplit) = t;
+            mbar_arrive_expect_tx(bar_full + 8 * lstage, OBJ_BLK_BYTES);
+            tma_load_2d(sB_u + lstage * OBJ_BLK_BYTES, &tm_obj, bar_full + 8 * lstage, lkb * KBLK, t * TILE_N + lq * QUART_N);
+            if (++lstage == (uint32_t)NS) lstage = 0;
+            ++issued;
+            if (++lkb == KB) {
+                lkb = 0;
+                if (++lq == 4) {
+                    lq = 0;
+                    if (++li == lnt) {
+                        li = 0;
+                        lw += n_pairs;
+                        ++lwork;
+                        lnew = true;
                     }
                 }
             }
-        }
-        __syncwarp();
-    } else if (warp == 1) {
-        // ===================================================================== MMA issuer (leader CTA only, one elected thread)
-        // One thread runs the whole role, waits included: with per-k-block election the issue loop cost ~315 cycles per
-        // 4 MMAs (256 cycles of tensor work) and the tensor pipe sat at 45 %.
-        if (rank == 0 && elect_one()) {
-            uint32_t stage = 0, ph = 0, tile_it = 0, work_it = 0;
-            const uint32_t a_lo0 = smem_desc_lo(smem_u32(sA)), b_lo0 = smem_desc_lo(smem_u32(sB));
-            const uint32_t idesc = p.idesc;
-            for (int w = pair; w < n_work; w += n_pairs, ++work_it) {
-                const int split = w / p.n_row_tiles;
-                const int t0 = split * p.tiles_per_split;
-                const int t1 = min(t0 + p.tiles_per_split, p.n_obj_tiles);
-                mbar_wait(bar_afull, work_it & 1);
-                tc_fence_after();
-                for (int t = t0; t < t1; ++t, ++tile_it) {
-                    const uint32_t buf = tile_it & 1, tph = (tile_it >> 1) & 1;
-                    mbar_wait(bar_tempty + 8 * buf, tph ^ 1);  // both CTAs' epilogues have copied this accumulator out
-                    tc_fence_after();
-                    const uint32_t d0 = buf * (uint32_t)TILE_N;
+            return true;
+        };
+        auto refill = [&]() {
+            mma_group_sync();
+            if (issuer)
+                while (issued < done + NS && issue_next()) {
+                }
+        };
+        refill();
+
+        // this thread's accumulator rows / columns in the staging buffer (m-half 1: + 64 rows; second row of a fragment: + 8)
+        const uint32_t stg_w = smem_u32(sStg) + (uint32_t)(((warp * 16 + (lane >> 2)) * STG_STRIDE + 2 * (lane & 3)) * 4);
+        const uint32_t a_lo0 = smem_desc_lo(sA_u), b_lo0 = smem_desc_lo(sB_u);
+        float acc[2][32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[0][i] = acc[1][i] = 0.f;
+        uint32_t stage = 0, ph = 0, work_it = 0, n_store = 0;
+        for (int w = pair; w < n_work; w += n_pairs, ++work_it) {
+            const int split = w / p.n_row_tiles, rt = w - split * p.n_row_tiles;
+            const int t0 = split * p.tiles_per_split;
+            const int t1 = min(t0 + p.tiles_per_split, p.n_obj_tiles);
+            // the previous work item's MMAs have all retired (every quarter ends in wgmma.wait_group 0)
+            if (issuer) {
+                mbar_arrive_expect_tx(bar_afull, (uint32_t)(KB * BLK_BYTES));
+                for (int kb = 0; kb < KB; ++kb)
+                    tma_load_2d(sA_u + (uint32_t)kb * BLK_BYTES, &tm_sub, bar_afull, kb * KBLK, (rt * 2 + rank) * TILE_M);
+            }
+            mbar_wait(bar_afull, work_it & 1);
+            for (int i = 0; i < t1 - t0; ++i) {
+                for (int q = 0; q < 4; ++q) {
                     uint32_t a_lo = a_lo0;
                     for (int kb = 0; kb < KB; ++kb, a_lo += BLK16) {
                         mbar_wait(bar_full + 8 * stage, ph);
-                        tc_fence_after();
-                        const uint32_t b_lo = b_lo0 + stage * BLK16;
-                        // +32 B per K = 16 step inside the 128 B swizzle atom = +2 in descriptor address units
-                        umma_f16_2sm(d0, a_lo, b_lo, SMEM_DESC_HI, idesc, (uint32_t)(kb != 0));
-                        umma_f16_2sm(d0, a_lo + 2, b_lo + 2, SMEM_DESC_HI, idesc, 1u);
-                        umma_f16_2sm(d0, a_lo + 4, b_lo + 4, SMEM_DESC_HI, idesc, 1u);
-                        umma_f16_2sm(d0, a_lo + 6, b_lo + 6, SMEM_DESC_HI, idesc, 1u);
-                        umma_commit_2sm(bar_empty + 8 * stage);  // frees this ring slot in both CTAs
+                        fence_acc(acc[0]);
+                        fence_acc(acc[1]);
+                        wgmma_fence();
+                        const uint32_t b_lo = b_lo0 + stage * OBJ16;
+                        // +32 B per K = 16 step inside the 128 B swizzle atom = +2 in descriptor address units; rows 64-127 of
+                        // the subject block start 8 KiB (+512) further
+#pragma unroll
+                        for (int k = 0; k < 4; ++k) {
+                            const uint32_t accum = (kb | k) != 0;
+                            wgmma_64x64<BF16>(acc[0], a_lo + 2 * k, b_lo + 2 * k, accum);
+                            wgmma_64x64<BF16>(acc[1], a_lo + 512 + 2 * k, b_lo + 2 * k, accum);
+                        }
+                        wgmma_commit();
+                        fence_acc(acc[0]);
+                        fence_acc(acc[1]);
                         if (++stage == (uint32_t)NS) {
                             stage = 0;
                             ph ^= 1;
                         }
+                        if (kb > 0) {
+                            wgmma_wait<1>();  // the previous k block's MMAs have read their ring slot
+                            ++done;
+                            refill();
+                        }
                     }
-                    umma_commit_2sm(bar_tfull + 8 * buf);
+                    wgmma_wait<0>();
+                    fence_acc(acc[0]);
+                    fence_acc(acc[1]);
+                    ++done;
+                    refill();
+                    // hand the quarter to the epilogue once its readers have taken the previous one
+                    mbar_wait(bar_qempty, (n_store & 1) ^ 1);
+#pragma unroll
+                    for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            const uint32_t a = stg_w + (uint32_t)((mh * 64 * STG_STRIDE + 8 * j) * 4);
+                            sts_v2(a, acc[mh][4 * j], __float_as_uint(acc[mh][4 * j + 1]));
+                            sts_v2(a + 8 * STG_STRIDE * 4, acc[mh][4 * j + 2], __float_as_uint(acc[mh][4 * j + 3]));
+                        }
+                    mbar_arrive(bar_qfull + 8 * q);
+                    ++n_store;
                 }
-                umma_commit_2sm(bar_aempty);
             }
         }
-        __syncwarp();
-    } else if (warp < Cfg::EPI0) {
-        // ===================================================================== peer-threshold helpers (warps 2 and 3)
-        // Thread h serves CTA-local rows h and h + 64.  Per round and row: read the row's own thresholds from the exchange
-        // slots, publish their maximum to this rank's global array, read the other ranks' published values (NVLink peer
-        // loads, latency irrelevant here), leave their maximum in the row's extra exchange slot.  All values are monotone
-        // lower bounds of the row's final threshold: a stale one is only weaker, never wrong.
-        if (PEERS && p.n_peers > 0) {
-            const int h = (warp - 2) * 32 + lane;
-            float published[2] = {-INFINITY, -INFINITY};
-            uint32_t pub_tag[2] = {0xffffffffu, 0xffffffffu};
-            bool done[2] = {false, false};
-            while (!(done[0] && done[1])) {
-#pragma unroll
-                for (int s = 0; s < 2; ++s) {
-                    const int r = h + 64 * s;
-                    uint32_t tag;
-                    float own;
-                    lds_thr(smem_u32(sThr + r), tag, own);
-                    done[s] = tag == TAG_DONE;  // the row's first column group has finished its last work item
-                    if (tag >= TAG_DONE) continue;
-#pragma unroll
-                    for (int l = 1; l < NLIST; ++l) {
-                        uint32_t tl;
-                        float vl;
-                        lds_thr(smem_u32(sThr + l * TILE_M + r), tl, vl);
-                        if (tl == tag) own = fmaxf(own, vl);
-                    }
-                    const int w = pair + (int)tag * n_pairs;
-                    if (w >= n_work) continue;
-                    const int rt = w % p.n_row_tiles;
-                    const int64_t grow = ((int64_t)rt * 2 + rank) * TILE_M + r;
-                    if (grow >= p.n_rows) continue;
-                    if (pub_tag[s] != tag) {
-                        pub_tag[s] = tag;
-                        published[s] = -INFINITY;
-                    }
-                    if (own > published[s] && own < INFINITY) {
-                        published[s] = own;
-                        stg_peer(p.peer_pub + p.peer_row0 + grow, p.peer_epoch, ldexpf(own, -p.peer_exp));
-                    }
-                    // all peer loads in flight at once: one NVLink round trip per row and round (issued one after the other the
-                    // seven loads took ~15 us -- 20 tiles -- and the shared thresholds arrived after the warm-up they are meant
-                    // to shorten: first 8-GPU measurement of round 2)
-                    unsigned long long v[MAX_PEERS];
-#pragma unroll
-                    for (int q = 0; q < MAX_PEERS; ++q) v[q] = q < p.n_peers ? ldg_peer(p.peer_in[q] + p.peer_row0 + grow) : 0ull;
-                    float best = -INFINITY;
-#pragma unroll
-                    for (int q = 0; q < MAX_PEERS; ++q)
-                        if (q < p.n_peers && (uint32_t)(v[q] >> 32) == p.peer_epoch) best = fmaxf(best, __uint_as_float((uint32_t)v[q]));
-                    if (best > -INFINITY) sts_thr(smem_u32(sThr + NLIST * TILE_M + r), tag, ldexpf(best, p.peer_exp));
-                }
-                __nanosleep(200);
-            }
-        }
-    } else if (warp >= Cfg::EPI0) {
-        // ===================================================================== epilogue (both CTAs): select candidates
-        reg_alloc<Cfg::REGS_EPI>();
+    } else if (warp < Cfg::EPI0 + NW) {
+        // ===================================================================== epilogue: select candidates
         const int ew = warp - Cfg::EPI0;
-        const int colg = ew >> 2, quarter = warp & 3;  // column group of the tile / TMEM lane quarter (== warp % 4)
+        const int colg = ew >> 2, quarter = warp & 3;  // column group of the tile / row quarter of the CTA's 128 rows
         const int wrow0 = quarter * 32;                // first CTA-local subject row of this warp
         // [slot][lane] arrays of this warp: SLOTS x 32 lanes x 4 B, slot stride 128 B (as list_insert expects)
         const uint32_t ls = pin(smem_u32(sLs) + (uint32_t)((colg * TILE_M + wrow0) * SLOTS * 4) + lane * 4);
@@ -342,16 +310,15 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
         const uint32_t qaddr = pin(smem_u32(sQ) + (uint32_t)(ew * 32 + lane) * 8);
         const uint32_t thr_row = pin(smem_u32(sThr + wrow0 + lane));  // + l * 128 * 8: the threads of this row, [NLIST]: peers
         const uint32_t my_thr = pin(thr_row + (uint32_t)colg * (TILE_M * 8));
-        const uint32_t tempty0 = pin(mapa_rank(bar_tempty, 0)), tempty1 = pin(mapa_rank(bar_tempty + 8, 0));  // the leader's copies
-        const uint32_t tfull0 = pin(bar_tfull), tfull1 = pin(bar_tfull + 8);
-        const uint32_t tbase = pin(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(colg * COLS));
+        const uint32_t stg_r = pin(smem_u32(sStg) + (uint32_t)((wrow0 + lane) * STG_STRIDE * 4));
+        const uint32_t qfull0 = pin(bar_qfull + (uint32_t)colg * 8), qempty = pin(bar_qempty);
         const bool lane0 = pin((uint32_t)lane) == 0;
         const uint32_t n_pos = (uint32_t)p.n_pos;
         const int kc = p.k_cand;  // (<= SLOTS, guaranteed by the host; a visible bound makes the compiler unroll the list scans fully and spill)
         const bool dbg_skip = p.debug_mode == 2;
         const bool peers = PEERS && p.n_peers > 0;
         const uint32_t other_thr = pin(thr_row + (uint32_t)(colg ^ 1) * (TILE_M * 8));  // two lists per row: the other one's slot
-        uint32_t buf = 0, tph = 0, work_tag = 0;  // accumulator buffer / its phase parity: tile_it & 1, (tile_it >> 1) & 1
+        uint32_t tpar = 0, work_tag = 0;  // parity of the quarter barriers (one phase per tile)
         for (int w = pair; w < n_work; w += n_pairs, ++work_tag) {
             const int split = w / p.n_row_tiles, rt = w - split * p.n_row_tiles;
             const int t0 = split * p.tiles_per_split;
@@ -377,7 +344,7 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
             sink.cap = p.cand_stride;
             sink.appending = false;
             auto cursors_at = [&](int tile) {  // (re)position the CSR / exclusion cursors at the first object of `tile`
-                const int64_t pos_first = (int64_t)tile * TILE_N + colg * COLS;
+                const int64_t pos_first = (int64_t)tile * TILE_N + colg * QUART_N;
                 const bool live = frow >= 0 && pos_first < p.n_pos;
                 const int g_first = live ? (p.pos2obj ? __ldg(p.pos2obj + pos_first) : (int)pos_first) + p.id_off : 0;
                 row_cursors_init(p, rs, live ? frow : -1, g_first);
@@ -390,7 +357,7 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
 #define B200_STEP() fifo_step<QN, QS, WIDE>(p, rs, cw, qaddr, head, tail, ls, li, kc, sink)
             cursors_at(ts);
             int t = ts;
-            uint32_t pos_t = (uint32_t)ts * TILE_N + (uint32_t)(colg * COLS);
+            uint32_t pos_t = (uint32_t)ts * TILE_N + (uint32_t)(colg * QUART_N);
             for (int it = 0; it < nt; ++it) {
                 // exchange thresholds with the threads that own the other column groups of this row and with the other
                 // ranks (monotone, racy by design: a stale value is only a weaker bound; the tag keeps a value of the
@@ -433,41 +400,19 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
                     }
                     sink.appending = true;
                 }
-                mbar_wait(buf ? tfull1 : tfull0, tph);
-                tc_fence_after();
                 // the last tile before the stream wraps around / of the work item: every pending hit must be handled
                 // before the cursors are repositioned or the list is written
                 const bool force = (t + 1 == t1);
                 const bool last = (it + 1 == nt);
-                if (!dbg_skip) {
-                    uint32_t r[COLS];
-                    tmem_ld_sync(tbase + buf * (uint32_t)TILE_N, r);
-                    tc_fence_before();
+#pragma unroll
+                for (int s = 0; s < NQ; ++s) {
+                    mbar_wait(qfull0 + (uint32_t)(s * NLIST * 8), tpar);
+                    uint32_t r[QUART_N];
+                    if (!dbg_skip) stage_ld(stg_r, r);
                     __syncwarp();
-                    if (lane0) mbar_arrive_cluster(buf ? tempty1 : tempty0);  // accumulator free again
-                    // (Measured and not kept: seeding the first tile's threshold with the K'-th largest group maximum -- the lists
-                    // are empty there and every column is a hit -- changed nothing at N = 1M and gained 1.3 % on a 125 K-object
-                    // shard, profiles/r02_ab_fused.txt.)
-                    if constexpr (COLS == 128) {
-                        const float m0 = chunk_max<0>(r), m1 = chunk_max<32>(r), m2 = chunk_max<64>(r), m3 = chunk_max<96>(r);
-                        const float mx = fmaxf(max3(m0, m1, m2), m3);
-                        if (__any_sync(B200_FULL_MASK, mx > rs.thr)) {
-                            const float thr = rs.thr;
-                            unsigned h0 = 0, h1 = 0, h2 = 0, h3 = 0;
-                            if (__any_sync(B200_FULL_MASK, m0 > thr)) h0 = chunk_hits<0>(r, thr);
-                            if (__any_sync(B200_FULL_MASK, m1 > thr)) h1 = chunk_hits<32>(r, thr);
-                            if (__any_sync(B200_FULL_MASK, m2 > thr)) h2 = chunk_hits<64>(r, thr);
-                            if (__any_sync(B200_FULL_MASK, m3 > thr)) h3 = chunk_hits<96>(r, thr);
-                            for (;;) {
-                                bool stuck = chunk_push<0, QN, QS>(r, h0, pos_t, rs.thr, n_pos, qaddr, head, tail);
-                                if (!stuck) stuck = chunk_push<32, QN, QS>(r, h1, pos_t, rs.thr, n_pos, qaddr, head, tail);
-                                if (!stuck) stuck = chunk_push<64, QN, QS>(r, h2, pos_t, rs.thr, n_pos, qaddr, head, tail);
-                                if (!stuck) stuck = chunk_push<96, QN, QS>(r, h3, pos_t, rs.thr, n_pos, qaddr, head, tail);
-                                if (!stuck) break;
-                                B200_STEP();  // dense phase: make room, then go on
-                            }
-                        }
-                    } else {
+                    if (lane0) mbar_arrive(qempty);  // staging buffer free again
+                    if (!dbg_skip) {
+                        const uint32_t pos_q = pos_t + (uint32_t)(s * NLIST * QUART_N);
                         const float m0 = chunk_max<0>(r), m1 = chunk_max<32>(r);
                         const float mx = fmaxf(m0, m1);
                         if (__any_sync(B200_FULL_MASK, mx > rs.thr)) {
@@ -476,16 +421,18 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
                             if (__any_sync(B200_FULL_MASK, m0 > thr)) h0 = chunk_hits<0>(r, thr);
                             if (__any_sync(B200_FULL_MASK, m1 > thr)) h1 = chunk_hits<32>(r, thr);
                             for (;;) {
-                                bool stuck = chunk_push<0, QN, QS>(r, h0, pos_t, rs.thr, n_pos, qaddr, head, tail);
-                                if (!stuck) stuck = chunk_push<32, QN, QS>(r, h1, pos_t, rs.thr, n_pos, qaddr, head, tail);
+                                bool stuck = chunk_push<0, QN, QS>(r, h0, pos_q, rs.thr, n_pos, qaddr, head, tail);
+                                if (!stuck) stuck = chunk_push<32, QN, QS>(r, h1, pos_q, rs.thr, n_pos, qaddr, head, tail);
                                 if (!stuck) break;
-                                B200_STEP();
+                                B200_STEP();  // dense phase: make room, then go on
                             }
                         }
                     }
-                    // deferred work: at most one step per tile (bounded latency in front of the next accumulator), by default
-                    // every PERIOD-th tile or as soon as some row has BACKLOG hits waiting (batching the steps measured +7 %),
-                    // except where everything pending has to be finished
+                }
+                if (!dbg_skip) {
+                    // deferred work: at most one step per tile (bounded latency in front of the next quarter), by default
+                    // every PERIOD-th tile or as soon as some row has BACKLOG hits waiting, except where everything pending
+                    // has to be finished
                     const bool due = (tail - head >= Cfg::BACKLOG) ||
                                      (head != tail && ((it & (Cfg::PERIOD - 1)) == Cfg::PERIOD - 1 || force || last));
                     if (__any_sync(B200_FULL_MASK, due)) {
@@ -493,18 +440,13 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
                         if (force || last)
                             while (__any_sync(B200_FULL_MASK, head != tail)) B200_STEP();
                     }
-                } else {
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane0) mbar_arrive_cluster(buf ? tempty1 : tempty0);
                 }
-                buf ^= 1;
-                tph ^= (buf == 0) ? 1u : 0u;
+                tpar ^= 1;
                 ++t;
                 pos_t += TILE_N;
                 if (t == t1 && !last) {  // wrapped around: objects ascend again from the split's first tile
                     t = t0;
-                    pos_t = (uint32_t)t0 * TILE_N + (uint32_t)(colg * COLS);
+                    pos_t = (uint32_t)t0 * TILE_N + (uint32_t)(colg * QUART_N);
                     cursors_at(t0);
                 }
             }
@@ -520,18 +462,61 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
                 p.cand_counts[lrow] = rs.cnt;
                 p.cand_thr[lrow] = rs.thr;
             }
-            // last work item of this pair: lets the helper warps leave their polling loop (kept INSIDE the loop: any code behind
-            // it made ptxas spill the staged accumulator, 1.5 KB of stack)
+            // last work item of this CTA: lets the helper warps leave their polling loop
             if (PEERS && peers && w + n_pairs >= n_work) sts_thr(my_thr, TAG_DONE, INFINITY);
         }
 #undef B200_STEP
-    }
-
-    tc_fence_before();
-    cluster_sync_all();  // no CTA may exit (or free TMEM) while its peer can still signal its barriers / read its smem
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc_2sm(tmem_base, TMEM_COLS);
+    } else if (PEERS && p.n_peers > 0) {
+        // ===================================================================== peer-threshold helpers (two warps)
+        // Thread h serves CTA-local rows h and h + 64.  Per round and row: read the row's own thresholds from the exchange
+        // slots, publish their maximum to this rank's global array, read the other ranks' published values (NVLink peer
+        // loads, latency irrelevant here), leave their maximum in the row's extra exchange slot.  All values are monotone
+        // lower bounds of the row's final threshold: a stale one is only weaker, never wrong.
+        const int h = (warp - Cfg::EPI0 - NW) * 32 + lane;
+        float published[2] = {-INFINITY, -INFINITY};
+        uint32_t pub_tag[2] = {0xffffffffu, 0xffffffffu};
+        bool done[2] = {false, false};
+        while (!(done[0] && done[1])) {
+#pragma unroll
+            for (int s = 0; s < 2; ++s) {
+                const int r = h + 64 * s;
+                uint32_t tag;
+                float own;
+                lds_thr(smem_u32(sThr + r), tag, own);
+                done[s] = tag == TAG_DONE;  // the row's first column group has finished its last work item
+                if (tag >= TAG_DONE) continue;
+#pragma unroll
+                for (int l = 1; l < NLIST; ++l) {
+                    uint32_t tl;
+                    float vl;
+                    lds_thr(smem_u32(sThr + l * TILE_M + r), tl, vl);
+                    if (tl == tag) own = fmaxf(own, vl);
+                }
+                const int w = pair + (int)tag * n_pairs;
+                if (w >= n_work) continue;
+                const int rt = w % p.n_row_tiles;
+                const int64_t grow = ((int64_t)rt * 2 + rank) * TILE_M + r;
+                if (grow >= p.n_rows) continue;
+                if (pub_tag[s] != tag) {
+                    pub_tag[s] = tag;
+                    published[s] = -INFINITY;
+                }
+                if (own > published[s] && own < INFINITY) {
+                    published[s] = own;
+                    stg_peer(p.peer_pub + p.peer_row0 + grow, p.peer_epoch, ldexpf(own, -p.peer_exp));
+                }
+                // all peer loads in flight at once: one NVLink round trip per row and round
+                unsigned long long v[MAX_PEERS];
+#pragma unroll
+                for (int q = 0; q < MAX_PEERS; ++q) v[q] = q < p.n_peers ? ldg_peer(p.peer_in[q] + p.peer_row0 + grow) : 0ull;
+                float best = -INFINITY;
+#pragma unroll
+                for (int q = 0; q < MAX_PEERS; ++q)
+                    if (q < p.n_peers && (uint32_t)(v[q] >> 32) == p.peer_epoch) best = fmaxf(best, __uint_as_float((uint32_t)v[q]));
+                if (best > -INFINITY) sts_thr(smem_u32(sThr + NLIST * TILE_M + r), tag, ldexpf(best, p.peer_exp));
+            }
+            __nanosleep(200);
+        }
     }
 }
 

@@ -1,5 +1,5 @@
-// sm_100a building blocks of the fused scoring + candidate-selection kernel (fused_topk.cuh): tcgen05 / TMEM / TMA /
-// mbarrier / cluster PTX wrappers, the kernel parameter block, and the per-row selection state of the epilogue
+// sm_90a building blocks of the fused scoring + candidate-selection kernel (fused_topk.cuh): wgmma / TMA / mbarrier
+// PTX wrappers, the kernel parameter block, and the per-row selection state of the epilogue
 // (candidate lists in shared memory, filter_pairs_csr merge cursor, exclusion cursor, register-chunk helpers).
 //
 // The code built from these pieces replaces `scores = query @ items.T` + mask + select of implicit's top-k (call site
@@ -14,19 +14,22 @@
 namespace b200 {
 namespace tc {
 
-constexpr int TILE_M = 128;                // subject rows per CTA = TMEM lanes
-constexpr int TILE_N = 256;                // objects per tile of a CTA pair (each CTA loads 128 of them)
-constexpr int HALF_N = 128;                // object rows per CTA and tile
+constexpr int TILE_M = 128;                // subject rows per CTA
+constexpr int TILE_N = 256;                // objects per tile (scored in four quarters of QUART_N)
+constexpr int QUART_N = 64;                // objects per MMA pass, object block and accumulator staging
+constexpr int HALF_N = 128;                // object rows the resident 16-bit copy is padded to
 constexpr int KBLK = 64;                   // 16-bit elements per shared-memory block row (128 B, one swizzle atom)
-constexpr int BLK_BYTES = 128 * KBLK * 2;  // 16 KiB: [128 rows][128 B]
-constexpr int MAX_STAGES = 12;
-constexpr int TMEM_COLS = 512;
+constexpr int BLK_BYTES = 128 * KBLK * 2;  // 16 KiB: [128 subject rows][128 B]
+constexpr int OBJ_BLK_BYTES = QUART_N * KBLK * 2;  // 8 KiB: [64 object rows][128 B], one ring stage
+constexpr int STG_STRIDE = QUART_N + 4;    // floats per staged accumulator row (+4: conflict-free 16-byte row reads)
+constexpr int STG_BYTES = TILE_M * STG_STRIDE * 4;
+constexpr int MAX_STAGES = 16;
 constexpr int SMEM_LIMIT = 232448;  // 227 KiB
 constexpr int MAX_PEERS = 8;        // ranks sharing pruning thresholds over NVLink peer memory (multi-GPU item sharding)
 
 struct TcParams {
     int32_t kblocks;          // d_pad / 64
-    int32_t n_stages;         // object ring depth (blocks of 16 KiB)
+    int32_t n_stages;         // object ring depth (blocks of 8 KiB)
     int32_t k_cand;           // K': slots used per candidate list (<= the kernel's list capacity)
     int64_t n_rows;           // valid subject rows
     int64_t n_pos;            // valid object positions
@@ -34,7 +37,6 @@ struct TcParams {
     int32_t n_splits;
     int32_t n_obj_tiles;
     int32_t tiles_per_split;
-    uint32_t idesc;           // UMMA instruction descriptor
     const int32_t* pos2obj;   // nullable whitelist map
     const int64_t* indptr;    // nullable CSR filter by subject row
     const int32_t* indices;
@@ -52,9 +54,9 @@ struct TcParams {
     // wide mode (k > 24): the first `phase1_tiles` tiles of a work item keep adaptive K'-slot lists; then the threshold is
     // frozen and every later score above it is appended to the global list (no more list maintenance)
     int32_t phase1_tiles;     // >= tiles of a work item: never switch (plain adaptive lists)
-    int32_t debug_mode;       // 0 = normal; 1 = no candidates (fast path only); 2 = epilogue skips the TMEM reads (measurement hooks)
+    int32_t debug_mode;       // 0 = normal; 1 = no candidates (fast path only); 2 = epilogue skips the staged-accumulator reads (measurement hooks)
     // carousel: a work item starts streaming the objects where the other CTA pairs currently are, so that all pairs keep
-    // reading the same few MB of the object matrix and the L2 serves 73 of 74 reads (nullptr: start at t0)
+    // reading the same few MB of the object matrix and the L2 serves most reads (nullptr: start at t0)
     int32_t* front;           // [n_splits] object tile most recently issued by the reference pair
     int32_t* starts;          // [n_pairs][starts_stride] start tile chosen for each work item (-1: not decided yet)
     int32_t starts_stride;
@@ -97,125 +99,75 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity))
         if (++spins > (1u << 24)) __trap();
 }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
 }
-// One lane of the (converged) warp; the same lane every time, so tcgen05.commit tracks the MMAs it issued.
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// 2-SM TMA load: data lands in THIS CTA's shared memory, the byte count is credited to the LEADER CTA's mbarrier
-// (shared::cta addresses carry the CTA-pair rank in bit 24; clearing it names the even CTA's copy of the barrier).
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t slot_smem, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slot_smem), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[both CTAs' smem, 128 rows each] * B[both CTAs' smem, 128 rows each]^T : 256 x 256 x 16.
-// The two shared-memory matrix descriptors differ only in their low word (start address >> 4).
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t desc_hi, uint32_t idesc,
-                                             uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %3};\n\t"
-        "mov.b64 db, {%2, %3};\n\t"
-        "setp.ne.b32 p, %5, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %4, p;\n\t}"
-        ::"r"(tmem_d), "r"(a_lo), "r"(b_lo), "r"(desc_hi), "r"(idesc), "r"(accum)
-        : "memory");
-}
-// Arrive (once the MMAs issued so far have retired) on the mbarrier at this offset in BOTH CTAs of the pair.
-__device__ __forceinline__ void umma_commit_2sm(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(bar), "h"((uint16_t)3)
-                 : "memory");
-}
-
-// Synchronous wide TMEM reads (load + wait in one asm statement so that no use can be scheduled in between):
-// thread i of the warp gets TMEM lane (base_lane + i), 64 / 128 consecutive fp32 columns.
-#define B200_R8(a, n) "=r"(a[n]), "=r"(a[n + 1]), "=r"(a[n + 2]), "=r"(a[n + 3]), "=r"(a[n + 4]), "=r"(a[n + 5]), "=r"(a[n + 6]), "=r"(a[n + 7])
-__device__ __forceinline__ void tmem_ld_sync(uint32_t taddr, uint32_t (&r)[64]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x64.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, [%64];\n\t"
-        "tcgen05.wait::ld.sync.aligned;"
-        : B200_R8(r, 0), B200_R8(r, 8), B200_R8(r, 16), B200_R8(r, 24), B200_R8(r, 32), B200_R8(r, 40), B200_R8(r, 48),
-          B200_R8(r, 56)
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_sync(uint32_t taddr, uint32_t (&r)[128]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x128.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, [%128];\n\t"
-        "tcgen05.wait::ld.sync.aligned;"
-        : B200_R8(r, 0), B200_R8(r, 8), B200_R8(r, 16), B200_R8(r, 24), B200_R8(r, 32), B200_R8(r, 40), B200_R8(r, 48),
-          B200_R8(r, 56), B200_R8(r, 64), B200_R8(r, 72), B200_R8(r, 80), B200_R8(r, 88), B200_R8(r, 96), B200_R8(r, 104),
-          B200_R8(r, 112), B200_R8(r, 120)
-        : "r"(taddr)
+        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1)
         : "memory");
 }
 
 // Shared-memory matrix descriptor of a K-major operand block: 128-byte rows, SWIZZLE_128B, 8-row groups 1024 B apart.
-//   lo: bits [0,14) start address >> 4, bits [16,30) leading byte offset >> 4 (unused for swizzled K-major: 0)
-//   hi: bits [0,14) stride byte offset >> 4 (1024 >> 4), bits [14,16) descriptor version 1 (sm_100), bits [29,32) layout 2
-__device__ __forceinline__ uint32_t smem_desc_lo(uint32_t saddr) { return (saddr & 0x3FFFF) >> 4; }
-constexpr uint32_t SMEM_DESC_HI = (1024u >> 4) | (1u << 14) | (2u << 29);
+//   lo: bits [0,14) start address >> 4, bits [16,30) leading byte offset >> 4 (ignored for swizzled K-major: 1)
+//   hi: bits [0,14) stride byte offset >> 4 (1024 >> 4), bits [30,32) layout 1 (128-byte swizzle)
+__device__ __forceinline__ uint32_t smem_desc_lo(uint32_t saddr) { return ((saddr & 0x3FFFF) >> 4) | (1u << 16); }
+constexpr uint32_t SMEM_DESC_HI = (1024u >> 4) | (1u << 30);
 
+// Barrier of the 128 threads of the MMA warp group only (named barrier 1; barrier 0 is __syncthreads).
+__device__ __forceinline__ void mma_group_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// Pin the accumulator registers at this point of the instruction stream: without it the compiler may copy an
+// accumulator while its wgmma is still in flight and feed the stale copy to the next wgmma or to a store.
 template <int N>
-__device__ __forceinline__ void reg_dealloc() {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+__device__ __forceinline__ void fence_acc(float (&r)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
 template <int N>
-__device__ __forceinline__ void reg_alloc() {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, both operands K-major in shared memory, fp32 accumulators in registers
+// (warp w of the warp group, lane l holds rows 16 w + l / 4 (+ 8) and columns 8 j + 2 (l % 4) (+ 1) of D).
+#define B200_F8(a, n) "+f"(a[n]), "+f"(a[n + 1]), "+f"(a[n + 2]), "+f"(a[n + 3]), "+f"(a[n + 4]), "+f"(a[n + 5]), "+f"(a[n + 6]), "+f"(a[n + 7])
+#define B200_WGMMA_64x64(TYPE)                                                                                              \
+    asm volatile(                                                                                                           \
+        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"                                                                       \
+        "mov.b64 da, {%32, %34};\n\t"                                                                                       \
+        "mov.b64 db, {%33, %34};\n\t"                                                                                       \
+        "setp.ne.b32 p, %35, 0;\n\t"                                                                                        \
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32." TYPE "." TYPE " "                                                     \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                           \
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, da, db, p, 1, 1, 0, 0;\n\t}"     \
+        : B200_F8(d, 0), B200_F8(d, 8), B200_F8(d, 16), B200_F8(d, 24)                                                      \
+        : "r"(a_lo), "r"(b_lo), "r"(SMEM_DESC_HI), "r"(accum))
+// (the operand type is a template parameter: a run-time branch around each wgmma makes ptxas serialise the pipeline)
+template <bool BF16>
+__device__ __forceinline__ void wgmma_64x64(float (&d)[32], uint32_t a_lo, uint32_t b_lo, uint32_t accum) {
+    if constexpr (BF16)
+        B200_WGMMA_64x64("bf16");
+    else
+        B200_WGMMA_64x64("f16");
+}
+#undef B200_WGMMA_64x64
+#undef B200_F8
+
+// One epilogue thread's row of a staged accumulator quarter: 64 fp32 columns, 16-byte loads.
+__device__ __forceinline__ void stage_ld(uint32_t a, uint32_t (&r)[64]) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
+                     : "=r"(r[4 * j]), "=r"(r[4 * j + 1]), "=r"(r[4 * j + 2]), "=r"(r[4 * j + 3])
+                     : "r"(a + 16 * j)
+                     : "memory");
 }
 
 __device__ __forceinline__ float max3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
@@ -435,8 +387,8 @@ __device__ __forceinline__ float chunk_select(const uint32_t (&r)[NR], int j) {
     return fu(b4 ? d[1] : d[0]);
 }
 
-// Start tile of a work item: decided once by the leader CTA's producer thread (the current front of its object split),
-// published through global memory, read by every other role of both CTAs.
+// Start tile of a work item: decided once by the even CTA's load-issuing thread (the current front of its object split),
+// published through global memory, read by every other role of both CTAs of the pair.
 __device__ __forceinline__ int carousel_start(const TcParams& p, int pair, uint32_t work_it, int split, int t0, int t1, bool decide) {
     if (p.front == nullptr) return t0;
     volatile int32_t* slot = p.starts + (size_t)pair * p.starts_stride + work_it;

@@ -4,7 +4,7 @@ Mirrors `rectools.models.rank.ImplicitRanker` (rectools/models/rank/rank_implici
 meaning `(distance, subjects_factors, objects_factors, ...)`, same `rank(subject_ids, k, filter_pairs_csr,
 sorted_object_whitelist)` signature, return triplet and error behaviour -- with the native top-k call
 (rank_implicit.py:264-272 / :175-182) and the per-user Python post-loop (:120-146) replaced by one C-ABI call plus
-vectorised numpy.  There is no CPU fallback: construction fails if the CUDA library or an sm_100 device is missing.
+vectorised numpy.  There is no CPU fallback: construction fails if the CUDA library or an sm_90 device is missing.
 """
 from __future__ import annotations
 

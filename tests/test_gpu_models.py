@@ -1,4 +1,4 @@
-"""GPU: the UNMODIFIED reference models with the real B200 engine under them (SURVEY 8 rows a9 / a11 / a13 / f3 / f4).
+"""GPU: the UNMODIFIED reference models with the real CUDA engine under them (SURVEY 8 rows a9 / a11 / a13 / f3 / f4).
 
 `oracle/_ref` holds the reference package as staged by `__graft_entry__.build()` (git-ignored; it travels to the GPU box
 like the built `.so`), `oracle/implicit_stub` stands in for the third-party `implicit` (its top-k = the CPU oracle).  Every

@@ -1,7 +1,7 @@
 """CPU: the `implicit.gpu` stand-ins (`rectools_b200/implicit_gpu.py`, the lowest seam of SURVEY section 8b) make the UNMODIFIED
 reference `ImplicitRanker(..., use_gpu=True)` (rank_implicit.py:148-185, :250-262) produce the same triplets as its CPU path.
-The top-k provider behind `KnnQuery.topk` is the oracle here (injected); on a B200 it is the engine (tests/test_gpu_parity.py).
-Needs the reference checkout (build container only; skipped on the GPU box)."""
+The top-k provider behind `KnnQuery.topk` is the oracle here (injected); on an H100 it is the engine (tests/test_gpu_parity.py).
+Needs the reference package (staged in oracle/_ref or a checkout found by oracle/stage_reference.py); skipped without it."""
 import os
 import sys
 
@@ -9,10 +9,12 @@ import numpy as np
 import pytest
 from scipy import sparse
 
-REF = "/root/reference"
+from oracle import stage_reference
+
+REF = stage_reference.reference_root()
 STUB = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "oracle", "implicit_stub")
 
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "rectools")), reason="reference checkout not present")
+pytestmark = pytest.mark.skipif(REF is None, reason="reference package neither staged nor checked out")
 
 
 def _oracle_backend(items, queries, k, item_norms, csr):

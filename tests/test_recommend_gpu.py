@@ -1,4 +1,4 @@
-"""GPU: `rectools_b200.recommend()` (vectorised `ModelBase.recommend`, SURVEY section 8f rank 1) with the real B200 ranker on
+"""GPU: `rectools_b200.recommend()` (vectorised `ModelBase.recommend`, SURVEY section 8f rank 1) with the real CUDA ranker on
 BASELINE config 1 -- the factors and the recommendations of the reference's `PureSVDModel(factors=32).recommend(K=10,
 filter_viewed=True)` on the 6040 x 3706 synthetic interactions (tests/golden/puresvd_c1.npz, made by oracle/make_golden.py).
 rectools itself is not on the GPU box: the dataset / model are the duck-typed stand-ins of tests/helpers.py."""
