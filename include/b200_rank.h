@@ -48,7 +48,7 @@
 extern "C" {
 #endif
 
-#define B200_RANK_ABI_VERSION 3
+#define B200_RANK_ABI_VERSION 4
 
 /* error codes */
 #define B200_OK 0
@@ -63,7 +63,9 @@ extern "C" {
 #define B200_DIST_COSINE 1
 
 /* tensor-core candidate pass */
-#define B200_TC_AUTO 0 /* fp16 (power-of-two scaled) when the factors fit its range, else bf16 */
+#define B200_TC_AUTO 0 /* bf16 for bf16 object factors (the copy is exact), else fp16.  Both types are power-of-two scaled
+                        * per subject row and by one global exponent for the objects; objects far below the largest one
+                        * may round to fp16 subnormals or zero, which the certificate's bound covers */
 #define B200_TC_FP16 1
 #define B200_TC_BF16 2
 #define B200_TC_OFF 3 /* exhaustive fp64 kernel only */
@@ -202,6 +204,50 @@ int b200_rank_merge_certified(int32_t device, void* stream, int32_t n_lists, int
  *           engine's own and is skipped).  At most 9 ranks. */
 int b200_rank_peer_export(b200_rank_engine* engine, int64_t max_rows, void* handle_out);
 int b200_rank_peer_import(b200_rank_engine* engine, int32_t n_ranks, int32_t self, const void* handles);
+
+/* ---- test interface (ABI 4): one tensor-core candidate pass, as the fused kernel left it.
+ * With the environment variable B200_TC_SNAPSHOT=n set, a ranking call copies (device to device, on the engine stream)
+ * the state of the n-th launch of the fused kernel of that call into engine-owned buffers.  Launches are counted like
+ * b200_rank_stats.n_tc_launches: 1 = the main pass, higher = the second-chance and re-rank passes.  A call with more
+ * than one row chunk counts one main-pass launch per chunk, so n = 1 snapshots the first chunk.  Unset (or 0), nothing
+ * is copied and nothing is allocated.  The state of a pass:
+ *   cand_scores / cand_ids  [n_lists][rows_pad][cand_stride]  approximate scores (units of 2^(row_exp + obj_exp)) and
+ *                           LOCAL object ids; list l = split * (nw / 4) + column group; entries beyond the count unused
+ *   cand_counts / cand_thr  [n_lists][rows_pad]  entries produced (wide mode: > cand_stride = overflow) and the list's
+ *                           final pruning threshold
+ *   row_exp                 [rows_pad]  power-of-two exponent of each subject row (batch order of the pass)
+ *   rows                    [n_sel]     the call's row number of each batch row of the pass
+ *   fb_rows                 [n_fb]      the call's rows that this pass's re-score sent to the fallback
+ * b200_rank_get_snapshot returns the last call's metadata (valid = 0: nothing was captured) and fills every array
+ * argument that is non-NULL, so a first call with NULL arrays asks for the sizes. */
+typedef struct b200_rank_snapshot {
+    int32_t valid;
+    int32_t launch;          /* n of B200_TC_SNAPSHOT */
+    int32_t nw;              /* epilogue warps of the pass (8 or 16): nw / 4 candidate lists per row and object split */
+    int32_t n_lists;         /* n_splits * nw / 4 */
+    int32_t n_splits;        /* object splits: split s streams tiles [s * tiles_per_split, (s + 1) * tiles_per_split) */
+    int32_t tiles_per_split;
+    int32_t n_obj_tiles;     /* tiles of 256 object positions */
+    int32_t cand_stride;     /* slots per list */
+    int64_t n_pos;           /* object positions (whitelist entries, or objects) */
+    int64_t rows_pad;        /* rows between consecutive lists */
+    int64_t n_sel;           /* subject rows of the pass */
+    int32_t k_out;
+    int32_t k_cand;          /* K': slots a list keeps while it is adaptive */
+    int32_t k0;              /* the pass produces output entries [k0, k0 + kp); ids of entries < k0 are excluded */
+    int32_t kp;
+    int32_t wide;            /* 1: lists stop adapting after phase1_tiles tiles and append everything above the threshold */
+    int32_t phase1_tiles;
+    int32_t bf16;            /* operand type: 1 bf16, 0 fp16 */
+    int32_t obj_exp;         /* power-of-two exponent applied to every object */
+    float eps_rel;           /* certificate: |approx - exact| <= eps_rel * |u|_2 * max_obj_norm */
+    float max_obj_norm;
+    int32_t id_off;          /* global id = local id + id_off */
+    int32_t n_fb;
+} b200_rank_snapshot;
+
+int b200_rank_get_snapshot(b200_rank_engine* engine, b200_rank_snapshot* meta, float* cand_scores, int32_t* cand_ids,
+                           int32_t* cand_counts, float* cand_thr, int32_t* row_exp, int32_t* rows, int32_t* fb_rows);
 
 const char* b200_rank_last_error(void);
 int b200_rank_abi_version(void);

@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200_RANK_LIB") or os.path.join(HERE, "libb200rank.so")
 
 # mirrors of the #defines in include/b200_rank.h
-ABI_VERSION = 3
+ABI_VERSION = 4
 OK, E_INVALID, E_CUDA, E_NOMEM, E_UNSUPPORTED = 0, -1, -2, -3, -4
 DIST_DOT, DIST_COSINE = 0, 1
 TC_AUTO, TC_FP16, TC_BF16, TC_OFF = 0, 1, 2, 3
@@ -30,6 +30,7 @@ EXPORTS = (
     "b200_rank_merge_certified",
     "b200_rank_peer_export",
     "b200_rank_peer_import",
+    "b200_rank_get_snapshot",
     "b200_rank_last_error",
     "b200_rank_abi_version",
 )
@@ -105,6 +106,36 @@ class Info(C.Structure):
     ]
 
 
+class Snapshot(C.Structure):
+    """`b200_rank_snapshot`: metadata of the tensor-core pass captured with B200_TC_SNAPSHOT (test interface)."""
+
+    _fields_ = [
+        ("valid", C.c_int32),
+        ("launch", C.c_int32),
+        ("nw", C.c_int32),
+        ("n_lists", C.c_int32),
+        ("n_splits", C.c_int32),
+        ("tiles_per_split", C.c_int32),
+        ("n_obj_tiles", C.c_int32),
+        ("cand_stride", C.c_int32),
+        ("n_pos", C.c_int64),
+        ("rows_pad", C.c_int64),
+        ("n_sel", C.c_int64),
+        ("k_out", C.c_int32),
+        ("k_cand", C.c_int32),
+        ("k0", C.c_int32),
+        ("kp", C.c_int32),
+        ("wide", C.c_int32),
+        ("phase1_tiles", C.c_int32),
+        ("bf16", C.c_int32),
+        ("obj_exp", C.c_int32),
+        ("eps_rel", C.c_float),
+        ("max_obj_norm", C.c_float),
+        ("id_off", C.c_int32),
+        ("n_fb", C.c_int32),
+    ]
+
+
 class B200RankError(RuntimeError):
     """CUDA / driver failure inside libb200rank.so."""
 
@@ -146,6 +177,8 @@ def load() -> C.CDLL:
     lib.b200_rank_peer_export.argtypes = [vp, i64, vp]
     lib.b200_rank_peer_import.restype = C.c_int
     lib.b200_rank_peer_import.argtypes = [vp, i32, i32, vp]
+    lib.b200_rank_get_snapshot.restype = C.c_int
+    lib.b200_rank_get_snapshot.argtypes = [vp, C.POINTER(Snapshot), vp, vp, vp, vp, vp, vp, vp]
     lib.b200_rank_last_error.restype = C.c_char_p
     lib.b200_rank_last_error.argtypes = []
     lib.b200_rank_abi_version.restype = C.c_int

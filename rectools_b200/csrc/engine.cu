@@ -160,10 +160,18 @@ struct b200_rank_engine {
     int32_t* h_pinned = nullptr;  // small pinned scratch (counters)
     std::vector<char> h_patch;    // host copy of re-ranked rows (host-output calls)
 
+    // B200_TC_SNAPSHOT test hook: one fused-kernel pass of the last call (b200_rank_get_snapshot)
+    DevBuf snap_scores, snap_ids, snap_counts, snap_thr, snap_row_exp, snap_rows;
+    DevBuf snap_fb;  // [failure counter before the pass, after it, the pass's failure list (n_rows entries)]
+    b200_rank_snapshot snap{};
+    int64_t snap_row0 = 0;  // rows of a pass without a row list: snap_row0 + batch row
+    bool snap_has_rows = false;
+
     std::vector<DevBuf*> all_bufs() {
         return {&obj32, &obj16, &obj_norms, &objT, &sub32_res, &peer_pub, &sub32, &sub16, &row_exp, &rowmap, &indptr, &indices, &wl,
                 &obj16_wl, &sp_indptr, &sp_indices, &sp_data, &sp_scores, &out_ids, &out_scores, &out_counts, &out_bounds, &cand_scores,
-                &cand_ids, &cand_counts, &cand_thr, &part_scores, &part_ids, &fb_rows, &scratch, &excl, &carousel, &patch};
+                &cand_ids, &cand_counts, &cand_thr, &part_scores, &part_ids, &fb_rows, &scratch, &excl, &carousel, &patch,
+                &snap_scores, &snap_ids, &snap_counts, &snap_thr, &snap_row_exp, &snap_rows, &snap_fb};
     }
     size_t hbm_bytes() {
         size_t t = 0;
@@ -221,17 +229,17 @@ void prepare_objects(b200_rank_engine* E, int tc_mode) {
         return;
     }
     E->tc_dtype = (tc_mode == B200_TC_BF16) ? B200_TC_BF16 : B200_TC_FP16;
-    E->obj_exp = (E->tc_dtype == B200_TC_FP16) ? fp16_scale_exp(absmax) : 0;
+    E->obj_exp = fp16_scale_exp(absmax);  // power-of-two scaling is exact in both types: a bf16 copy of bf16 factors stays exact
     E->n_obj_pad = round_up(std::max<int64_t>(n, 1), tc::HALF_N);
     E->obj16.ensure((size_t)E->n_obj_pad * E->d_pad * 2);
     const float* norms = cosine ? E->obj_norms.as<float>() : nullptr;
     const int grid = grid_for(E->n_obj_pad * 32, 256);
     if (E->tc_dtype == B200_TC_FP16)
         convert_rows_kernel<__half, false><<<grid, 256, 0, E->st>>>(E->obj32_ptr, nullptr, nullptr, n, E->n_obj_pad, d, E->d_pad, norms,
-                                                                    E->obj_exp, 1, E->obj16.as<__half>(), nullptr);
+                                                                    E->obj_exp, E->obj16.as<__half>(), nullptr);
     else
         convert_rows_kernel<__nv_bfloat16, false><<<grid, 256, 0, E->st>>>(E->obj32_ptr, nullptr, nullptr, n, E->n_obj_pad, d, E->d_pad,
-                                                                           norms, 0, 0, E->obj16.as<__nv_bfloat16>(), nullptr);
+                                                                           norms, E->obj_exp, E->obj16.as<__nv_bfloat16>(), nullptr);
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(E->st));
 }
@@ -367,6 +375,8 @@ struct Call {
     bool wl_gathered = false;
     bool bf16 = false;
     int nw = 8;  // epilogue warps of the main pass
+    int n_tc = 0;       // fused-kernel launches so far
+    int snap_at = 0;    // B200_TC_SNAPSHOT: the launch whose state is copied (0: none)
     size_t n_evt = 0;
     std::vector<int> evt_kind;  // 0 = fused kernel, 1 = selection
 
@@ -485,6 +495,53 @@ struct TcPass {
     bool main = false;          // reported in the statistics as the main pass
 };
 
+// B200_TC_SNAPSHOT: copy the state the fused kernel and the re-score of this pass left behind (after both launches,
+// before the next pass reuses the buffers).  The failure counter was saved before the pass (snap_fb[0]).
+void take_snapshot(Call& c, const TcPass& t, const tc::TcParams& tp, int nw, float eps_rel) {
+    b200_rank_engine* E = c.E;
+    const int n_lists = tp.n_splits * (nw / 4);
+    const size_t n_lr = (size_t)n_lists * tp.rows_pad, n_cand = n_lr * tp.cand_stride;
+    auto d2d = [&](DevBuf& dst, const void* src, size_t bytes) {
+        dst.ensure(std::max<size_t>(bytes, 16));
+        if (bytes) CK(cudaMemcpyAsync(dst.p, src, bytes, cudaMemcpyDeviceToDevice, c.st));
+    };
+    d2d(E->snap_scores, tp.cand_scores, sizeof(float) * n_cand);
+    d2d(E->snap_ids, tp.cand_ids, sizeof(int32_t) * n_cand);
+    d2d(E->snap_counts, tp.cand_counts, sizeof(int32_t) * n_lr);
+    d2d(E->snap_thr, tp.cand_thr, sizeof(float) * n_lr);
+    d2d(E->snap_row_exp, E->row_exp.p, sizeof(int32_t) * tp.rows_pad);
+    if (t.rows_dev) d2d(E->snap_rows, t.rows_dev, sizeof(int32_t) * t.n_sel);
+    int32_t* fb = E->snap_fb.as<int32_t>();
+    CK(cudaMemcpyAsync(fb + 1, t.fb_count, sizeof(int32_t), cudaMemcpyDeviceToDevice, c.st));
+    CK(cudaMemcpyAsync(fb + 2, t.fb_list, sizeof(int32_t) * c.n_rows, cudaMemcpyDeviceToDevice, c.st));
+    E->snap_row0 = t.row0;
+    E->snap_has_rows = t.rows_dev != nullptr;
+    b200_rank_snapshot& m = E->snap;
+    m = b200_rank_snapshot{};
+    m.valid = 1;
+    m.launch = c.n_tc;
+    m.nw = nw;
+    m.n_lists = n_lists;
+    m.n_splits = tp.n_splits;
+    m.tiles_per_split = tp.tiles_per_split;
+    m.n_obj_tiles = tp.n_obj_tiles;
+    m.cand_stride = tp.cand_stride;
+    m.n_pos = tp.n_pos;
+    m.rows_pad = tp.rows_pad;
+    m.n_sel = t.n_sel;
+    m.k_out = c.k_out;
+    m.k_cand = tp.k_cand;
+    m.k0 = t.k0;
+    m.kp = t.kp;
+    m.wide = t.wide ? 1 : 0;
+    m.phase1_tiles = tp.phase1_tiles;
+    m.bf16 = c.bf16 ? 1 : 0;
+    m.obj_exp = E->obj_exp;
+    m.eps_rel = eps_rel;
+    m.max_obj_norm = E->max_obj_norm;
+    m.id_off = tp.id_off;
+}
+
 // One tensor-core candidate pass + fp64 re-score + certificate.  Rows whose certificate fails are appended to `fb_list`.
 void run_tc(Call& c, const TcPass& t) {
     b200_rank_engine* E = c.E;
@@ -501,11 +558,11 @@ void run_tc(Call& c, const TcPass& t) {
     {
         const int grid = grid_for(rows_pad * 32, 256);
         if (!bf16)
-            convert_rows_kernel<__half, true><<<grid, 256, 0, st>>>(t.sub32, t.rowmap, t.rows_dev, t.n_sel, rows_pad, d, E->d_pad, nullptr, 0, 1,
+            convert_rows_kernel<__half, true><<<grid, 256, 0, st>>>(t.sub32, t.rowmap, t.rows_dev, t.n_sel, rows_pad, d, E->d_pad, nullptr, 0,
                                                                     E->sub16.as<__half>(), E->row_exp.as<int32_t>());
         else
             convert_rows_kernel<__nv_bfloat16, true><<<grid, 256, 0, st>>>(t.sub32, t.rowmap, t.rows_dev, t.n_sel, rows_pad, d, E->d_pad, nullptr,
-                                                                           0, 0, E->sub16.as<__nv_bfloat16>(), E->row_exp.as<int32_t>());
+                                                                           0, E->sub16.as<__nv_bfloat16>(), E->row_exp.as<int32_t>());
         CK(cudaGetLastError());
         c.S.n_launches++;
     }
@@ -621,6 +678,11 @@ void run_tc(Call& c, const TcPass& t) {
         tp.starts_stride = per_pair;
     }
     const int grid = 2 * std::min(n_work, n_units);
+    const bool snap = ++c.n_tc == c.snap_at;
+    if (snap) {
+        E->snap_fb.ensure(sizeof(int32_t) * (size_t)(c.n_rows + 2));
+        CK(cudaMemcpyAsync(E->snap_fb.p, t.fb_count, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    }
     c.time_begin(0);
     const bool use_peers = t.peers && tp.n_peers > 0;  // (wide mode and threshold sharing never meet: sharing needs k <= 24)
 #define B200_LAUNCH(NW_, WIDE_, PEERS_)                                                                                              \
@@ -687,6 +749,7 @@ void run_tc(Call& c, const TcPass& t) {
     CK(cudaGetLastError());
     c.time_end();
     c.S.n_launches++;
+    if (snap) take_snapshot(c, t, tp, t.nw, sp.eps_rel);
 }
 
 // Sparse subjects (EASE): SpMM score rows for bounded row chunks + streaming top-k (sparse.cuh).
@@ -911,6 +974,8 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
     c.E = E;
     c.q = q;
     memset(&c.S, 0, sizeof(c.S));
+    c.snap_at = env_int("B200_TC_SNAPSHOT", 0);  // test hook, see b200_rank_get_snapshot
+    E->snap.valid = 0;
     b200_rank_stats& S = c.S;
     const int64_t n_rows = q->n_rows;
     const int64_t n_pos = q->whitelist ? q->n_whitelist : E->n_obj;
@@ -1357,6 +1422,44 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
                     ce.line, cudaGetErrorString(ce.e));
     }
     if (stats) *stats = c.S;
+    return B200_OK;
+}
+
+int b200_rank_get_snapshot(b200_rank_engine* E, b200_rank_snapshot* meta, float* cand_scores, int32_t* cand_ids, int32_t* cand_counts,
+                           float* cand_thr, int32_t* row_exp, int32_t* rows, int32_t* fb_rows) {
+    if (!E || !meta) return fail(B200_E_INVALID, "b200_rank_get_snapshot: NULL argument");
+    std::lock_guard<std::mutex> lock(E->mu);
+    *meta = E->snap;
+    if (!E->snap.valid) return B200_OK;
+    try {
+        CK(cudaSetDevice(E->device));
+        const b200_rank_snapshot& m = E->snap;
+        cudaStream_t st = E->st;
+        int32_t cnt[2];
+        CK(cudaMemcpyAsync(cnt, E->snap_fb.p, sizeof(cnt), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        meta->n_fb = cnt[1] - cnt[0];
+        const size_t n_lr = (size_t)m.n_lists * m.rows_pad, n_cand = n_lr * m.cand_stride;
+        auto d2h = [&](void* dst, const DevBuf& src, size_t bytes) {
+            if (dst && bytes) CK(cudaMemcpyAsync(dst, src.p, bytes, cudaMemcpyDeviceToHost, st));
+        };
+        d2h(cand_scores, E->snap_scores, sizeof(float) * n_cand);
+        d2h(cand_ids, E->snap_ids, sizeof(int32_t) * n_cand);
+        d2h(cand_counts, E->snap_counts, sizeof(int32_t) * n_lr);
+        d2h(cand_thr, E->snap_thr, sizeof(float) * n_lr);
+        d2h(row_exp, E->snap_row_exp, sizeof(int32_t) * m.rows_pad);
+        if (fb_rows && meta->n_fb > 0)
+            CK(cudaMemcpyAsync(fb_rows, E->snap_fb.as<int32_t>() + 2 + cnt[0], sizeof(int32_t) * meta->n_fb, cudaMemcpyDeviceToHost, st));
+        if (rows) {
+            if (E->snap_has_rows)
+                d2h(rows, E->snap_rows, sizeof(int32_t) * m.n_sel);
+            else
+                for (int64_t i = 0; i < m.n_sel; ++i) rows[i] = (int32_t)(E->snap_row0 + i);
+        }
+        CK(cudaStreamSynchronize(st));
+    } catch (const CudaError& ce) {
+        return fail(B200_E_CUDA, "b200_rank_get_snapshot: %s failed: %s", ce.what, cudaGetErrorString(ce.e));
+    }
     return B200_OK;
 }
 

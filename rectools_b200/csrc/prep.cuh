@@ -50,7 +50,9 @@ __device__ __forceinline__ __nv_bfloat16 to_tc<__nv_bfloat16>(float v) {
     return __float2bfloat16_rn(v);
 }
 
-// Power-of-two exponent e such that amax * 2^e lies in [2^13, 2^14) (fp16 operand scaling); 0 when amax is 0.
+// Power-of-two exponent e such that amax * 2^e lies in [2^13, 2^14); 0 when amax is 0 or not finite.  Both operand types
+// are scaled: fp16 for its narrow range, bf16 because the tensor cores do not keep fp32-subnormal (bf16-subnormal)
+// operands, so a tiny unscaled row would lose its scores entirely while eps, relative to the row's norm, stays tight.
 __host__ __device__ __forceinline__ int fp16_scale_exp(float amax) {
     if (!(amax > 0.f) || !isfinite(amax)) return 0;
     int ex;
@@ -63,7 +65,7 @@ __host__ __device__ __forceinline__ int fp16_scale_exp(float amax) {
 template <typename T, bool PER_ROW_EXP>
 __global__ void convert_rows_kernel(const float* __restrict__ x, const int64_t* __restrict__ row_map,
                                     const int32_t* __restrict__ sel_rows, int64_t n, int64_t n_pad, int d, int d_pad,
-                                    const float* __restrict__ norms, int fixed_exp, int use_scale, T* __restrict__ out,
+                                    const float* __restrict__ norms, int fixed_exp, T* __restrict__ out,
                                     int32_t* __restrict__ row_exp) {
     const int lane = threadIdx.x & 31;
     const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -83,7 +85,7 @@ __global__ void convert_rows_kernel(const float* __restrict__ x, const int64_t* 
         for (int j = lane; j < d; j += 32) amax = fmaxf(amax, fabsf(xr[j]));
 #pragma unroll
         for (int o2 = 16; o2 > 0; o2 >>= 1) amax = fmaxf(amax, __shfl_xor_sync(B200_FULL_MASK, amax, o2));
-        e = use_scale ? fp16_scale_exp(amax) : 0;
+        e = fp16_scale_exp(amax);
         if (lane == 0) row_exp[row] = e;
     }
     for (int j = lane; j < d_pad; j += 32) {

@@ -179,6 +179,37 @@ class Engine:
         assert len(blob) == 64 * len(handles)
         _lib.check(self._lib.b200_rank_peer_import(self._h, len(handles), int(self_index), blob))
 
+    def candidate_snapshot(self) -> tp.Optional[tp.Dict[str, tp.Any]]:
+        """Test interface: the tensor-core pass the last call captured with B200_TC_SNAPSHOT=n set (None: nothing was
+        captured).  The metadata of `b200_rank_snapshot` plus numpy arrays: `cand_scores` / `cand_ids`
+        [n_lists, rows_pad, cand_stride], `cand_counts` / `cand_thr` [n_lists, rows_pad], `row_exp` [n_sel], `rows` [n_sel]
+        (the call's row of each batch row of the pass), `fb_rows` [n_fb] (rows the pass's re-score sent to the fallback)."""
+        meta = _lib.Snapshot()
+        null = [None] * 7
+        _lib.check(self._lib.b200_rank_get_snapshot(self._h, C.byref(meta), *null))
+        if not meta.valid:
+            return None
+        n_lr = meta.n_lists * meta.rows_pad
+        out: tp.Dict[str, tp.Any] = {name: getattr(meta, name) for name, _ in meta._fields_}  # pylint: disable=protected-access
+        arrays = {
+            "cand_scores": np.empty(n_lr * meta.cand_stride, np.float32),
+            "cand_ids": np.empty(n_lr * meta.cand_stride, np.int32),
+            "cand_counts": np.empty(n_lr, np.int32),
+            "cand_thr": np.empty(n_lr, np.float32),
+            "row_exp": np.empty(meta.rows_pad, np.int32),
+            "rows": np.empty(meta.n_sel, np.int32),
+            "fb_rows": np.empty(meta.n_fb, np.int32),
+        }
+        _lib.check(self._lib.b200_rank_get_snapshot(self._h, C.byref(meta), *[a.ctypes.data for a in arrays.values()]))
+        lists = (meta.n_lists, meta.rows_pad)
+        arrays["cand_scores"] = arrays["cand_scores"].reshape(*lists, meta.cand_stride)
+        arrays["cand_ids"] = arrays["cand_ids"].reshape(*lists, meta.cand_stride)
+        arrays["cand_counts"] = arrays["cand_counts"].reshape(lists)
+        arrays["cand_thr"] = arrays["cand_thr"].reshape(lists)
+        arrays["row_exp"] = arrays["row_exp"][: meta.n_sel]
+        out.update(arrays)
+        return out
+
     def topk_raw(self, q: _lib.Query) -> tp.Dict[str, tp.Any]:
         st = _lib.Stats()
         _lib.check(self._lib.b200_rank_topk(self._h, C.byref(q), C.byref(st)))

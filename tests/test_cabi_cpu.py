@@ -33,7 +33,12 @@ def test_struct_layouts_match_header():
     from rectools_b200 import _lib
 
     header = open(os.path.join(ROOT, "include", "b200_rank.h")).read()
-    for cname, struct in (("b200_rank_query", _lib.Query), ("b200_rank_stats", _lib.Stats), ("b200_rank_info", _lib.Info)):
+    for cname, struct in (
+        ("b200_rank_query", _lib.Query),
+        ("b200_rank_stats", _lib.Stats),
+        ("b200_rank_info", _lib.Info),
+        ("b200_rank_snapshot", _lib.Snapshot),
+    ):
         body = re.search(r"typedef struct %s \{(.*?)\} %s;" % (cname, cname), header, re.S).group(1)
         body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
         names = [re.search(r"(\w+)(\[\d+\])?\s*$", stmt.strip()).group(1) for stmt in body.split(";") if stmt.strip()]
