@@ -130,13 +130,16 @@ typedef struct b200_rank_query {
 
 typedef struct b200_rank_stats {
     int32_t path;            /* 0 = exhaustive fp64 kernel, 1 = tensor-core candidates + fp64 re-score, 2 = sparse subjects (SpMM
-                              * scores + streaming selection), 3 = k > 128: exhaustive scores materialised once + selection passes */
+                              * scores + streaming selection), 3 = k > 128 without the tensor-core path (k > 1024, k = None, a
+                              * problem below the tiny-problem size, B200_Q_FORCE_EXACT, B200_WIDE=0, or an expected candidate count
+                              * above half the catalogue): exhaustive scores materialised once + selection passes */
     int32_t tc_dtype;        /* B200_TC_FP16 / B200_TC_BF16 when path == 1 */
     int32_t k_out;           /* columns of the output arrays */
     int32_t k_cand;          /* candidates kept per row and item split by the tensor-core pass */
     int32_t n_splits;        /* item splits of the main kernel */
     int32_t n_launches;      /* kernels launched by this call */
-    int64_t n_fallback_rows; /* rows whose certificate failed after the first tensor-core pass (re-ranked with wider lists) */
+    int64_t n_fallback_rows; /* rows whose certificate failed after the first tensor-core pass (re-ranked with wider lists;
+                              * k > 128: by the exhaustive kernels of path 3 over these rows only) */
     int64_t n_exact_rows;    /* rows that still failed and were ranked by the exhaustive fp64 kernel */
     float ms_main;           /* CUDA-event time of the dominant kernel (tensor-core pass or exhaustive kernel), summed over chunks */
     float ms_total;          /* CUDA-event time of the whole call on the engine stream (copies included) */
@@ -147,7 +150,7 @@ typedef struct b200_rank_stats {
     int32_t n_chunks;        /* row chunks of the copy / compute pipeline (1: call not chunked) */
     int32_t n_tc_launches;   /* launches of the fused tensor-core kernel summed in ms_main (main pass, second chance, re-rank passes) */
     int32_t epi_warps;       /* epilogue warps per CTA of the fused kernel (8 or 16) */
-    int32_t wide;            /* 1: single-pass wide mode (24 < k <= 128) */
+    int32_t wide;            /* 1: single-pass wide mode (24 < k <= 1024) */
     float ms_select;         /* CUDA-event time of the fp64 re-score / selection kernels */
     int32_t reserved;
 } b200_rank_stats;

@@ -345,6 +345,7 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
         }
         CK(cudaFuncSetAttribute(rescore_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
         CK(cudaFuncSetAttribute(rescore_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
+        CK(cudaFuncSetAttribute(rescore_wide_large_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     } catch (const CudaError& ce) {
         int rc = fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_create: %s failed at line %d: %s",
                       ce.what, ce.line, cudaGetErrorString(ce.e));
@@ -354,6 +355,30 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
     }
     *out = E;
     return B200_OK;
+}
+
+// Wide mode: T = the candidates a row is expected to collect, and the slots of each of its `nlist` append lists.  The
+// threshold frozen after a fraction q of the stream is about the (lists x K' - 6)-th best of that fraction, i.e. rank
+// ~ (lists x K' - 6) / q overall, so q follows from T.  k <= 128: T = 1.35 k + 40 (K' = 24), at most WIDE_MAX slots per row.
+// k > 128: T = 1.6 k + 64 (K' = 32), at most WIDE_MAX_L slots per row -- the frozen threshold is an order statistic of
+// ~58 samples, and this margin keeps the rows with fewer than k candidates (or an overflowing list) near 0.3 % (DESIGN 3.4).
+struct WideGeom {
+    double T;
+    int cand_stride;
+};
+
+WideGeom wide_geom(int kp, int nlist) {
+    WideGeom g;
+    if (kp <= 128) {
+        g.T = env_int("B200_WIDE_T", (int)(1.35 * kp + 40));
+        g.cand_stride = (int)round_up((int64_t)(g.T / nlist * 1.5 + 32), 8);
+        g.cand_stride = std::min(g.cand_stride, WIDE_MAX / nlist);
+    } else {
+        g.T = env_int("B200_WIDE_T", (int)(1.6 * kp + 64));
+        g.cand_stride = (int)round_up((int64_t)(g.T / nlist * 1.5 + 32), 8);
+        g.cand_stride = std::min(g.cand_stride, WIDE_MAX_L / nlist);
+    }
+    return g;
 }
 
 // Everything one b200_rank_topk call needs, so that the passes below can be plain functions.
@@ -627,17 +652,15 @@ void run_tc(Call& c, const TcPass& t) {
     }
     tp.id_off = (int32_t)E->id_offset;
     const int n_lists = best_splits * nlist;
-    // wide mode: the lists hold ~T = 1.35 k + 40 candidates per row -- the threshold frozen after a fraction q of the stream
-    // is about the (lists x K' - 6)-th best of that fraction, i.e. rank ~ (lists x K' - 6) / q overall
+    // wide mode: the lists hold ~T candidates per row (wide_geom)
     int cand_stride = 32;
     tp.phase1_tiles = 0x7fffffff;
     if (t.wide) {
-        const double T = env_int("B200_WIDE_T", (int)(1.35 * t.kp + 40));
+        const WideGeom g = wide_geom(t.kp, nlist);
         const double rank_frozen = nlist * tp.k_cand - 6;
-        const double qf = std::min(1.0, rank_frozen / T);
+        const double qf = std::min(1.0, rank_frozen / g.T);
         tp.phase1_tiles = std::max(1, (int)std::ceil(qf * tp.tiles_per_split));
-        cand_stride = (int)round_up((int64_t)(T / nlist * 1.5 + 32), 8);
-        cand_stride = std::min(cand_stride, WIDE_MAX / nlist);
+        cand_stride = g.cand_stride;
     }
     tp.cand_stride = cand_stride;
     E->cand_scores.ensure(sizeof(float) * (size_t)n_lists * rows_pad * cand_stride);
@@ -740,7 +763,9 @@ void run_tc(Call& c, const TcPass& t) {
     sp.fb_row0 = t.rows_dev ? 0 : t.row0;
     sp.out_bounds = t.o_bounds;
     c.time_begin(1);
-    if (t.wide) {
+    if (t.wide && t.kp > 128) {
+        rescore_wide_large_kernel<<<(unsigned)t.n_sel, WIDE_THREADS_L, wide_large_smem(d), st>>>(sp);
+    } else if (t.wide) {
         rescore_wide_kernel<<<(unsigned)t.n_sel, WIDE_THREADS, (size_t)d * sizeof(float), st>>>(sp);
     } else {
         const size_t sel_smem = (size_t)SEL_WARPS * d * sizeof(float);
@@ -776,7 +801,7 @@ void run_sparse(Call& c, const int64_t* sp_indptr, const int32_t* sp_indices, co
         c.S.n_launches++;
         for (int k0 = 0; k0 < c.k_out; k0 += 32) {
             c.time_begin(1);
-            scores_topk_kernel<<<grid_for(nb * 32, 256), 256, 0, st>>>(E->sp_scores.as<float>(), nb, c.n_pos, c.wl, f_indptr ? f_indptr + b0 : nullptr,
+            scores_topk_kernel<<<grid_for(nb * 32, 256), 256, 0, st>>>(E->sp_scores.as<float>(), nullptr, nb, c.n_pos, c.wl, f_indptr ? f_indptr + b0 : nullptr,
                                                                       c.indices, (int32_t)E->id_offset, c.k_out, k0, std::min(32, c.k_out - k0),
                                                                       o_ids + b0 * c.k_out, o_scores + b0 * c.k_out, o_counts + b0);
             CK(cudaGetLastError());
@@ -787,8 +812,10 @@ void run_sparse(Call& c, const int64_t* sp_indptr, const int32_t* sp_indices, co
 }
 
 // Dense subjects with k > 128: one exhaustive scoring of bounded row chunks into HBM + k / 32 streaming selection passes.
-void run_dense_large_k(Call& c, const float* sub32, const int64_t* rowmap, const int64_t* f_indptr, int64_t nr, int32_t* o_ids,
-                       float* o_scores, int32_t* o_counts) {
+// rows == nullptr: rows [0, nr) of the given base pointers (a chunk's slices);  otherwise the nr logical rows listed in
+// `rows` (absolute rows of the call, whole-call base pointers): the re-rank of rows a k > 128 wide pass could not certify.
+void run_dense_large_k(Call& c, const int32_t* rows, const float* sub32, const int64_t* rowmap, const int64_t* f_indptr, int64_t nr,
+                       int32_t* o_ids, float* o_scores, int32_t* o_counts, bool timed) {
     b200_rank_engine* E = c.E;
     cudaStream_t st = c.st;
     const int64_t rows_max = std::max<int64_t>(32, std::min<int64_t>(nr, ((int64_t)1 << 30) / std::max<int64_t>(4 * c.n_pos, 1)) / 32 * 32);
@@ -798,20 +825,23 @@ void run_dense_large_k(Call& c, const float* sub32, const int64_t* rowmap, const
         const int blocks_x = grid_for(nb, 32);
         const int64_t tiles_total = (c.n_pos + 31) / 32;
         const int splits = (int)std::max<int64_t>(1, std::min<int64_t>((4 * E->sm_count + blocks_x - 1) / blocks_x, tiles_total));
-        c.time_begin(0);
+        const int32_t* rl = rows ? rows + b0 : nullptr;
+        if (timed) c.time_begin(0);
         dense_scores_kernel<<<dim3((unsigned)blocks_x, (unsigned)splits), 256, 0, st>>>(
-            rowmap ? sub32 : sub32 + b0 * c.d, rowmap ? rowmap + b0 : nullptr, nb, E->obj32_ptr, c.wl, c.n_pos, c.d, c.norms(),
-            E->sp_scores.as<float>());
+            (rowmap || rows) ? sub32 : sub32 + b0 * c.d, (rowmap && !rows) ? rowmap + b0 : rowmap, rl, nb, E->obj32_ptr, c.wl, c.n_pos,
+            c.d, c.norms(), E->sp_scores.as<float>());
         CK(cudaGetLastError());
-        c.time_end();
+        if (timed) c.time_end();
         c.S.n_launches++;
+        const int64_t ob = rows ? 0 : b0;  // outputs / filter rows: listed rows are absolute
         for (int k0 = 0; k0 < c.k_out; k0 += 32) {
-            c.time_begin(1);
-            scores_topk_kernel<<<grid_for(nb * 32, 256), 256, 0, st>>>(E->sp_scores.as<float>(), nb, c.n_pos, c.wl, f_indptr ? f_indptr + b0 : nullptr,
-                                                                      c.indices, (int32_t)E->id_offset, c.k_out, k0, std::min(32, c.k_out - k0),
-                                                                      o_ids + b0 * c.k_out, o_scores + b0 * c.k_out, o_counts + b0);
+            if (timed) c.time_begin(1);
+            scores_topk_kernel<<<grid_for(nb * 32, 256), 256, 0, st>>>(E->sp_scores.as<float>(), rl, nb, c.n_pos, c.wl,
+                                                                      f_indptr ? f_indptr + ob : nullptr, c.indices, (int32_t)E->id_offset,
+                                                                      c.k_out, k0, std::min(32, c.k_out - k0), o_ids + ob * c.k_out,
+                                                                      o_scores + ob * c.k_out, o_counts + ob);
             CK(cudaGetLastError());
-            c.time_end();
+            if (timed) c.time_end();
             c.S.n_launches++;
         }
     }
@@ -1129,9 +1159,14 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
         // certificate and take the second-chance pass.  Inserts, the dominant epilogue cost, scale with K'.
         c.bf16 = E->tc_dtype == B200_TC_BF16;
         const bool wide = k_out > 24 && k_out <= 128 && env_int("B200_WIDE", 1) != 0;
+        // 128 < k <= 1024: the same single wide pass with longer append lists and a large-k re-score, when the expected
+        // candidate count stays well inside the catalogue (k = None and near-catalogue requests keep path 3).  Item-sharded
+        // calls that share thresholds need k <= 24 and keep path 3 here as well.
+        const bool wide_l = k_out > 128 && k_out <= 1024 && env_int("B200_WIDE", 1) != 0 && !sparse_sub && !shared &&
+                            wide_geom(k_out, 2).T <= 0.5 * (double)n_pos;
         // 16 epilogue warps (B200_EPI_WARPS=16) are opt-in: next to the MMA warp group they get 96 registers a thread and
         // spill.  The wide mode always runs the 8-warp geometry: four lists per row freeze at a weaker, noisier rank.
-        c.nw = (!wide && env_int("B200_EPI_WARPS", 8) == 16) ? 16 : 8;
+        c.nw = (!wide && !wide_l && env_int("B200_EPI_WARPS", 8) == 16) ? 16 : 8;
         int k_cand = 0;
         if (k_out <= 24) {
             if (c.nw == 16) {
@@ -1144,6 +1179,8 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
             }
         } else if (k_out <= 128) {
             k_cand = wide ? 24 : (c.bf16 ? 30 : 25);  // wide: adaptive lists of phase 1;  else passes of 20
+        } else if (wide_l) {
+            k_cand = 32;  // the full 32 slots: the frozen threshold samples ~58 ranks instead of ~42
         }
         if (shared && E->n_peers > 0 && k_out <= 24) {
             // Shared thresholds: the pruning bound of a row is the MAXIMUM over all L = ranks x lists list minima, i.e. the
@@ -1159,7 +1196,7 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
         }
         {
             const int forced = env_int("B200_TC_KCAND", 0);  // tuning hook
-            if (forced >= 4 && forced <= 32 && (forced >= k_out || c.nw == 16 || wide || shared)) k_cand = forced;
+            if (forced >= 4 && forced <= 32 && (forced >= k_out || c.nw == 16 || wide || wide_l || shared)) k_cand = forced;
         }
         bool use_tc = !sparse_sub && E->tc_dtype != B200_TC_OFF && k_cand > 0 && !(q->flags & B200_Q_FORCE_EXACT) && n_pos >= (int64_t)k_cand * 4;
         if (use_tc && !(q->flags & B200_Q_FORCE_TC)) {
@@ -1182,7 +1219,7 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
         int32_t* fbB = fbA + n_rows;
         int32_t* cnt = fbB + n_rows;
         CK(cudaMemsetAsync(cnt, 0, 16 * sizeof(int32_t), st));
-        if (wide || (use_tc && k_out > 24)) E->excl.ensure(sizeof(int32_t) * (size_t)n_rows * k_out);
+        if (k_out <= 128 && (wide || (use_tc && k_out > 24))) E->excl.ensure(sizeof(int32_t) * (size_t)n_rows * k_out);  // (k > 128: no exclusion passes)
 
         // ---------------- main pass over the rows of one chunk
         auto main_pass = [&](int64_t r0, int64_t r1) {
@@ -1201,7 +1238,7 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
                 run_sparse(c, sp_indptr + r0, sp_indices, sp_data, nr, ip, oi, os, oc);
             } else if (!use_tc && k_out > 128) {
                 S.path = 3;  // materialised exhaustive scores + streaming selection passes
-                run_dense_large_k(c, sub, rm, ip, nr, oi, os, oc);
+                run_dense_large_k(c, nullptr, sub, rm, ip, nr, oi, os, oc, true);
                 if (c.o_bounds) {
                     fill_f32_kernel<<<grid_for(nr, 256), 256, 0, st>>>(c.o_bounds + r0, nr, -INFINITY);
                     CK(cudaGetLastError());
@@ -1234,7 +1271,7 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
                 t.peers = peers;
                 t.k0 = 0;
                 t.kp = k_out;
-                t.wide = wide;
+                t.wide = wide || wide_l;
                 run_tc(c, t);
             }
             if (E->id_offset != 0) {
@@ -1297,14 +1334,33 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
             }
         };
 
+        // k > 128: rows the wide pass could not certify are ranked by the exhaustive kernels of path 3, over these rows only.
+        auto rerank_exhaustive = [&](const int32_t* rows, int64_t n_sel) {
+            init_rows_kernel<<<grid_for(n_sel * k_out, 256), 256, 0, st>>>(c.o_ids, c.o_scores, c.o_counts, rows, n_sel, k_out);
+            CK(cudaGetLastError());
+            S.n_launches++;
+            run_dense_large_k(c, rows, c.sub32, c.rowmap, c.indptr, n_sel, c.o_ids, c.o_scores, c.o_counts, false);
+            S.n_exact_rows += n_sel;
+        };
+
         // ---------------- chunk pipeline
-        const bool multipass_main = use_tc && k_out > 24 && !wide;
+        const bool multipass_main = use_tc && k_out > 24 && !wide && !wide_l;
         int64_t chunk = n_rows;
         if (!in_dev && use_tc && !multipass_main) {
             const int64_t wave = (int64_t)(E->sm_count / 2) * 256;  // subject rows one wave of CTA pairs works on
             int64_t want = 8 * wave;
             if (const char* env = getenv("B200_CHUNK_ROWS")) want = std::max<int64_t>(256, atoll(env));  // test hook
             if (n_rows >= 2 * want) chunk = want;
+        }
+        if (use_tc && wide_l) {
+            // the append lists take lists x cand_stride x 8 B per row (~21 GB for 1M rows at k = 1000): row chunks keep them
+            // within the budget, for device inputs too.  Whole waves of CTA pairs where the budget allows.
+            const int64_t per_row = (int64_t)2 * wide_geom(k_out, 2).cand_stride * 8;
+            const int64_t budget = (int64_t)env_int("B200_WIDE_BUDGET_MB", 2048) << 20;  // test hook
+            const int64_t wave = (int64_t)(E->sm_count / 2) * 256;
+            int64_t fit = std::max<int64_t>(256, budget / per_row / 256 * 256);
+            if (fit >= wave) fit = fit / wave * wave;
+            chunk = std::min(chunk, fit);
         }
         const int64_t n_chunks = (n_rows + chunk - 1) / chunk;
         cudaStream_t cs = n_chunks > 1 ? E->cs : st;
@@ -1364,7 +1420,10 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
             n_fb = read_counter(c, cnt);
             S.n_fallback_rows = n_fb;
             if (n_fb > 0) {
-                rerank_rows(fb1, n_fb);
+                if (k_out > 128)
+                    rerank_exhaustive(fb1, n_fb);
+                else
+                    rerank_rows(fb1, n_fb);
                 if (E->id_offset != 0) {
                     add_offset_rows_kernel<<<grid_for(n_fb * k_out, 256), 256, 0, st>>>(c.o_ids, fb1, n_fb, k_out, (int32_t)E->id_offset);
                     CK(cudaGetLastError());

@@ -18,7 +18,7 @@
 //
 // Three selection modes share the epilogue:
 //   * adaptive lists (k <= 24): replace-minimum lists of K' slots, the list minimum is the running threshold;
-//   * wide mode (24 < k <= 128): adaptive lists for the first `phase1_tiles` tiles of the stream, then the threshold is
+//   * wide mode (24 < k <= 1024): adaptive lists for the first `phase1_tiles` tiles of the stream, then the threshold is
 //     FROZEN and every later score above it is appended to a global list -- ~1.5 k candidates per row in ONE pass with
 //     ~3x fewer hits than adaptive lists of that size would take;
 //   * shared thresholds (item-sharded multi-GPU): the row's threshold is the maximum over all ranks' thresholds.

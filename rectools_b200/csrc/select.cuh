@@ -177,7 +177,8 @@ __global__ void __launch_bounds__(EX_THREADS) exact_topk_kernel(const ExactParam
 //                           item-sharded catalogue); optional certificate over per-list bounds.
 //   rescore_select_kernel : lists carry approximate (tensor-core) scores; every candidate is re-scored in fp64 from the
 //                           fp32 master copies and the row is certified or queued for a re-rank (kp <= 32).
-//   rescore_wide_kernel   : the same for the wide mode (kp <= 128, up to 512 candidates per row), one block per row.
+//   rescore_wide_kernel   : the same for the wide mode (kp <= 128, up to 512 candidates per row), one block per row;
+//   rescore_wide_large_kernel : the wide mode for 128 < kp <= 1024 (up to 4096 candidates per row), one block per row.
 // Certificate: every list reports the final pruning threshold `thr` of its stream -- no discarded object had an
 // approximate score above it.  With eps = eps_rel * |u|_2 * max_i |i|_2 bounding |approx - exact|, a row whose kp-th exact
 // score exceeds max(thr) + eps cannot have lost a top-kp object.
@@ -440,18 +441,24 @@ __global__ void __launch_bounds__(SEL_WARPS * 32) rescore_select_kernel(const Se
     }
 }
 
-// Wide mode: one block of 128 threads per row, up to WIDE_MAX candidates.  Two stages: the candidates are sorted by their
-// APPROXIMATE scores first; only those within 2 eps of the kp-th best approximate score can reach the exact top-kp (everything
-// below ranks under kp others, see rescore_select_kernel) and are re-scored (thread = candidate) -- ~110 of ~180 gathered rows
-// at k = 100 -- then sorted by (exact score desc, id asc) with the same bitonic network in shared memory.
+// Wide mode: one block per row.  Two stages: the candidates are sorted by their APPROXIMATE scores first; only those within
+// 2 eps of the kp-th best approximate score can reach the exact top-kp (everything below ranks under kp others, see
+// rescore_select_kernel) and are re-scored (thread = candidate) -- ~110 of ~180 gathered rows at k = 100 -- then sorted by
+// (exact score desc, id asc) with the same bitonic network in shared memory.
+//   rescore_wide_kernel       : kp <= 128, up to WIDE_MAX candidates per row, 128 threads, static shared arrays;
+//   rescore_wide_large_kernel : 128 < kp <= 1024, up to WIDE_MAX_L candidates per row, 256 threads, the arrays in dynamic
+//                               shared memory behind the subject row (32 KiB of score / id pairs at full capacity).
 constexpr int WIDE_THREADS = 128;
 constexpr int WIDE_MAX = 512;
+constexpr int WIDE_THREADS_L = 256;
+constexpr int WIDE_MAX_L = 4096;
 
 // best-first bitonic sort of s_sc / s_id [0, n), n a power of two (all threads of the block)
+template <int THREADS>
 __device__ __forceinline__ void block_bitonic_sort(float* s_sc, int* s_id, int n, int tid) {
     for (int k = 2; k <= n; k <<= 1) {
         for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int i = tid; i < n; i += WIDE_THREADS) {
+            for (int i = tid; i < n; i += THREADS) {
                 const int ixj = i ^ j;
                 if (ixj > i) {
                     const float a = s_sc[i], b = s_sc[ixj];
@@ -471,13 +478,21 @@ __device__ __forceinline__ void block_bitonic_sort(float* s_sc, int* s_id, int n
     }
 }
 
-__global__ void __launch_bounds__(WIDE_THREADS) rescore_wide_kernel(const SelectParams p) {
-    extern __shared__ float s_dyn[];  // [d] subject row
-    __shared__ float s_sc[WIDE_MAX];
-    __shared__ int s_id[WIDE_MAX];
+// sum over the warps of the block (s_part: one slot per warp, written by lane 0 before the barrier that precedes the call)
+template <int THREADS, typename T>
+__device__ __forceinline__ T warp_slots_sum(const T* s_part) {
+    T v = s_part[0];
+#pragma unroll
+    for (int w = 1; w < THREADS / 32; ++w) v += s_part[w];
+    return v;
+}
+
+// The body shared by both wide re-score kernels: s_dyn = subject row [d], s_sc / s_id = MAX candidate slots.
+template <int THREADS, int MAX>
+__device__ __forceinline__ void rescore_wide_row(const SelectParams& p, float* s_dyn, float* s_sc, int* s_id) {
     __shared__ int s_off[65];
-    __shared__ double s_red[WIDE_THREADS / 32];
-    __shared__ int s_cnt[WIDE_THREADS / 32];
+    __shared__ double s_red[THREADS / 32];
+    __shared__ int s_cnt[THREADS / 32];
     __shared__ float s_thr;
     __shared__ int s_flag;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -494,7 +509,7 @@ __global__ void __launch_bounds__(WIDE_THREADS) rescore_wide_kernel(const Select
     double un = 0.0;
     {
         const int64_t pr = p.row_map ? p.row_map[lrow] : lrow;
-        for (int j = tid; j < p.d; j += WIDE_THREADS) {
+        for (int j = tid; j < p.d; j += THREADS) {
             const float v = __ldg(p.subjects + pr * p.d + j);
             s_dyn[j] = v;
             un = fma((double)v, (double)v, un);
@@ -514,9 +529,9 @@ __global__ void __launch_bounds__(WIDE_THREADS) rescore_wide_kernel(const Select
             acc += min(c, p.L);
             tm = fmaxf(tm, p.in_thr[o]);
         }
-        if (acc > WIDE_MAX) {  // (cannot happen when the engine keeps n_lists * L <= WIDE_MAX)
+        if (acc > MAX) {  // (cannot happen when the engine keeps n_lists * L <= MAX)
             ovf = 1;
-            acc = WIDE_MAX;
+            acc = MAX;
         }
         s_off[p.n_lists] = acc;
         s_thr = tm;
@@ -524,14 +539,14 @@ __global__ void __launch_bounds__(WIDE_THREADS) rescore_wide_kernel(const Select
     }
     __syncthreads();
     const int total = s_off[p.n_lists];
-    const double unorm2 = s_red[0] + s_red[1] + s_red[2] + s_red[3];
+    const double unorm2 = warp_slots_sum<THREADS>(s_red);
     const int ex = (p.row_exp ? p.row_exp[sel] : 0) + p.obj_exp;
     const double eps = (double)p.eps_rel * sqrt(unorm2) * (double)p.max_obj_norm;
     int n = 2;
     while (n < total) n <<= 1;
     // ---- stage 1: candidates with their approximate scores, best first
     int n_valid = 0;
-    for (int c = tid; c < n; c += WIDE_THREADS) {
+    for (int c = tid; c < n; c += THREADS) {
         float s = -INFINITY;
         int id = B200_PAD_ID;
         if (c < total) {
@@ -553,26 +568,26 @@ __global__ void __launch_bounds__(WIDE_THREADS) rescore_wide_kernel(const Select
     for (int o = 16; o > 0; o >>= 1) n_valid += __shfl_xor_sync(B200_FULL_MASK, n_valid, o);
     if (lane == 0) s_cnt[warp] = n_valid;
     __syncthreads();
-    n_valid = s_cnt[0] + s_cnt[1] + s_cnt[2] + s_cnt[3];
-    block_bitonic_sort(s_sc, s_id, n, tid);
+    n_valid = warp_slots_sum<THREADS>(s_cnt);
+    block_bitonic_sort<THREADS>(s_sc, s_id, n, tid);
     // ---- the band: [0, m) = candidates that may still reach the exact top-kp (first pass only; later passes re-score all)
     int m = n_valid;
     if (p.k0 == 0 && n_valid > p.kp) {
         const double cut = (double)s_sc[p.kp - 1] - 2.0 * ldexp(eps, ex) * (1.0 + 1e-6);
         int below = 0;  // sorted: the candidates under the cut form a suffix of [0, n_valid)
-        for (int c = tid; c < n_valid; c += WIDE_THREADS) below += (double)s_sc[c] < cut ? 1 : 0;
+        for (int c = tid; c < n_valid; c += THREADS) below += (double)s_sc[c] < cut ? 1 : 0;
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) below += __shfl_xor_sync(B200_FULL_MASK, below, o);
         __syncthreads();  // (s_cnt is read above by every thread before it is rewritten)
         if (lane == 0) s_cnt[warp] = below;
         __syncthreads();
-        m = n_valid - (s_cnt[0] + s_cnt[1] + s_cnt[2] + s_cnt[3]);
+        m = n_valid - warp_slots_sum<THREADS>(s_cnt);
     }
     __syncthreads();
     // ---- stage 2: exact scores of the band, everything else leaves the ranking
     int n2 = 2;
     while (n2 < m) n2 <<= 1;
-    for (int c = tid; c < n; c += WIDE_THREADS) {
+    for (int c = tid; c < n; c += THREADS) {
         float s = -INFINITY;
         int id = B200_PAD_ID;
         if (c < m) {
@@ -587,18 +602,18 @@ __global__ void __launch_bounds__(WIDE_THREADS) rescore_wide_kernel(const Select
         s_id[c] = id;
     }
     __syncthreads();
-    block_bitonic_sort(s_sc, s_id, n2, tid);
+    block_bitonic_sort<THREADS>(s_sc, s_id, n2, tid);
     int n_rank = 0;  // candidates still in the ranking (valid ones sort before the (-inf, PAD) fillers)
-    for (int i = tid; i < n2; i += WIDE_THREADS) n_rank += s_id[i] != B200_PAD_ID ? 1 : 0;
+    for (int i = tid; i < n2; i += THREADS) n_rank += s_id[i] != B200_PAD_ID ? 1 : 0;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) n_rank += __shfl_xor_sync(B200_FULL_MASK, n_rank, o);
     __syncthreads();
     if (lane == 0) s_cnt[warp] = n_rank;
     __syncthreads();
-    n_rank = s_cnt[0] + s_cnt[1] + s_cnt[2] + s_cnt[3];
+    n_rank = warp_slots_sum<THREADS>(s_cnt);
     if (p.k0 > 0) n_valid = n_rank;  // later passes: only what survived the bound counts
     const int n_out = min(n_rank, p.kp);
-    for (int i = tid; i < p.kp; i += WIDE_THREADS) {
+    for (int i = tid; i < p.kp; i += THREADS) {
         const bool w = i < n_out;
         p.out_ids[lrow * p.k_out + p.k0 + i] = w ? s_id[i] : -1;
         p.out_scores[lrow * p.k_out + p.k0 + i] = w ? s_sc[i] : -FLT_MAX;
@@ -616,6 +631,23 @@ __global__ void __launch_bounds__(WIDE_THREADS) rescore_wide_kernel(const Select
             }
         }
     }
+}
+
+__global__ void __launch_bounds__(WIDE_THREADS) rescore_wide_kernel(const SelectParams p) {
+    extern __shared__ float s_dyn[];  // [d] subject row
+    __shared__ float s_sc[WIDE_MAX];
+    __shared__ int s_id[WIDE_MAX];
+    rescore_wide_row<WIDE_THREADS, WIDE_MAX>(p, s_dyn, s_sc, s_id);
+}
+
+// dynamic shared memory: [d] subject row (rounded up to 4 floats), [WIDE_MAX_L] scores, [WIDE_MAX_L] ids
+__host__ __device__ constexpr size_t wide_large_smem(int d) { return ((size_t)(d + 3) / 4 * 4 + 2 * WIDE_MAX_L) * 4; }
+
+__global__ void __launch_bounds__(WIDE_THREADS_L) rescore_wide_large_kernel(const SelectParams p) {
+    extern __shared__ float s_dyn[];
+    float* s_sc = s_dyn + (p.d + 3) / 4 * 4;
+    int* s_id = reinterpret_cast<int*>(s_sc + WIDE_MAX_L);
+    rescore_wide_row<WIDE_THREADS_L, WIDE_MAX_L>(p, s_dyn, s_sc, s_id);
 }
 
 // Multi-pass ranking: the ids a row has received so far, sorted ascending, become the row's exclusion list for the next

@@ -70,10 +70,12 @@ __global__ void __launch_bounds__(SP_THREADS) sparse_scores_kernel(const int64_t
 // exhaustive kernel's arithmetic (fp64-accumulated dot, / norm for COSINE, rounded to fp32) and the k / 32 selection passes
 // stream 4-byte scores instead of repeating 2 d fp64 FLOP per object and pass.
 // Block = 32 subjects x 32 positions per step (lane = position), grid (row blocks, position splits).
+// `rows` (nullable): entry r of the batch is logical row rows[r] (the rows a wide pass could not certify); score row r of
+// the output stays compact.
 constexpr int DS_DK = 64;
 
 __global__ void __launch_bounds__(256) dense_scores_kernel(const float* __restrict__ subjects, const int64_t* __restrict__ row_map,
-                                                           int64_t n_rows, const float* __restrict__ objects,
+                                                           const int32_t* __restrict__ rows, int64_t n_rows, const float* __restrict__ objects,
                                                            const int32_t* __restrict__ pos2obj, int64_t n_pos, int32_t d,
                                                            const float* __restrict__ obj_norms, float* __restrict__ scores) {
     __shared__ float s_obj[32][DS_DK + 1];
@@ -98,7 +100,10 @@ __global__ void __launch_bounds__(256) dense_scores_kernel(const float* __restri
                 s_obj[it][j] = v;
                 const int64_t r = row0 + it;
                 float u = 0.f;
-                if (r < n_rows && dk0 + j < d) u = __ldg(subjects + (row_map ? row_map[r] : r) * d + dk0 + j);
+                if (r < n_rows && dk0 + j < d) {
+                    const int64_t lr = rows ? (int64_t)rows[r] : r;
+                    u = __ldg(subjects + (row_map ? row_map[lr] : lr) * d + dk0 + j);
+                }
                 s_sub[it][j] = u;
             }
             __syncthreads();
@@ -124,15 +129,18 @@ __global__ void __launch_bounds__(256) dense_scores_kernel(const float* __restri
 
 // One warp per row: streaming top-kp (kp <= 32) over a materialised score row, order (score desc, id asc), objects listed
 // in the row's filter_pairs_csr slice never returned; entries [k0, k0 + kp) of a k > 32 query are bounded by the previous
-// pass's last entry exactly as in exact_topk_kernel.
-__global__ void __launch_bounds__(256) scores_topk_kernel(const float* __restrict__ scores, int64_t n_rows, int64_t n_pos,
+// pass's last entry exactly as in exact_topk_kernel.  `rows` (nullable): score row r belongs to logical row rows[r], which
+// indexes the filter and the outputs.
+__global__ void __launch_bounds__(256) scores_topk_kernel(const float* __restrict__ scores, const int32_t* __restrict__ rows, int64_t n_rows,
+                                                          int64_t n_pos,
                                                           const int32_t* __restrict__ pos2obj, const int64_t* __restrict__ f_indptr,
                                                           const int32_t* __restrict__ f_indices, int32_t id_off, int32_t k_out, int32_t k0,
                                                           int32_t kp, int32_t* __restrict__ out_ids, float* __restrict__ out_scores,
                                                           int32_t* __restrict__ out_counts) {
     const int lane = threadIdx.x & 31;
-    const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (row >= n_rows) return;
+    const int64_t sr = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (sr >= n_rows) return;
+    const int64_t row = rows ? (int64_t)rows[sr] : sr;
     float bs = INFINITY;
     int bi = -1;
     if (k0 > 0) {
@@ -147,7 +155,7 @@ __global__ void __launch_bounds__(256) scores_topk_kernel(const float* __restric
     }
     float thr = -INFINITY, ls = -INFINITY;
     int li = B200_PAD_ID;
-    const float* srow = scores + row * n_pos;
+    const float* srow = scores + sr * n_pos;
     for (int64_t p0 = 0; p0 < n_pos; p0 += 32) {
         const int64_t pos = p0 + lane;
         const bool valid = pos < n_pos;
