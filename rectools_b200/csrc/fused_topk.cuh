@@ -2,8 +2,8 @@
 //
 //   TMA (own 128 subject rows once per work item; every 256-object tile as four quarters of 64 objects, streamed through a
 //   ring of 8 KiB blocks) -> wgmma 64 x 64 x 16 (fp16 / bf16 -> fp32) into the registers of the MMA warp group
-//   -> each finished quarter [128 rows x 64 columns] is staged in shared memory and read back by the epilogue warps, one
-//   row per thread; the staging buffer is handed back as soon as the rows are in registers
+//   -> each finished quarter [128 rows x 64 columns] is staged in shared memory, one m-half of 64 rows at a time, and
+//   read back by the epilogue warps, one row per thread; a staged half is handed back as soon as its rows are in registers
 //   -> threshold scan (3-input max tree), hits extracted into per-thread ring FIFOs in shared memory
 //   -> deferred, bounded steps: filter_pairs_csr lookup through a prefetched 4-entry window, candidate-list insertion.
 // Score rows never reach HBM: only the K' best (score, id) pairs per row and column group are written.
@@ -134,6 +134,50 @@ __device__ __forceinline__ void fifo_step(const TcParams& p, RowState& rs, CsrWi
     }
 }
 
+// One m-half of a quarter (64 subject rows x 64 objects, all KB k blocks) as one wgmma commit group, straight-line code
+// (ptxas serialises a group whose wgmmas are spread over a loop or a barrier wait): the object blocks sit in ring slots
+// s, s + 1, ... (mod NS) and have landed.  Every accumulator sums its k steps in the same order as ever: kb, then k.
+template <bool BF16, int KB>
+__device__ __forceinline__ void mma_half(uint32_t (&d)[32], uint32_t a_lo, uint32_t b_lo0, int NS, uint32_t s) {
+    constexpr uint32_t BLK16 = BLK_BYTES >> 4, OBJ16 = OBJ_BLK_BYTES >> 4;
+    fence_acc(d);
+    wgmma_fence();
+#pragma unroll
+    for (int kb = 0; kb < KB; ++kb) {
+        const uint32_t b_lo = b_lo0 + s * OBJ16;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_64x64<BF16>(d, a_lo + kb * BLK16 + 2 * k, b_lo + 2 * k, (kb | k) != 0);
+        if (++s == (uint32_t)NS) s = 0;
+    }
+    wgmma_commit();
+}
+
+// Wait until the KB object blocks of a quarter (ring slots s, s + 1, ... from phase ph) have landed.
+template <int KB>
+__device__ __forceinline__ void blocks_landed(uint32_t bar_full, int NS, uint32_t s, uint32_t ph) {
+#pragma unroll
+    for (int kb = 0; kb < KB; ++kb) {
+        mbar_wait(bar_full + 8 * s, ph);
+        if (++s == (uint32_t)NS) {
+            s = 0;
+            ph ^= 1;
+        }
+    }
+}
+
+// Hand one m-half of a finished quarter to the epilogue: wait until its two readers have taken the previous one, store
+// this thread's 32 accumulators of it, arrive on the half's `full` barrier.
+__device__ __forceinline__ void store_half(const uint32_t (&d)[32], uint32_t stg, uint32_t qempty, uint32_t parity, uint32_t qfull) {
+    mbar_wait(qempty, parity);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const uint32_t a = stg + (uint32_t)(8 * j * 4);
+        sts_v2(a, d[4 * j], d[4 * j + 1]);
+        sts_v2(a + 8 * STG_STRIDE * 4, d[4 * j + 2], d[4 * j + 3]);
+    }
+    mbar_arrive(qfull);
+}
+
 // Shared-memory map (dynamic, 1 KiB aligned): [KB] subject blocks (16 KiB each) | [NS] object blocks (8 KiB each: 64
 // objects of a tile quarter) | accumulator staging [128 rows][STG_STRIDE] fp32 | candidate lists [NLIST][128 rows][SLOTS]
 // scores + ids | FIFOs | thresholds [NLIST + 1][128] | barriers.
@@ -158,8 +202,9 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
     uint64_t* bars = reinterpret_cast<uint64_t*>(sThr + (NLIST + 1) * TILE_M);
     const uint32_t bar_full = smem_u32(bars);                     // [NS] object block landed
     const uint32_t bar_afull = smem_u32(bars + MAX_STAGES);       // subject blocks landed
-    const uint32_t bar_qfull = smem_u32(bars + MAX_STAGES + 1);   // [4] quarter q of the current tile staged
-    const uint32_t bar_qempty = smem_u32(bars + MAX_STAGES + 5);  // staged quarter read by its four epilogue warps
+    // the staging buffer's two m-halves (rows 0-63 / 64-127) are handed over separately
+    const uint32_t bar_qfull = smem_u32(bars + MAX_STAGES + 1);   // [4][2] half h of quarter q of the current tile staged
+    const uint32_t bar_qempty = smem_u32(bars + MAX_STAGES + 9);  // [2] staged half read by its two epilogue warps
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int rank = blockIdx.x & 1;  // which 128 rows of the pair's 256 (== the CTA's rank in its cluster)
@@ -168,8 +213,8 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
     if (threadIdx.x == 0) {
         for (int i = 0; i < NS; ++i) mbar_init(bar_full + 8 * i, 1);
         mbar_init(bar_afull, 1);
-        for (int q = 0; q < 4; ++q) mbar_init(bar_qfull + 8 * q, 128);  // every thread of the MMA warp group
-        mbar_init(bar_qempty, 4);
+        for (int i = 0; i < 8; ++i) mbar_init(bar_qfull + 8 * i, 128);  // every thread of the MMA warp group
+        for (int h = 0; h < 2; ++h) mbar_init(bar_qempty + 8 * h, 2);
         fence_barrier_init();
         tma_prefetch_desc(&tm_sub);
         tma_prefetch_desc(&tm_obj);
@@ -233,33 +278,83 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
 
         // this thread's accumulator rows / columns in the staging buffer (m-half 1: + 64 rows; second row of a fragment: + 8)
         const uint32_t stg_w = smem_u32(sStg) + (uint32_t)(((warp * 16 + (lane >> 2)) * STG_STRIDE + 2 * (lane & 3)) * 4);
+        const uint32_t stg_w1 = stg_w + (uint32_t)(64 * STG_STRIDE * 4);
         const uint32_t a_lo0 = smem_desc_lo(sA_u), b_lo0 = smem_desc_lo(sB_u);
-        float acc[2][32];
+        // fp32 accumulators of the two m-halves, as bit patterns
+        uint32_t acc[2][32];
 #pragma unroll
-        for (int i = 0; i < 32; ++i) acc[0][i] = acc[1][i] = 0.f;
+        for (int i = 0; i < 32; ++i) acc[0][i] = acc[1][i] = 0u;
         uint32_t stage = 0, ph = 0, work_it = 0, n_store = 0;
+        // d_pad = 128 (two k blocks; the ring holds two quarters' object blocks): each m-half is its own commit group and
+        // the hand-off of one half overlaps the MMAs of the other --
+        //   G0(q), G1(q) | wait<1>, store half 0 of q, G0(q + 1) | wait<1>, release q's blocks, store half 1 of q,
+        //   G1(q + 1) | ...
+        // The ring slots of quarter q are refilled once G1(q), their second reader, has retired.  (The 16-warp geometry
+        // leaves the MMA warp group 80-96 registers: it keeps the per-k-block schedule below, which spills less there.)
+        constexpr int PKB = 2;
+        const bool pipelined = NW == 8 && KB == PKB && 2 * PKB <= NS;
+        auto advance = [&]() {  // ring position of the next quarter's first block
+            stage += (uint32_t)PKB;
+            if (stage >= (uint32_t)NS) {
+                stage -= (uint32_t)NS;
+                ph ^= 1;
+            }
+        };
         for (int w = pair; w < n_work; w += n_pairs, ++work_it) {
             const int split = w / p.n_row_tiles, rt = w - split * p.n_row_tiles;
             const int t0 = split * p.tiles_per_split;
             const int t1 = min(t0 + p.tiles_per_split, p.n_obj_tiles);
-            // the previous work item's MMAs have all retired (every quarter ends in wgmma.wait_group 0)
+            // the previous work item's MMAs have all retired (every work item ends in wgmma.wait_group 0)
             if (issuer) {
                 mbar_arrive_expect_tx(bar_afull, (uint32_t)(KB * BLK_BYTES));
                 for (int kb = 0; kb < KB; ++kb)
                     tma_load_2d(sA_u + (uint32_t)kb * BLK_BYTES, &tm_sub, bar_afull, kb * KBLK, (rt * 2 + rank) * TILE_M);
             }
             mbar_wait(bar_afull, work_it & 1);
-            for (int i = 0; i < t1 - t0; ++i) {
-                for (int q = 0; q < 4; ++q) {
+            const int nq = 4 * (t1 - t0);  // quarters of the work item, in stream order
+            // (rows 64-127 of the subject block start 8 KiB = +512 descriptor units further)
+            if (pipelined) {
+                blocks_landed<PKB>(bar_full, NS, stage, ph);
+                mma_half<BF16, PKB>(acc[0], a_lo0, b_lo0, NS, stage);
+                mma_half<BF16, PKB>(acc[1], a_lo0 + 512, b_lo0, NS, stage);
+                advance();
+                for (int qi = 0; qi + 1 < nq; ++qi, ++n_store) {
+                    const uint32_t qf = bar_qfull + 16 * (qi & 3), par = (n_store & 1) ^ 1;
+                    wgmma_wait<1>();  // G0(qi)
+                    fence_acc(acc[0]);
+                    store_half(acc[0], stg_w, bar_qempty, par, qf);
+                    blocks_landed<PKB>(bar_full, NS, stage, ph);
+                    mma_half<BF16, PKB>(acc[0], a_lo0, b_lo0, NS, stage);
+                    wgmma_wait<1>();  // G1(qi): quarter qi's object blocks are free
+                    fence_acc(acc[1]);
+                    done += PKB;
+                    refill();
+                    store_half(acc[1], stg_w1, bar_qempty + 8, par, qf + 8);
+                    mma_half<BF16, PKB>(acc[1], a_lo0 + 512, b_lo0, NS, stage);
+                    advance();
+                }
+                const uint32_t qf = bar_qfull + 16 * ((nq - 1) & 3), par = (n_store & 1) ^ 1;
+                wgmma_wait<1>();
+                fence_acc(acc[0]);
+                store_half(acc[0], stg_w, bar_qempty, par, qf);
+                wgmma_wait<0>();  // the work item's last MMAs (the next one reloads the subject blocks)
+                fence_acc(acc[1]);
+                done += PKB;
+                refill();
+                store_half(acc[1], stg_w1, bar_qempty + 8, par, qf + 8);
+                ++n_store;
+            } else {
+                // deeper d: one commit group per k block (both m-halves), its ring slot refilled as soon as the next
+                // block's group has been issued and the block's own group has retired
+                for (int qi = 0; qi < nq; ++qi, ++n_store) {
                     uint32_t a_lo = a_lo0;
+                    fence_acc(acc[0]);
+                    fence_acc(acc[1]);
                     for (int kb = 0; kb < KB; ++kb, a_lo += BLK16) {
                         mbar_wait(bar_full + 8 * stage, ph);
-                        fence_acc(acc[0]);
-                        fence_acc(acc[1]);
                         wgmma_fence();
                         const uint32_t b_lo = b_lo0 + stage * OBJ16;
-                        // +32 B per K = 16 step inside the 128 B swizzle atom = +2 in descriptor address units; rows 64-127 of
-                        // the subject block start 8 KiB (+512) further
+                        // +32 B per K = 16 step inside the 128 B swizzle atom = +2 in descriptor address units
 #pragma unroll
                         for (int k = 0; k < 4; ++k) {
                             const uint32_t accum = (kb | k) != 0;
@@ -267,8 +362,6 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
                             wgmma_64x64<BF16>(acc[1], a_lo + 512 + 2 * k, b_lo + 2 * k, accum);
                         }
                         wgmma_commit();
-                        fence_acc(acc[0]);
-                        fence_acc(acc[1]);
                         if (++stage == (uint32_t)NS) {
                             stage = 0;
                             ph ^= 1;
@@ -284,18 +377,9 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
                     fence_acc(acc[1]);
                     ++done;
                     refill();
-                    // hand the quarter to the epilogue once its readers have taken the previous one
-                    mbar_wait(bar_qempty, (n_store & 1) ^ 1);
-#pragma unroll
-                    for (int mh = 0; mh < 2; ++mh)
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const uint32_t a = stg_w + (uint32_t)((mh * 64 * STG_STRIDE + 8 * j) * 4);
-                            sts_v2(a, acc[mh][4 * j], __float_as_uint(acc[mh][4 * j + 1]));
-                            sts_v2(a + 8 * STG_STRIDE * 4, acc[mh][4 * j + 2], __float_as_uint(acc[mh][4 * j + 3]));
-                        }
-                    mbar_arrive(bar_qfull + 8 * q);
-                    ++n_store;
+                    const uint32_t qf = bar_qfull + 16 * (qi & 3), par = (n_store & 1) ^ 1;
+                    store_half(acc[0], stg_w, bar_qempty, par, qf);
+                    store_half(acc[1], stg_w1, bar_qempty + 8, par, qf + 8);
                 }
             }
         }
@@ -311,7 +395,9 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
         const uint32_t thr_row = pin(smem_u32(sThr + wrow0 + lane));  // + l * 128 * 8: the threads of this row, [NLIST]: peers
         const uint32_t my_thr = pin(thr_row + (uint32_t)colg * (TILE_M * 8));
         const uint32_t stg_r = pin(smem_u32(sStg) + (uint32_t)((wrow0 + lane) * STG_STRIDE * 4));
-        const uint32_t qfull0 = pin(bar_qfull + (uint32_t)colg * 8), qempty = pin(bar_qempty);
+        // the m-half of the staging buffer that holds this warp's rows: quarters 0, 1 -> half 0; 2, 3 -> half 1
+        const uint32_t half = (uint32_t)quarter >> 1;
+        const uint32_t qfull0 = pin(bar_qfull + (uint32_t)colg * 16 + half * 8), qempty = pin(bar_qempty + half * 8);
         const bool lane0 = pin((uint32_t)lane) == 0;
         const uint32_t n_pos = (uint32_t)p.n_pos;
         const int kc = p.k_cand;  // (<= SLOTS, guaranteed by the host; a visible bound makes the compiler unroll the list scans fully and spill)
@@ -406,7 +492,7 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
                 const bool last = (it + 1 == nt);
 #pragma unroll
                 for (int s = 0; s < NQ; ++s) {
-                    mbar_wait(qfull0 + (uint32_t)(s * NLIST * 8), tpar);
+                    mbar_wait(qfull0 + (uint32_t)(s * NLIST * 16), tpar);
                     uint32_t r[QUART_N];
                     if (!dbg_skip) stage_ld(stg_r, r);
                     __syncwarp();

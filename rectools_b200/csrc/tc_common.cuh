@@ -124,20 +124,22 @@ constexpr uint32_t SMEM_DESC_HI = (1024u >> 4) | (1u << 30);
 __device__ __forceinline__ void mma_group_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-// Pin the accumulator registers at this point of the instruction stream: without it the compiler may copy an
-// accumulator while its wgmma is still in flight and feed the stale copy to the next wgmma or to a store.
+// Pin the accumulator registers at this point of the instruction stream (before wgmma.fence, after wgmma.wait_group:
+// never while a wgmma that writes them is in flight, or ptxas drains the pipe there).  The accumulators are b32
+// registers from the wgmma to the staging store, so no type conversion ever copies one.
 template <int N>
-__device__ __forceinline__ void fence_acc(float (&r)[N]) {
+__device__ __forceinline__ void fence_acc(uint32_t (&r)[N]) {
 #pragma unroll
-    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+    for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
 }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() {
     asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 // D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, both operands K-major in shared memory, fp32 accumulators in registers
-// (warp w of the warp group, lane l holds rows 16 w + l / 4 (+ 8) and columns 8 j + 2 (l % 4) (+ 1) of D).
-#define B200_F8(a, n) "+f"(a[n]), "+f"(a[n + 1]), "+f"(a[n + 2]), "+f"(a[n + 3]), "+f"(a[n + 4]), "+f"(a[n + 5]), "+f"(a[n + 6]), "+f"(a[n + 7])
+// (warp w of the warp group, lane l holds rows 16 w + l / 4 (+ 8) and columns 8 j + 2 (l % 4) (+ 1) of D).  The fp32
+// accumulators are bound as b32 registers ("+r"), the type the staging store reads them in.
+#define B200_F8(a, n) "+r"(a[n]), "+r"(a[n + 1]), "+r"(a[n + 2]), "+r"(a[n + 3]), "+r"(a[n + 4]), "+r"(a[n + 5]), "+r"(a[n + 6]), "+r"(a[n + 7])
 #define B200_WGMMA_64x64(TYPE)                                                                                              \
     asm volatile(                                                                                                           \
         "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"                                                                       \
@@ -151,7 +153,7 @@ __device__ __forceinline__ void wgmma_wait() {
         : "r"(a_lo), "r"(b_lo), "r"(SMEM_DESC_HI), "r"(accum))
 // (the operand type is a template parameter: a run-time branch around each wgmma makes ptxas serialise the pipeline)
 template <bool BF16>
-__device__ __forceinline__ void wgmma_64x64(float (&d)[32], uint32_t a_lo, uint32_t b_lo, uint32_t accum) {
+__device__ __forceinline__ void wgmma_64x64(uint32_t (&d)[32], uint32_t a_lo, uint32_t b_lo, uint32_t accum) {
     if constexpr (BF16)
         B200_WGMMA_64x64("bf16");
     else
@@ -197,6 +199,9 @@ __device__ __forceinline__ void sts_f32(uint32_t a, float v) { asm volatile("st.
 __device__ __forceinline__ void sts_s32(uint32_t a, int v) { asm volatile("st.shared.s32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
 __device__ __forceinline__ void sts_v2(uint32_t a, float x, uint32_t y) {
     asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(a), "r"(__float_as_uint(x)), "r"(y) : "memory");
+}
+__device__ __forceinline__ void sts_v2(uint32_t a, uint32_t x, uint32_t y) {
+    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(a), "r"(x), "r"(y) : "memory");
 }
 __device__ __forceinline__ void lds_v2(uint32_t a, float& x, uint32_t& y) {
     uint32_t xb;
