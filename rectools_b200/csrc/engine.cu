@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "../../include/b200_rank.h"
+#include "plan.h"
 #include "common.cuh"
 #include "prep.cuh"
 #include "select.cuh"
@@ -103,13 +104,6 @@ bool make_tensor_map(CUtensorMap* tm, const void* base, int64_t rows, int d_pad,
     return r == CUDA_SUCCESS;
 }
 
-inline int64_t round_up(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
-
-int env_int(const char* name, int dflt) {
-    const char* v = getenv(name);
-    return v ? atoi(v) : dflt;
-}
-
 }  // namespace
 
 struct b200_rank_engine {
@@ -125,7 +119,9 @@ struct b200_rank_engine {
     int64_t n_obj_pad = 0;
     cudaStream_t st = nullptr;
     cudaStream_t cs = nullptr;          // copy stream of the chunk pipeline
-    cudaEvent_t ev[8] = {nullptr};
+    // a call's timing (begin, first chunk's inputs staged, last chunk ranked, end) and its hand-over from / to the caller's stream
+    cudaEvent_t ev_begin = nullptr, ev_staged = nullptr, ev_ranked = nullptr, ev_end = nullptr;
+    cudaEvent_t ev_from_user = nullptr, ev_to_user = nullptr;
     cudaEvent_t evp[3] = {nullptr};     // chunk pipeline: inputs of chunk c / c+1 staged, stream hand-over
     std::vector<cudaEvent_t> evt;       // timing pairs of the fused-kernel / selection launches of a call
 
@@ -173,6 +169,7 @@ struct b200_rank_engine {
                 &cand_ids, &cand_counts, &cand_thr, &part_scores, &part_ids, &fb_rows, &scratch, &excl, &carousel, &patch,
                 &snap_scores, &snap_ids, &snap_counts, &snap_thr, &snap_row_exp, &snap_rows, &snap_fb};
     }
+    std::vector<cudaEvent_t*> call_events() { return {&ev_begin, &ev_staged, &ev_ranked, &ev_end, &ev_from_user, &ev_to_user}; }
     size_t hbm_bytes() {
         size_t t = 0;
         for (auto* b : all_bufs()) t += b->cap;
@@ -184,8 +181,8 @@ struct b200_rank_engine {
         for (auto* b : all_bufs()) b->release();
         if (h_pinned) cudaFreeHost(h_pinned);
         h_pinned = nullptr;
-        for (auto& e : ev)
-            if (e) cudaEventDestroy(e);
+        for (auto* e : call_events())
+            if (*e) cudaEventDestroy(*e);
         for (auto& e : evp)
             if (e) cudaEventDestroy(e);
         for (auto& e : evt)
@@ -263,6 +260,35 @@ TcPlan plan_fused(int d_pad) {
     return pl;
 }
 
+// The instantiations of the fused kernel: the function (for its attributes) and a launcher.
+template <int NW, bool WIDE, bool PEERS, bool BF16>
+void launch_fused(int grid, int smem, cudaStream_t st, const CUtensorMap& tm_sub, const CUtensorMap& tm_obj, const tc::TcParams& tp) {
+    tc::fused_topk_kernel<NW, WIDE, PEERS, BF16><<<grid, tc::FusedCfg<NW>::threads(PEERS), smem, st>>>(tm_sub, tm_obj, tp);
+}
+
+struct FusedKernel {
+    const void* fn;
+    decltype(&launch_fused<8, false, false, false>) launch;
+};
+
+template <int NW, bool WIDE, bool PEERS, bool BF16>
+FusedKernel fused_entry() {
+    return {(const void*)tc::fused_topk_kernel<NW, WIDE, PEERS, BF16>, launch_fused<NW, WIDE, PEERS, BF16>};
+}
+
+// [nw == 16][bf16][plain, wide, peers]
+const FusedKernel FUSED_KERNELS[2][2][3] = {
+    {{fused_entry<8, false, false, false>(), fused_entry<8, true, false, false>(), fused_entry<8, false, true, false>()},
+     {fused_entry<8, false, false, true>(), fused_entry<8, true, false, true>(), fused_entry<8, false, true, true>()}},
+    {{fused_entry<16, false, false, false>(), fused_entry<16, true, false, false>(), fused_entry<16, false, true, false>()},
+     {fused_entry<16, false, false, true>(), fused_entry<16, true, false, true>(), fused_entry<16, false, true, true>()}},
+};
+
+// Wide wins over peers: no kernel has both (threshold sharing needs k <= 24, the wide mode k > 24).
+const FusedKernel& fused_kernel(int nw, bool wide, bool peers, bool bf16) {
+    return FUSED_KERNELS[nw == 16][bf16][wide ? 1 : peers ? 2 : 0];
+}
+
 int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int64_t n_objects, int32_t d, int32_t distance,
                 int32_t device, int32_t tc_mode, int32_t flags) {
     if (!out) return fail(B200_E_INVALID, "b200_rank_create: out is NULL");
@@ -302,7 +328,7 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
         E->d_pad = (int)round_up(d, tc::KBLK);
         CK(cudaStreamCreateWithFlags(&E->st, cudaStreamNonBlocking));
         CK(cudaStreamCreateWithFlags(&E->cs, cudaStreamNonBlocking));
-        for (auto& e : E->ev) CK(cudaEventCreate(&e));
+        for (auto* e : E->call_events()) CK(cudaEventCreate(e));
         for (auto& e : E->evp) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         CK(cudaMallocHost(&E->h_pinned, 256));
         if ((flags & B200_F_OBJECTS_ON_DEVICE) && dtype == B200_DT_F32) {
@@ -330,17 +356,10 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
             if (!p8.ok || !p16.ok) {
                 E->tc_dtype = B200_TC_OFF;
             } else {
-                auto allow = [](const void* f, int bytes) { CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)); };
-#define B200_ALLOW(NW_, PL_)                                                                                        \
-    allow((const void*)tc::fused_topk_kernel<NW_, false, false, false>, PL_.smem_bytes);                            \
-    allow((const void*)tc::fused_topk_kernel<NW_, true, false, false>, PL_.smem_bytes);                             \
-    allow((const void*)tc::fused_topk_kernel<NW_, false, true, false>, PL_.smem_bytes);                             \
-    allow((const void*)tc::fused_topk_kernel<NW_, false, false, true>, PL_.smem_bytes);                             \
-    allow((const void*)tc::fused_topk_kernel<NW_, true, false, true>, PL_.smem_bytes);                              \
-    allow((const void*)tc::fused_topk_kernel<NW_, false, true, true>, PL_.smem_bytes)
-                B200_ALLOW(8, p8);
-                B200_ALLOW(16, p16);
-#undef B200_ALLOW
+                for (int w = 0; w < 2; ++w)
+                    for (const auto& by_type : FUSED_KERNELS[w])
+                        for (const FusedKernel& k : by_type)
+                            CK(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (w ? p16 : p8).smem_bytes));
             }
         }
         CK(cudaFuncSetAttribute(rescore_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
@@ -357,51 +376,32 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
     return B200_OK;
 }
 
-// Wide mode: T = the candidates a row is expected to collect, and the slots of each of its `nlist` append lists.  The
-// threshold frozen after a fraction q of the stream is about the (lists x K' - 6)-th best of that fraction, i.e. rank
-// ~ (lists x K' - 6) / q overall, so q follows from T.  k <= 128: T = 1.35 k + 40 (K' = 24), at most WIDE_MAX slots per row.
-// k > 128: T = 1.6 k + 64 (K' = 32), at most WIDE_MAX_L slots per row -- the frozen threshold is an order statistic of
-// ~58 samples, and this margin keeps the rows with fewer than k candidates (or an overflowing list) near 0.3 % (DESIGN 3.4).
-struct WideGeom {
-    double T;
-    int cand_stride;
-};
-
-WideGeom wide_geom(int kp, int nlist) {
-    WideGeom g;
-    if (kp <= 128) {
-        g.T = env_int("B200_WIDE_T", (int)(1.35 * kp + 40));
-        g.cand_stride = (int)round_up((int64_t)(g.T / nlist * 1.5 + 32), 8);
-        g.cand_stride = std::min(g.cand_stride, WIDE_MAX / nlist);
-    } else {
-        g.T = env_int("B200_WIDE_T", (int)(1.6 * kp + 64));
-        g.cand_stride = (int)round_up((int64_t)(g.T / nlist * 1.5 + 32), 8);
-        g.cand_stride = std::min(g.cand_stride, WIDE_MAX_L / nlist);
-    }
-    return g;
-}
-
 // Everything one b200_rank_topk call needs, so that the passes below can be plain functions.
 struct Call {
     b200_rank_engine* E;
     const b200_rank_query* q;
+    Hooks hooks;
+    CallPlan plan;
     b200_rank_stats S;
     cudaStream_t st;
     int64_t n_rows, n_pos;
     int k_out, d;
+    bool in_dev, out_dev;
     // whole-call device views (absolute rows)
     const float* sub32 = nullptr;
     const int64_t* rowmap = nullptr;
     const int64_t* indptr = nullptr;
     const int32_t* indices = nullptr;
     const int32_t* wl = nullptr;
+    const int64_t* sp_indptr = nullptr;  // sparse subjects
+    const int32_t* sp_indices = nullptr;
+    const float* sp_data = nullptr;
     int32_t *o_ids = nullptr, *o_counts = nullptr;
     float *o_scores = nullptr, *o_bounds = nullptr;
+    // failure lists (absolute rows) of the main pass, of one re-rank pass and of its second chance, and their counters
+    int32_t *fb_main = nullptr, *fb_pass = nullptr, *fb_second = nullptr, *cnt = nullptr;
     bool wl_gathered = false;
-    bool bf16 = false;
-    int nw = 8;  // epilogue warps of the main pass
     int n_tc = 0;       // fused-kernel launches so far
-    int snap_at = 0;    // B200_TC_SNAPSHOT: the launch whose state is copied (0: none)
     size_t n_evt = 0;
     std::vector<int> evt_kind;  // 0 = fused kernel, 1 = selection
 
@@ -510,9 +510,9 @@ struct TcPass {
     int32_t* o_counts = nullptr;
     float* o_bounds = nullptr;  // shared-threshold mode: bounds out, no verdict
     int nw = 8;                 // epilogue warps
-    int kc = 12;                // K' per list
+    int kc = 12;                // K' per list (<= the kernel's list capacity)
     int k0 = 0, kp = 0;         // this pass produces entries [k0, k0 + kp)
-    bool wide = false;          // single-pass wide mode (frozen threshold + global append)
+    TcMode mode = TcMode::NARROW;  // WIDE / WIDE_L: the plan's single wide pass (frozen threshold + global append)
     bool peers = false;         // share thresholds with the other ranks
     int64_t row0 = 0;           // absolute row of batch row 0 (failure list entries, peer arrays)
     int32_t* fb_list = nullptr;
@@ -558,9 +558,9 @@ void take_snapshot(Call& c, const TcPass& t, const tc::TcParams& tp, int nw, flo
     m.k_cand = tp.k_cand;
     m.k0 = t.k0;
     m.kp = t.kp;
-    m.wide = t.wide ? 1 : 0;
+    m.wide = t.mode != TcMode::NARROW ? 1 : 0;
     m.phase1_tiles = tp.phase1_tiles;
-    m.bf16 = c.bf16 ? 1 : 0;
+    m.bf16 = c.plan.bf16 ? 1 : 0;
     m.obj_exp = E->obj_exp;
     m.eps_rel = eps_rel;
     m.max_obj_norm = E->max_obj_norm;
@@ -571,10 +571,10 @@ void take_snapshot(Call& c, const TcPass& t, const tc::TcParams& tp, int nw, flo
 void run_tc(Call& c, const TcPass& t) {
     b200_rank_engine* E = c.E;
     cudaStream_t st = c.st;
-    const bool bf16 = c.bf16;
+    const bool bf16 = c.plan.bf16;
+    const bool wide = t.mode != TcMode::NARROW;
     const int d = c.d;
     const int nlist = t.nw / 4;
-    const int slots = 64 / nlist;
     const TcPlan pl = t.nw == 8 ? plan_fused<8>(E->d_pad) : plan_fused<16>(E->d_pad);
     const int64_t rows_pad = round_up(t.n_sel, 2 * tc::TILE_M);
     // subjects -> 16-bit, per-row power-of-two scale
@@ -616,29 +616,13 @@ void run_tc(Call& c, const TcPass& t) {
     tc::TcParams tp{};
     tp.kblocks = pl.kblocks;
     tp.n_stages = pl.n_stages;
-    tp.k_cand = std::min(t.kc, slots);
+    tp.k_cand = t.kc;
     tp.n_rows = t.n_sel;
     tp.n_pos = c.n_pos;
     tp.n_row_tiles = (int)(rows_pad / (2 * tc::TILE_M));
     tp.n_obj_tiles = (int)((c.n_pos + tc::TILE_N - 1) / tc::TILE_N);
-    // object splits: fill the machine when there are few row tiles, even out the last wave otherwise
-    int best_splits = 1;
-    double best_eff = -1.0;
-    const int max_splits = t.wide ? 1 : std::max(1, std::min(16, tp.n_obj_tiles * 2 / 32));
     const int n_units = E->sm_count / 2;  // CTA pairs working concurrently
-    for (int s = 1; s <= max_splits; ++s) {
-        const double work = (double)tp.n_row_tiles * s;
-        const double waves = std::ceil(work / n_units);
-        const double eff = work / (waves * n_units) - 0.01 * (s - 1);
-        if (eff > best_eff + 1e-9) {
-            best_eff = eff;
-            best_splits = s;
-        }
-    }
-    {
-        const int forced = env_int("B200_TC_SPLITS", 0);  // tuning / test hook
-        if (forced >= 1 && forced <= max_splits) best_splits = forced;
-    }
+    const int best_splits = choose_splits(tp.n_row_tiles, tp.n_obj_tiles, n_units, wide, c.hooks.tc_splits);
     tp.n_splits = best_splits;
     tp.tiles_per_split = (tp.n_obj_tiles + best_splits - 1) / best_splits;
     tp.pos2obj = c.wl;
@@ -655,8 +639,8 @@ void run_tc(Call& c, const TcPass& t) {
     // wide mode: the lists hold ~T candidates per row (wide_geom)
     int cand_stride = 32;
     tp.phase1_tiles = 0x7fffffff;
-    if (t.wide) {
-        const WideGeom g = wide_geom(t.kp, nlist);
+    if (wide) {
+        const WideGeom& g = c.plan.geom;
         const double rank_frozen = nlist * tp.k_cand - 6;
         const double qf = std::min(1.0, rank_frozen / g.T);
         tp.phase1_tiles = std::max(1, (int)std::ceil(qf * tp.tiles_per_split));
@@ -672,7 +656,7 @@ void run_tc(Call& c, const TcPass& t) {
     tp.cand_counts = E->cand_counts.as<int32_t>();
     tp.cand_thr = E->cand_thr.as<float>();
     tp.rows_pad = rows_pad;
-    tp.debug_mode = env_int("B200_TC_DEBUG", 0);  // measurement hook, results are invalid
+    tp.debug_mode = c.hooks.tc_debug;
     if (t.peers) {
         tp.n_peers = E->n_peers;
         tp.peer_epoch = c.q->peer_epoch;
@@ -681,14 +665,9 @@ void run_tc(Call& c, const TcPass& t) {
         tp.peer_pub = E->peer_pub.as<unsigned long long>();
         for (int i = 0; i < E->n_peers; ++i) tp.peer_in[i] = reinterpret_cast<const unsigned long long*>(E->peer_in[i]);
     }
-    if (t.main) {
-        c.S.n_splits = best_splits;
-        c.S.k_cand = tp.k_cand;
-        c.S.epi_warps = t.nw;
-        c.S.wide = t.wide ? 1 : 0;
-    }
+    if (t.main) c.S.n_splits = best_splits;
     const int n_work = tp.n_row_tiles * tp.n_splits;
-    if (env_int("B200_TC_CAROUSEL", 1) != 0) {  // 0: every work item starts at its first object tile
+    if (c.hooks.tc_carousel != 0) {
         const int n_pairs_run = std::min(n_work, n_units);
         const int per_pair = (n_work + n_pairs_run - 1) / n_pairs_run;
         const int64_t n_ints = (int64_t)best_splits + (int64_t)n_pairs_run * per_pair;
@@ -701,30 +680,13 @@ void run_tc(Call& c, const TcPass& t) {
         tp.starts_stride = per_pair;
     }
     const int grid = 2 * std::min(n_work, n_units);
-    const bool snap = ++c.n_tc == c.snap_at;
+    const bool snap = ++c.n_tc == c.hooks.tc_snapshot;
     if (snap) {
         E->snap_fb.ensure(sizeof(int32_t) * (size_t)(c.n_rows + 2));
         CK(cudaMemcpyAsync(E->snap_fb.p, t.fb_count, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
     }
     c.time_begin(0);
-    const bool use_peers = t.peers && tp.n_peers > 0;  // (wide mode and threshold sharing never meet: sharing needs k <= 24)
-#define B200_LAUNCH(NW_, WIDE_, PEERS_)                                                                                              \
-    do {                                                                                                                       \
-        if (bf16)                                                                                                              \
-            tc::fused_topk_kernel<NW_, WIDE_, PEERS_, true><<<grid, tc::FusedCfg<NW_>::threads(PEERS_), pl.smem_bytes, st>>>(tm_sub, tm_obj, tp); \
-        else                                                                                                                   \
-            tc::fused_topk_kernel<NW_, WIDE_, PEERS_, false><<<grid, tc::FusedCfg<NW_>::threads(PEERS_), pl.smem_bytes, st>>>(tm_sub, tm_obj, tp); \
-    } while (0)
-    if (t.nw == 8) {
-        if (t.wide) B200_LAUNCH(8, true, false);
-        else if (use_peers) B200_LAUNCH(8, false, true);
-        else B200_LAUNCH(8, false, false);
-    } else {
-        if (t.wide) B200_LAUNCH(16, true, false);
-        else if (use_peers) B200_LAUNCH(16, false, true);
-        else B200_LAUNCH(16, false, false);
-    }
-#undef B200_LAUNCH
+    fused_kernel(t.nw, wide, t.peers && tp.n_peers > 0, bf16).launch(grid, pl.smem_bytes, st, tm_sub, tm_obj, tp);
     CK(cudaGetLastError());
     c.time_end();
     c.S.n_launches++;
@@ -763,9 +725,9 @@ void run_tc(Call& c, const TcPass& t) {
     sp.fb_row0 = t.rows_dev ? 0 : t.row0;
     sp.out_bounds = t.o_bounds;
     c.time_begin(1);
-    if (t.wide && t.kp > 128) {
+    if (t.mode == TcMode::WIDE_L) {
         rescore_wide_large_kernel<<<(unsigned)t.n_sel, WIDE_THREADS_L, wide_large_smem(d), st>>>(sp);
-    } else if (t.wide) {
+    } else if (wide) {
         rescore_wide_kernel<<<(unsigned)t.n_sel, WIDE_THREADS, (size_t)d * sizeof(float), st>>>(sp);
     } else {
         const size_t sel_smem = (size_t)SEL_WARPS * d * sizeof(float);
@@ -847,10 +809,345 @@ void run_dense_large_k(Call& c, const int32_t* rows, const float* sub32, const i
     }
 }
 
-int32_t read_counter(Call& c, const int32_t* dev) {
-    CK(cudaMemcpyAsync(c.E->h_pinned, dev, sizeof(int32_t), cudaMemcpyDeviceToHost, c.st));
+// a device-memory scalar, read after everything queued on the engine stream
+template <typename T>
+T read_scalar(b200_rank_engine* E, const T* dev) {
+    T v;
+    CK(cudaMemcpyAsync(E->h_pinned, dev, sizeof(T), cudaMemcpyDeviceToHost, E->st));
+    CK(cudaStreamSynchronize(E->st));
+    memcpy(&v, E->h_pinned, sizeof(T));
+    return v;
+}
+
+// indptr[n_rows] of a CSR array in host or (in_dev) device memory
+int64_t read_nnz(b200_rank_engine* E, const int64_t* indptr, int64_t n_rows, bool in_dev) {
+    return in_dev ? read_scalar(E, indptr + n_rows) : indptr[n_rows];
+}
+
+// The checks of a query that need neither the device nor the engine lock (B200_OK: none failed).
+int validate_query(const b200_rank_engine* E, const b200_rank_query* q) {
+    if (!E || !q) return fail(B200_E_INVALID, "b200_rank_topk: NULL argument");
+    if (q->n_rows < 0) return fail(B200_E_INVALID, "b200_rank_topk: n_rows < 0");
+    if (q->k <= 0) return fail(B200_E_INVALID, "b200_rank_topk: k must be positive");
+    const bool sparse_sub = q->sub_indptr != nullptr;
+    if (!sparse_sub && !q->subjects && !q->subject_ids) return fail(B200_E_INVALID, "b200_rank_topk: neither subjects nor subject_ids given");
+    if (sparse_sub && (q->subjects || q->subject_ids)) return fail(B200_E_INVALID, "b200_rank_topk: sparse subjects exclude subjects / subject_ids");
+    if (sparse_sub && E->distance != B200_DIST_DOT)
+        return fail(B200_E_INVALID, "b200_rank_topk: sparse subjects need B200_DIST_DOT (rank_implicit.py:66-67)");
+    if (!sparse_sub && !q->subjects && !E->sub32_res_ptr)
+        return fail(B200_E_INVALID, "b200_rank_topk: subject_ids given but b200_rank_set_subjects was never called");
+    if (q->subjects && q->subject_ids && q->n_subjects_total <= 0)
+        return fail(B200_E_INVALID, "b200_rank_topk: subjects + subject_ids need n_subjects_total");
+    if (q->whitelist && q->n_whitelist < 0) return fail(B200_E_INVALID, "b200_rank_topk: n_whitelist < 0");
+    if (q->n_rows > 0 && (!q->out_ids || !q->out_scores || !q->out_counts))
+        return fail(B200_E_INVALID, "b200_rank_topk: output pointers are NULL");
+    if (q->n_rows >= (1ll << 31) - 64) return fail(B200_E_UNSUPPORTED, "b200_rank_topk: more than 2^31 rows per call");
+    if ((q->flags & B200_Q_FORCE_EXACT) && (q->flags & B200_Q_FORCE_TC))
+        return fail(B200_E_INVALID, "b200_rank_topk: FORCE_EXACT and FORCE_TC are exclusive");
+    const bool in_dev = q->flags & B200_Q_INPUTS_ON_DEVICE;
+    const bool shared = q->flags & B200_Q_SHARED_THRESHOLDS;
+    if (q->subject_dtype != B200_DT_F32 && !(in_dev && q->subjects && !q->subject_ids))
+        return fail(B200_E_INVALID, "b200_rank_topk: 16-bit subjects must be a device matrix in batch order");
+    if (q->subject_dtype < B200_DT_F32 || q->subject_dtype > B200_DT_BF16) return fail(B200_E_INVALID, "b200_rank_topk: bad subject_dtype");
+    if (shared && (!q->out_bounds || q->peer_epoch == 0))
+        return fail(B200_E_INVALID, "b200_rank_topk: B200_Q_SHARED_THRESHOLDS needs out_bounds and peer_epoch >= 1");
+    if (shared && sparse_sub) return fail(B200_E_UNSUPPORTED, "b200_rank_topk: sparse subjects cannot share thresholds");
+    return B200_OK;
+}
+
+// Host inputs of a large call are staged in row chunks on a second stream: the copy of chunk c+1 (subject rows / ids,
+// its slice of the CSR filter) and the copy-back of chunk c-1 run while chunk c is being ranked.  Buffers are full-size
+// and addressed by absolute row / nnz offsets, so the kernels see the same layout with or without chunking.
+// stage_inputs copies the un-chunked items on the main stream and sizes the chunked ones, the outputs and the failure lists.
+void stage_inputs(Call& c, int64_t sp_nnz, int64_t f_nnz) {
+    b200_rank_engine* E = c.E;
+    const b200_rank_query* q = c.q;
+    const int64_t n_rows = c.n_rows;
+    const int d = c.d;
+    auto stage = [&](DevBuf& buf, const void* src, size_t bytes) -> const void* {
+        if (c.in_dev) return src;
+        buf.ensure(std::max<size_t>(bytes, 16));
+        if (bytes) CK(cudaMemcpyAsync(buf.p, src, bytes, cudaMemcpyHostToDevice, c.st));
+        c.S.h2d_bytes += (int64_t)bytes;
+        return buf.p;
+    };
+    if (q->sub_indptr) {
+        c.sp_indptr = (const int64_t*)stage(E->sp_indptr, q->sub_indptr, sizeof(int64_t) * (n_rows + 1));
+        c.sp_indices = (const int32_t*)stage(E->sp_indices, q->sub_indices, sizeof(int32_t) * sp_nnz);
+        c.sp_data = (const float*)stage(E->sp_data, q->sub_data, sizeof(float) * sp_nnz);
+    } else if (q->subjects) {
+        const int64_t rows_in = q->subject_ids ? q->n_subjects_total : n_rows;
+        if (q->subject_dtype != B200_DT_F32) {
+            E->sub32.ensure(sizeof(float) * rows_in * d);
+            widen16_kernel<<<grid_for(rows_in * d, 256), 256, 0, c.st>>>(q->subjects, q->subject_dtype == B200_DT_BF16 ? 1 : 0, rows_in * d,
+                                                                         E->sub32.as<float>());
+            CK(cudaGetLastError());
+            c.S.n_launches++;
+            c.sub32 = E->sub32.as<float>();
+        } else if (!q->subject_ids && !c.in_dev) {  // rows in batch order: chunked (stage_rows)
+            E->sub32.ensure(std::max<size_t>(sizeof(float) * rows_in * d, 16));
+            c.sub32 = E->sub32.as<float>();
+        } else {
+            c.sub32 = (const float*)stage(E->sub32, q->subjects, sizeof(float) * rows_in * d);
+        }
+    } else {
+        c.sub32 = E->sub32_res_ptr;
+    }
+    if (q->subject_ids) {
+        if (c.in_dev) {
+            c.rowmap = q->subject_ids;
+        } else {
+            E->rowmap.ensure(std::max<size_t>(sizeof(int64_t) * n_rows, 16));
+            c.rowmap = E->rowmap.as<int64_t>();
+        }
+    }
+    if (q->csr_indptr) {
+        if (c.in_dev) {
+            c.indptr = q->csr_indptr;
+            c.indices = q->csr_indices;
+        } else {
+            E->indptr.ensure(sizeof(int64_t) * (n_rows + 1));
+            E->indices.ensure(std::max<size_t>(sizeof(int32_t) * f_nnz, 16));
+            c.indptr = E->indptr.as<int64_t>();
+            c.indices = E->indices.as<int32_t>();
+        }
+        if (f_nnz == 0) c.indptr = nullptr;  // an all-empty filter is no filter (cf. rank_implicit.py:169-173)
+    }
+    if (q->whitelist) c.wl = (const int32_t*)stage(E->wl, q->whitelist, sizeof(int32_t) * c.n_pos);
+
+    const bool shared = q->flags & B200_Q_SHARED_THRESHOLDS;
+    const int k_out = c.k_out;
+    if (c.out_dev) {
+        c.o_ids = q->out_ids;
+        c.o_scores = q->out_scores;
+        c.o_counts = q->out_counts;
+        c.o_bounds = shared ? q->out_bounds : nullptr;
+    } else {
+        E->out_ids.ensure(sizeof(int32_t) * n_rows * k_out);
+        E->out_scores.ensure(sizeof(float) * n_rows * k_out);
+        E->out_counts.ensure(sizeof(int32_t) * n_rows);
+        c.o_ids = E->out_ids.as<int32_t>();
+        c.o_scores = E->out_scores.as<float>();
+        c.o_counts = E->out_counts.as<int32_t>();
+        if (shared) {
+            E->out_bounds.ensure(sizeof(float) * n_rows);
+            c.o_bounds = E->out_bounds.as<float>();
+        }
+    }
+
+    E->fb_rows.ensure(sizeof(int32_t) * (3 * n_rows + 3));
+    c.fb_main = E->fb_rows.as<int32_t>();
+    c.fb_pass = c.fb_main + n_rows;
+    c.fb_second = c.fb_pass + n_rows;
+    c.cnt = c.fb_second + n_rows;  // [main pass, re-rank pass, second chance]
+    CK(cudaMemsetAsync(c.cnt, 0, 3 * sizeof(int32_t), c.st));
+    // exclusion lists of the re-rank passes after the first (k <= 24 takes one pass, k > 128 the path-3 kernels)
+    if (c.plan.tc() && k_out > 24 && k_out <= 128) E->excl.ensure(sizeof(int32_t) * (size_t)n_rows * k_out);
+}
+
+// host -> device copy of the chunked inputs of rows [r0, r1) on stream `s`
+void stage_rows(Call& c, int64_t r0, int64_t r1, cudaStream_t s) {
+    if (c.in_dev) return;
+    b200_rank_engine* E = c.E;
+    const b200_rank_query* q = c.q;
+    size_t bytes = 0;
+    auto h2d = [&](void* dst, const void* src, size_t n) {
+        if (n) CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, s));
+        bytes += n;
+    };
+    if (q->subjects && !q->subject_ids) h2d(E->sub32.as<float>() + r0 * c.d, q->subjects + r0 * c.d, sizeof(float) * (r1 - r0) * c.d);
+    if (q->subject_ids) h2d(E->rowmap.as<int64_t>() + r0, q->subject_ids + r0, sizeof(int64_t) * (r1 - r0));
+    if (c.indptr) {
+        h2d(E->indptr.as<int64_t>() + r0, q->csr_indptr + r0, sizeof(int64_t) * (r1 - r0 + 1));
+        const int64_t z0 = q->csr_indptr[r0], z1 = q->csr_indptr[r1];
+        if (z1 < z0) throw CudaError{cudaErrorInvalidValue, "csr_indptr must be non-decreasing", __LINE__};
+        h2d(E->indices.as<int32_t>() + z0, q->csr_indices + z0, sizeof(int32_t) * (z1 - z0));
+    }
+    c.S.h2d_bytes += (int64_t)bytes;
+}
+
+// device -> host copy of the results of rows [r0, r1) on stream `s`
+void copy_back(Call& c, int64_t r0, int64_t r1, cudaStream_t s) {
+    const b200_rank_query* q = c.q;
+    const int k_out = c.k_out;
+    CK(cudaMemcpyAsync(q->out_ids + r0 * k_out, c.o_ids + r0 * k_out, sizeof(int32_t) * (r1 - r0) * k_out, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(q->out_scores + r0 * k_out, c.o_scores + r0 * k_out, sizeof(float) * (r1 - r0) * k_out, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(q->out_counts + r0, c.o_counts + r0, sizeof(int32_t) * (r1 - r0), cudaMemcpyDeviceToHost, s));
+    c.S.d2h_bytes += (int64_t)((r1 - r0) * k_out * 8 + (r1 - r0) * 4);
+    if (c.o_bounds) {
+        CK(cudaMemcpyAsync(q->out_bounds + r0, c.o_bounds + r0, sizeof(float) * (r1 - r0), cudaMemcpyDeviceToHost, s));
+        c.S.d2h_bytes += (int64_t)(r1 - r0) * 4;
+    }
+}
+
+// Re-rank `n_sel` rows (absolute row numbers in `rows`) without any shortcut that could fail again unnoticed:
+// k <= 24: one pass with the widest lists (32 slots, 8-warp kernel), then the exhaustive kernel for what still fails;
+// k  > 24: certified passes of 20 results with exclusion lists, each followed by its own wide-list pass and the
+// exhaustive kernel.  Results are written with LOCAL ids; the caller applies the id offset.
+void rerank_rows(Call& c, const int32_t* rows, int64_t n_sel) {
+    b200_rank_engine* E = c.E;
+    const int k_out = c.k_out;
+    init_rows_kernel<<<grid_for(n_sel * k_out, 256), 256, 0, c.st>>>(c.o_ids, c.o_scores, c.o_counts, rows, n_sel, k_out);
+    CK(cudaGetLastError());
+    c.S.n_launches++;
+    const int k_pass = k_out <= 24 ? k_out : 20;
+    const int kc_pass = k_out <= 24 ? 32 : (c.plan.bf16 ? 30 : 25);
+    for (int k0 = 0; k0 < k_out; k0 += k_pass) {
+        const int kp = std::min(k_pass, k_out - k0);
+        if (k0 > 0) {
+            build_exclusion_kernel<<<grid_for(n_sel * 32, 256), 256, 0, c.st>>>(c.o_ids, rows, n_sel, k_out, k0, (int32_t)E->id_offset,
+                                                                               E->excl.as<int32_t>());
+            CK(cudaGetLastError());
+            c.S.n_launches++;
+        }
+        CK(cudaMemsetAsync(c.cnt + 1, 0, 2 * sizeof(int32_t), c.st));
+        TcPass t;
+        t.rows_dev = rows;
+        t.n_sel = n_sel;
+        t.sub32 = c.sub32;
+        t.rowmap = c.rowmap;
+        t.indptr = c.indptr;
+        t.o_ids = c.o_ids;
+        t.o_scores = c.o_scores;
+        t.o_counts = c.o_counts;
+        t.nw = 8;
+        t.kc = std::min(32, std::max(kc_pass - (k_pass - kp), kp));
+        t.k0 = k0;
+        t.kp = kp;
+        t.fb_list = c.fb_pass;
+        t.fb_count = c.cnt + 1;
+        run_tc(c, t);
+        int64_t n_fb = read_scalar(E, c.cnt + 1);
+        const int32_t* f = c.fb_pass;
+        if (n_fb > 0 && t.kc < 32) {  // the pass's own second chance: widest lists
+            TcPass t2 = t;
+            t2.rows_dev = c.fb_pass;
+            t2.n_sel = n_fb;
+            t2.kc = 32;
+            t2.fb_list = c.fb_second;
+            t2.fb_count = c.cnt + 2;
+            run_tc(c, t2);
+            n_fb = read_scalar(E, c.cnt + 2);
+            f = c.fb_second;
+        }
+        c.S.n_exact_rows += n_fb;
+        if (n_fb > 0) run_exact(c, f, n_fb, c.sub32, c.rowmap, c.indptr, c.o_ids, c.o_scores, c.o_counts, k0, k0 + kp, false);
+    }
+}
+
+// The main pass over rows [r0, r1) of the call, on the plan's path.
+void main_pass(Call& c, int64_t r0, int64_t r1) {
+    b200_rank_engine* E = c.E;
+    const CallPlan& P = c.plan;
+    const int k_out = c.k_out;
+    const int64_t nr = r1 - r0;
+    int32_t* oi = c.o_ids + r0 * k_out;
+    float* os = c.o_scores + r0 * k_out;
+    int32_t* oc = c.o_counts + r0;
+    const float* sub = (c.sub32 && !c.rowmap) ? c.sub32 + r0 * c.d : c.sub32;
+    const int64_t* rm = c.rowmap ? c.rowmap + r0 : nullptr;
+    const int64_t* ip = c.indptr ? c.indptr + r0 : nullptr;
+    const bool multi_pass = P.tc() && P.mode == TcMode::MULTI_PASS;
+    if (multi_pass) {  // every row takes the certified passes of the re-rank (one chunk)
+        iota_kernel<<<grid_for(nr, 256), 256, 0, c.st>>>(c.fb_main, nr);
+        CK(cudaGetLastError());
+        rerank_rows(c, c.fb_main, nr);
+    } else {
+        init_outputs_kernel<<<grid_for(std::max<int64_t>(nr * k_out, nr), 256), 256, 0, c.st>>>(oi, os, oc, nr, k_out);
+        CK(cudaGetLastError());
+        c.S.n_launches++;
+        if (P.path == Path::SPARSE) {
+            run_sparse(c, c.sp_indptr + r0, c.sp_indices, c.sp_data, nr, ip, oi, os, oc);
+        } else if (P.path == Path::DENSE_LARGE_K) {  // materialised exhaustive scores + streaming selection passes
+            run_dense_large_k(c, nullptr, sub, rm, ip, nr, oi, os, oc, true);
+        } else if (P.path == Path::EXACT) {
+            run_exact(c, nullptr, nr, sub, rm, ip, oi, os, oc, 0, k_out, true);
+        } else {
+            TcPass t;
+            t.n_sel = nr;
+            t.sub32 = sub;
+            t.rowmap = rm;
+            t.indptr = ip;
+            t.o_ids = oi;
+            t.o_scores = os;
+            t.o_counts = oc;
+            t.o_bounds = c.o_bounds ? c.o_bounds + r0 : nullptr;
+            t.nw = P.nw;
+            t.kc = P.k_cand;
+            t.mode = P.mode;
+            t.peers = P.peers;
+            t.row0 = r0;
+            t.fb_list = c.fb_main;
+            t.fb_count = c.cnt;
+            t.main = true;
+            t.kp = k_out;
+            run_tc(c, t);
+        }
+        if (c.o_bounds && !P.tc()) {  // exhaustive lists: nothing was discarded
+            fill_f32_kernel<<<grid_for(nr, 256), 256, 0, c.st>>>(c.o_bounds + r0, nr, -INFINITY);
+            CK(cudaGetLastError());
+        }
+    }
+    if (E->id_offset != 0) {
+        add_offset_kernel<<<grid_for(nr * k_out, 256), 256, 0, c.st>>>(oi, nr * k_out, (int32_t)E->id_offset);
+        CK(cudaGetLastError());
+        if (!multi_pass) c.S.n_launches++;  // (n_launches does not count the multi-pass route's iota and offset launches)
+    }
+}
+
+// Rows whose certificate failed in the main pass (all chunks): re-rank them and patch the results.  Host outputs get
+// packed copies of the patched rows (one more small transfer), scattered into the caller's arrays once every chunk's
+// copy-back on `cs` has landed.
+void rerank_failures(Call& c, cudaStream_t cs) {
+    b200_rank_engine* E = c.E;
+    const b200_rank_query* q = c.q;
+    const int k_out = c.k_out;
+    const int64_t n_fb = read_scalar(E, c.cnt);
+    c.S.n_fallback_rows = n_fb;
+    if (n_fb == 0) return;
+    if (k_out > 128) {  // the exhaustive kernels of path 3, over these rows only
+        init_rows_kernel<<<grid_for(n_fb * k_out, 256), 256, 0, c.st>>>(c.o_ids, c.o_scores, c.o_counts, c.fb_main, n_fb, k_out);
+        CK(cudaGetLastError());
+        c.S.n_launches++;
+        run_dense_large_k(c, c.fb_main, c.sub32, c.rowmap, c.indptr, n_fb, c.o_ids, c.o_scores, c.o_counts, false);
+        c.S.n_exact_rows += n_fb;
+    } else {
+        rerank_rows(c, c.fb_main, n_fb);
+    }
+    if (E->id_offset != 0) {
+        add_offset_rows_kernel<<<grid_for(n_fb * k_out, 256), 256, 0, c.st>>>(c.o_ids, c.fb_main, n_fb, k_out, (int32_t)E->id_offset);
+        CK(cudaGetLastError());
+        c.S.n_launches++;
+    }
+    if (c.out_dev) return;
+    const size_t row_bytes = (size_t)k_out * 8 + 8;
+    E->patch.ensure(row_bytes * n_fb);
+    int32_t* g_ids = E->patch.as<int32_t>();
+    float* g_sc = reinterpret_cast<float*>(g_ids + n_fb * k_out);
+    int32_t* g_cnt = reinterpret_cast<int32_t*>(g_sc + n_fb * k_out);
+    int32_t* g_rows = g_cnt + n_fb;
+    gather_rows_kernel<<<grid_for(n_fb * k_out, 256), 256, 0, c.st>>>(c.o_ids, c.o_scores, c.o_counts, c.fb_main, n_fb, k_out, g_ids, g_sc,
+                                                                     g_cnt);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(g_rows, c.fb_main, sizeof(int32_t) * n_fb, cudaMemcpyDeviceToDevice, c.st));
+    E->h_patch.resize(row_bytes * n_fb);
+    if (cs != c.st) {
+        CK(cudaEventRecord(E->evp[2], cs));
+        CK(cudaStreamWaitEvent(c.st, E->evp[2], 0));
+    }
+    CK(cudaMemcpyAsync(E->h_patch.data(), E->patch.p, row_bytes * n_fb, cudaMemcpyDeviceToHost, c.st));
     CK(cudaStreamSynchronize(c.st));
-    return c.E->h_pinned[0];
+    const int32_t* h_ids = reinterpret_cast<const int32_t*>(E->h_patch.data());
+    const float* h_sc = reinterpret_cast<const float*>(h_ids + n_fb * k_out);
+    const int32_t* h_cnt = reinterpret_cast<const int32_t*>(h_sc + n_fb * k_out);
+    const int32_t* h_rows = h_cnt + n_fb;
+    for (int64_t i = 0; i < n_fb; ++i) {
+        const int64_t r = h_rows[i];
+        memcpy(q->out_ids + r * k_out, h_ids + i * k_out, sizeof(int32_t) * k_out);
+        memcpy(q->out_scores + r * k_out, h_sc + i * k_out, sizeof(float) * k_out);
+        q->out_counts[r] = h_cnt[i];
+    }
+    c.S.d2h_bytes += (int64_t)(row_bytes * n_fb);
 }
 
 }  // namespace
@@ -971,510 +1268,105 @@ int b200_rank_peer_import(b200_rank_engine* E, int32_t n_ranks, int32_t self, co
 }
 
 int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stats* stats) {
-    if (!E || !q) return fail(B200_E_INVALID, "b200_rank_topk: NULL argument");
-    if (q->n_rows < 0) return fail(B200_E_INVALID, "b200_rank_topk: n_rows < 0");
-    if (q->k <= 0) return fail(B200_E_INVALID, "b200_rank_topk: k must be positive");
-    const bool sparse_sub = q->sub_indptr != nullptr;
-    if (!sparse_sub && !q->subjects && !q->subject_ids) return fail(B200_E_INVALID, "b200_rank_topk: neither subjects nor subject_ids given");
-    if (sparse_sub && (q->subjects || q->subject_ids)) return fail(B200_E_INVALID, "b200_rank_topk: sparse subjects exclude subjects / subject_ids");
-    if (sparse_sub && E->distance != B200_DIST_DOT)
-        return fail(B200_E_INVALID, "b200_rank_topk: sparse subjects need B200_DIST_DOT (rank_implicit.py:66-67)");
-    if (!sparse_sub && !q->subjects && !E->sub32_res_ptr)
-        return fail(B200_E_INVALID, "b200_rank_topk: subject_ids given but b200_rank_set_subjects was never called");
-    if (q->subjects && q->subject_ids && q->n_subjects_total <= 0)
-        return fail(B200_E_INVALID, "b200_rank_topk: subjects + subject_ids need n_subjects_total");
-    if (q->whitelist && q->n_whitelist < 0) return fail(B200_E_INVALID, "b200_rank_topk: n_whitelist < 0");
-    if (q->n_rows > 0 && (!q->out_ids || !q->out_scores || !q->out_counts))
-        return fail(B200_E_INVALID, "b200_rank_topk: output pointers are NULL");
-    if (q->n_rows >= (1ll << 31) - 64) return fail(B200_E_UNSUPPORTED, "b200_rank_topk: more than 2^31 rows per call");
-    if ((q->flags & B200_Q_FORCE_EXACT) && (q->flags & B200_Q_FORCE_TC))
-        return fail(B200_E_INVALID, "b200_rank_topk: FORCE_EXACT and FORCE_TC are exclusive");
-    const bool in_dev = q->flags & B200_Q_INPUTS_ON_DEVICE;
-    const bool out_dev = q->flags & B200_Q_OUTPUTS_ON_DEVICE;
-    const bool shared = q->flags & B200_Q_SHARED_THRESHOLDS;
-    if (q->subject_dtype != B200_DT_F32 && !(in_dev && q->subjects && !q->subject_ids))
-        return fail(B200_E_INVALID, "b200_rank_topk: 16-bit subjects must be a device matrix in batch order");
-    if (q->subject_dtype < B200_DT_F32 || q->subject_dtype > B200_DT_BF16) return fail(B200_E_INVALID, "b200_rank_topk: bad subject_dtype");
-    if (shared && (!q->out_bounds || q->peer_epoch == 0))
-        return fail(B200_E_INVALID, "b200_rank_topk: B200_Q_SHARED_THRESHOLDS needs out_bounds and peer_epoch >= 1");
-    if (shared && sparse_sub) return fail(B200_E_UNSUPPORTED, "b200_rank_topk: sparse subjects cannot share thresholds");
-
+    if (const int rc = validate_query(E, q)) return rc;
     std::lock_guard<std::mutex> lock(E->mu);
+    E->snap.valid = 0;
     Call c{};
     c.E = E;
     c.q = q;
     memset(&c.S, 0, sizeof(c.S));
-    c.snap_at = env_int("B200_TC_SNAPSHOT", 0);  // test hook, see b200_rank_get_snapshot
-    E->snap.valid = 0;
     b200_rank_stats& S = c.S;
-    const int64_t n_rows = q->n_rows;
-    const int64_t n_pos = q->whitelist ? q->n_whitelist : E->n_obj;
-    const int k_out = (int)std::min<int64_t>(q->k, n_pos);
-    S.k_out = k_out;
-    const int d = E->d;
-    c.n_rows = n_rows;
-    c.n_pos = n_pos;
-    c.k_out = k_out;
-    c.d = d;
-    if (n_rows == 0 || k_out <= 0) {
+    c.n_rows = q->n_rows;
+    c.n_pos = q->whitelist ? q->n_whitelist : E->n_obj;
+    c.d = E->d;
+    c.in_dev = q->flags & B200_Q_INPUTS_ON_DEVICE;
+    c.out_dev = q->flags & B200_Q_OUTPUTS_ON_DEVICE;
+    const CallShape shape{c.n_rows, c.n_pos, q->k, E->d, E->d_pad, E->sm_count, E->tc_dtype, E->n_peers, q->flags, q->sub_indptr != nullptr};
+    c.hooks = read_hooks();
+    c.plan = plan_call(shape, c.hooks);
+    const CallPlan& P = c.plan;
+    S.k_out = c.k_out = P.k_out;
+    if (c.n_rows == 0 || c.k_out <= 0) {
         if (stats) *stats = S;
         return B200_OK;
     }
-    if (shared && E->n_peers > 0 && n_rows > E->peer_rows)
-        return fail(B200_E_INVALID, "b200_rank_topk: %lld rows exceed the %lld exported for threshold sharing", (long long)n_rows,
+    if ((q->flags & B200_Q_SHARED_THRESHOLDS) && E->n_peers > 0 && c.n_rows > E->peer_rows)
+        return fail(B200_E_INVALID, "b200_rank_topk: %lld rows exceed the %lld exported for threshold sharing", (long long)c.n_rows,
                     (long long)E->peer_rows);
     try {
         CK(cudaSetDevice(E->device));
-        cudaStream_t st = E->st;
-        c.st = st;
+        cudaStream_t st = c.st = E->st;
         cudaStream_t user = reinterpret_cast<cudaStream_t>(q->stream);
         // device pointers + NULL stream = CUDA's (legacy) default stream, like every CUDA API: producers / consumers of the
         // buffers on that stream are ordered against the engine stream (torch's current stream is the default stream unless
         // the caller switched it: without this a collective reading the outputs could overlap the next call's kernels)
-        if (!user && (in_dev || out_dev)) user = cudaStreamLegacy;
-        if (user && (in_dev || out_dev)) {
-            CK(cudaEventRecord(E->ev[6], user));
-            CK(cudaStreamWaitEvent(st, E->ev[6], 0));
+        if (!user && (c.in_dev || c.out_dev)) user = cudaStreamLegacy;
+        if (user && (c.in_dev || c.out_dev)) {
+            CK(cudaEventRecord(E->ev_from_user, user));
+            CK(cudaStreamWaitEvent(st, E->ev_from_user, 0));
         }
-        CK(cudaEventRecord(E->ev[0], st));
+        CK(cudaEventRecord(E->ev_begin, st));
 
-        // ---------------- stage inputs
-        // Host inputs of a large call are staged in row chunks on a second stream: the copy of chunk c+1 (subject rows / ids,
-        // its slice of the CSR filter) and the copy-back of chunk c-1 run while chunk c is being ranked.  Buffers are
-        // full-size and addressed by absolute row / nnz offsets, so the kernels see the same layout with or without chunking.
-        auto stage = [&](DevBuf& buf, const void* src, size_t bytes) -> const void* {  // un-chunked items, main stream
-            if (in_dev) return src;
-            buf.ensure(std::max<size_t>(bytes, 16));
-            if (bytes) CK(cudaMemcpyAsync(buf.p, src, bytes, cudaMemcpyHostToDevice, st));
-            S.h2d_bytes += (int64_t)bytes;
-            return buf.p;
-        };
-        const bool chunk_subjects = q->subjects && !q->subject_ids && !in_dev;  // subject rows arrive in batch order
-        const int64_t* sp_indptr = nullptr;
-        const int32_t* sp_indices = nullptr;
-        const float* sp_data = nullptr;
-        if (sparse_sub) {
-            int64_t nnz = 0;
-            if (in_dev) {
-                CK(cudaMemcpyAsync(E->h_pinned, q->sub_indptr + n_rows, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-                CK(cudaStreamSynchronize(st));
-                memcpy(&nnz, E->h_pinned, sizeof(int64_t));
-            } else {
-                nnz = q->sub_indptr[n_rows];
-            }
-            if (nnz < 0 || (nnz > 0 && (!q->sub_indices || !q->sub_data))) return fail(B200_E_INVALID, "b200_rank_topk: bad sparse subjects");
-            sp_indptr = (const int64_t*)stage(E->sp_indptr, q->sub_indptr, sizeof(int64_t) * (n_rows + 1));
-            sp_indices = (const int32_t*)stage(E->sp_indices, q->sub_indices, sizeof(int32_t) * nnz);
-            sp_data = (const float*)stage(E->sp_data, q->sub_data, sizeof(float) * nnz);
-        } else if (q->subjects) {
-            const int64_t rows_in = q->subject_ids ? q->n_subjects_total : n_rows;
-            if (q->subject_dtype != B200_DT_F32) {
-                E->sub32.ensure(sizeof(float) * rows_in * d);
-                widen16_kernel<<<grid_for(rows_in * d, 256), 256, 0, st>>>(q->subjects, q->subject_dtype == B200_DT_BF16 ? 1 : 0, rows_in * d,
-                                                                           E->sub32.as<float>());
-                CK(cudaGetLastError());
-                S.n_launches++;
-                c.sub32 = E->sub32.as<float>();
-            } else if (chunk_subjects) {
-                E->sub32.ensure(std::max<size_t>(sizeof(float) * rows_in * d, 16));
-                c.sub32 = E->sub32.as<float>();
-            } else {
-                c.sub32 = (const float*)stage(E->sub32, q->subjects, sizeof(float) * rows_in * d);
-            }
-        } else {
-            c.sub32 = E->sub32_res_ptr;
+        // ---------------- validate the CSR arrays, refuse what the plan cannot run, stage
+        const int64_t sp_nnz = q->sub_indptr ? read_nnz(E, q->sub_indptr, c.n_rows, c.in_dev) : 0;
+        if (sp_nnz < 0 || (sp_nnz > 0 && (!q->sub_indices || !q->sub_data))) return fail(B200_E_INVALID, "b200_rank_topk: bad sparse subjects");
+        const int64_t f_nnz = q->csr_indptr ? read_nnz(E, q->csr_indptr, c.n_rows, c.in_dev) : 0;
+        if (f_nnz < 0) return fail(B200_E_INVALID, "b200_rank_topk: csr_indptr[n_rows] < 0");
+        if (f_nnz > 0 && !q->csr_indices) return fail(B200_E_INVALID, "b200_rank_topk: csr_indices is NULL");
+        if (P.error != B200_OK) return fail(P.error, "%s", P.message.c_str());
+        S.path = (int)P.path;
+        if (P.tc()) {
+            S.tc_dtype = E->tc_dtype;
+            S.k_cand = P.k_cand;
+            S.epi_warps = P.nw;
+            S.wide = P.wide() ? 1 : 0;
         }
-        if (q->subject_ids) {
-            if (in_dev) {
-                c.rowmap = q->subject_ids;
-            } else {
-                E->rowmap.ensure(std::max<size_t>(sizeof(int64_t) * n_rows, 16));
-                c.rowmap = E->rowmap.as<int64_t>();
-            }
-        }
-        if (q->csr_indptr) {
-            int64_t nnz = 0;
-            if (in_dev) {
-                CK(cudaMemcpyAsync(E->h_pinned, q->csr_indptr + n_rows, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-                CK(cudaStreamSynchronize(st));
-                memcpy(&nnz, E->h_pinned, sizeof(int64_t));
-            } else {
-                nnz = q->csr_indptr[n_rows];
-            }
-            if (nnz < 0) return fail(B200_E_INVALID, "b200_rank_topk: csr_indptr[n_rows] < 0");
-            if (nnz > 0 && !q->csr_indices) return fail(B200_E_INVALID, "b200_rank_topk: csr_indices is NULL");
-            if (in_dev) {
-                c.indptr = q->csr_indptr;
-                c.indices = q->csr_indices;
-            } else {
-                E->indptr.ensure(sizeof(int64_t) * (n_rows + 1));
-                E->indices.ensure(std::max<size_t>(sizeof(int32_t) * nnz, 16));
-                c.indptr = E->indptr.as<int64_t>();
-                c.indices = E->indices.as<int32_t>();
-            }
-            if (nnz == 0) c.indptr = nullptr;  // an all-empty filter is no filter (cf. rank_implicit.py:169-173)
-        }
-        if (q->whitelist) c.wl = (const int32_t*)stage(E->wl, q->whitelist, sizeof(int32_t) * n_pos);
-        // host -> device copy of the chunked inputs of rows [r0, r1) on stream `s`
-        auto stage_rows = [&](int64_t r0, int64_t r1, cudaStream_t s) {
-            if (in_dev) return;
-            size_t bytes = 0;
-            auto h2d = [&](void* dst, const void* src, size_t n) {
-                if (n) CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, s));
-                bytes += n;
-            };
-            if (chunk_subjects) h2d(E->sub32.as<float>() + r0 * d, q->subjects + r0 * d, sizeof(float) * (r1 - r0) * d);
-            if (q->subject_ids) h2d(E->rowmap.as<int64_t>() + r0, q->subject_ids + r0, sizeof(int64_t) * (r1 - r0));
-            if (c.indptr) {
-                h2d(E->indptr.as<int64_t>() + r0, q->csr_indptr + r0, sizeof(int64_t) * (r1 - r0 + 1));
-                const int64_t z0 = q->csr_indptr[r0], z1 = q->csr_indptr[r1];
-                if (z1 < z0) throw CudaError{cudaErrorInvalidValue, "csr_indptr must be non-decreasing", __LINE__};
-                h2d(E->indices.as<int32_t>() + z0, q->csr_indices + z0, sizeof(int32_t) * (z1 - z0));
-            }
-            S.h2d_bytes += (int64_t)bytes;
-        };
-
-        // ---------------- outputs
-        if (out_dev) {
-            c.o_ids = q->out_ids;
-            c.o_scores = q->out_scores;
-            c.o_counts = q->out_counts;
-            c.o_bounds = shared ? q->out_bounds : nullptr;
-        } else {
-            E->out_ids.ensure(sizeof(int32_t) * n_rows * k_out);
-            E->out_scores.ensure(sizeof(float) * n_rows * k_out);
-            E->out_counts.ensure(sizeof(int32_t) * n_rows);
-            c.o_ids = E->out_ids.as<int32_t>();
-            c.o_scores = E->out_scores.as<float>();
-            c.o_counts = E->out_counts.as<int32_t>();
-            if (shared) {
-                E->out_bounds.ensure(sizeof(float) * n_rows);
-                c.o_bounds = E->out_bounds.as<float>();
-            }
-        }
-        // ---------------- path choice
-        // Candidates kept per list by the tensor-core pass (K' >= k / lists; the surplus is the certificate's safety margin).
-        // A row has 2 (8 epilogue warps) or 4 (16) lists, one per column group of the tile stream, so a small surplus per
-        // list already gives ~2k candidates; rows where (nearly) all of the top-k fall into one column group fail the
-        // certificate and take the second-chance pass.  Inserts, the dominant epilogue cost, scale with K'.
-        c.bf16 = E->tc_dtype == B200_TC_BF16;
-        const bool wide = k_out > 24 && k_out <= 128 && env_int("B200_WIDE", 1) != 0;
-        // 128 < k <= 1024: the same single wide pass with longer append lists and a large-k re-score, when the expected
-        // candidate count stays well inside the catalogue (k = None and near-catalogue requests keep path 3).  Item-sharded
-        // calls that share thresholds need k <= 24 and keep path 3 here as well.
-        const bool wide_l = k_out > 128 && k_out <= 1024 && env_int("B200_WIDE", 1) != 0 && !sparse_sub && !shared &&
-                            wide_geom(k_out, 2).T <= 0.5 * (double)n_pos;
-        // 16 epilogue warps (B200_EPI_WARPS=16) are opt-in: next to the MMA warp group they get 96 registers a thread and
-        // spill.  The wide mode always runs the 8-warp geometry: four lists per row freeze at a weaker, noisier rank.
-        c.nw = (!wide && !wide_l && env_int("B200_EPI_WARPS", 8) == 16) ? 16 : 8;
-        int k_cand = 0;
-        if (k_out <= 24) {
-            if (c.nw == 16) {
-                // four lists per row: a list may be SHORTER than k (the certificate only needs the k-th exact score above every
-                // list's threshold); rows whose top-k crowd into one column quarter take the second-chance pass
-                k_cand = std::min(16, (k_out <= 10 ? 8 : k_out <= 16 ? 12 : 16) + (c.bf16 ? 2 : 0));
-            } else {
-                const int surplus = c.bf16 ? std::max(6, k_out / 2) : std::max(2, k_out / 4);
-                k_cand = std::min(32, k_out + surplus);
-            }
-        } else if (k_out <= 128) {
-            k_cand = wide ? 24 : (c.bf16 ? 30 : 25);  // wide: adaptive lists of phase 1;  else passes of 20
-        } else if (wide_l) {
-            k_cand = 32;  // the full 32 slots: the frozen threshold samples ~58 ranks instead of ~42
-        }
-        if (shared && E->n_peers > 0 && k_out <= 24) {
-            // Shared thresholds: the pruning bound of a row is the MAXIMUM over all L = ranks x lists list minima, i.e. the
-            // largest K'-th best of L samples of N/L objects -- about global rank L K' - c_L L sqrt(K') (c_L = expected maximum
-            // of L standard normals).  The certificate needs that rank to stay above k plus a margin; everything beyond is
-            // wasted insertions (K' = 12 on 8 ranks sits near rank 100, K' = 6 near rank 27).
-            const int L = (E->n_peers + 1) * (c.nw / 4);
-            const double cL = L <= 2 ? 0.56 : L <= 4 ? 1.03 : L <= 8 ? 1.42 : L <= 16 ? 1.77 : L <= 32 ? 2.07 : 2.33;
-            const double target = k_out + std::max(12.0, 0.6 * k_out) + (c.bf16 ? 20.0 : 0.0);
-            int kc = 4;
-            while (kc < 32 && L * kc - cL * L * std::sqrt((double)kc) < target) ++kc;
-            k_cand = std::min(kc, c.nw == 16 ? 16 : 32);
-        }
-        {
-            const int forced = env_int("B200_TC_KCAND", 0);  // tuning hook
-            if (forced >= 4 && forced <= 32 && (forced >= k_out || c.nw == 16 || wide || wide_l || shared)) k_cand = forced;
-        }
-        bool use_tc = !sparse_sub && E->tc_dtype != B200_TC_OFF && k_cand > 0 && !(q->flags & B200_Q_FORCE_EXACT) && n_pos >= (int64_t)k_cand * 4;
-        if (use_tc && !(q->flags & B200_Q_FORCE_TC)) {
-            // tiny problems are cheaper (and exercised) on the exhaustive kernel
-            if ((double)n_rows * (double)n_pos < 4.0e6) use_tc = false;
-        }
-        if (use_tc && (size_t)SEL_WARPS * d * sizeof(float) > 64 * 1024)
-            return fail(B200_E_UNSUPPORTED, "b200_rank_topk: d too large for the re-score kernel");
-        if ((q->flags & B200_Q_FORCE_TC) && !use_tc)
-            return fail(B200_E_UNSUPPORTED, "b200_rank_topk: tensor-core path unavailable (tc_dtype=%d, k=%d, d_pad=%d, n_pos=%lld)",
-                        E->tc_dtype, k_out, E->d_pad, (long long)n_pos);
-        const bool peers = shared && use_tc;  // (zero peers: the same protocol, nothing to adopt)
-        if (shared && use_tc && k_out > 24) return fail(B200_E_UNSUPPORTED, "b200_rank_topk: B200_Q_SHARED_THRESHOLDS needs k <= 24");
-
-        // failure lists (absolute rows) + counters: [fb1 | fb2 | fbA | fbB | counters]
-        E->fb_rows.ensure(sizeof(int32_t) * (4 * n_rows + 16));
-        int32_t* fb1 = E->fb_rows.as<int32_t>();
-        int32_t* fb2 = fb1 + n_rows;
-        int32_t* fbA = fb2 + n_rows;
-        int32_t* fbB = fbA + n_rows;
-        int32_t* cnt = fbB + n_rows;
-        CK(cudaMemsetAsync(cnt, 0, 16 * sizeof(int32_t), st));
-        if (k_out <= 128 && (wide || (use_tc && k_out > 24))) E->excl.ensure(sizeof(int32_t) * (size_t)n_rows * k_out);  // (k > 128: no exclusion passes)
-
-        // ---------------- main pass over the rows of one chunk
-        auto main_pass = [&](int64_t r0, int64_t r1) {
-            const int64_t nr = r1 - r0;
-            int32_t* oi = c.o_ids + r0 * k_out;
-            float* os = c.o_scores + r0 * k_out;
-            int32_t* oc = c.o_counts + r0;
-            init_outputs_kernel<<<grid_for(std::max<int64_t>(nr * k_out, nr), 256), 256, 0, st>>>(oi, os, oc, nr, k_out);
-            CK(cudaGetLastError());
-            S.n_launches++;
-            const float* sub = (c.sub32 && !c.rowmap) ? c.sub32 + r0 * d : c.sub32;
-            const int64_t* rm = c.rowmap ? c.rowmap + r0 : nullptr;
-            const int64_t* ip = c.indptr ? c.indptr + r0 : nullptr;
-            if (sparse_sub) {
-                S.path = 2;
-                run_sparse(c, sp_indptr + r0, sp_indices, sp_data, nr, ip, oi, os, oc);
-            } else if (!use_tc && k_out > 128) {
-                S.path = 3;  // materialised exhaustive scores + streaming selection passes
-                run_dense_large_k(c, nullptr, sub, rm, ip, nr, oi, os, oc, true);
-                if (c.o_bounds) {
-                    fill_f32_kernel<<<grid_for(nr, 256), 256, 0, st>>>(c.o_bounds + r0, nr, -INFINITY);
-                    CK(cudaGetLastError());
-                }
-            } else if (!use_tc) {
-                S.path = 0;
-                run_exact(c, nullptr, nr, sub, rm, ip, oi, os, oc, 0, k_out, true);
-                if (c.o_bounds) {  // exhaustive lists: nothing was discarded
-                    fill_f32_kernel<<<grid_for(nr, 256), 256, 0, st>>>(c.o_bounds + r0, nr, -INFINITY);
-                    CK(cudaGetLastError());
-                }
-            } else {
-                S.path = 1;
-                S.tc_dtype = E->tc_dtype;
-                TcPass t;
-                t.n_sel = nr;
-                t.sub32 = sub;
-                t.rowmap = rm;
-                t.indptr = ip;
-                t.o_ids = oi;
-                t.o_scores = os;
-                t.o_counts = oc;
-                t.o_bounds = c.o_bounds ? c.o_bounds + r0 : nullptr;
-                t.nw = c.nw;
-                t.kc = k_cand;
-                t.row0 = r0;
-                t.fb_list = fb1;
-                t.fb_count = cnt;
-                t.main = true;
-                t.peers = peers;
-                t.k0 = 0;
-                t.kp = k_out;
-                t.wide = wide || wide_l;
-                run_tc(c, t);
-            }
-            if (E->id_offset != 0) {
-                add_offset_kernel<<<grid_for(nr * k_out, 256), 256, 0, st>>>(oi, nr * k_out, (int32_t)E->id_offset);
-                CK(cudaGetLastError());
-                S.n_launches++;
-            }
-        };
-
-        // Re-rank `n_sel` rows (absolute row numbers in `rows`) without any shortcut that could fail again unnoticed:
-        // k <= 24: one pass with the widest lists (32 slots, 8-warp kernel), then the exhaustive kernel for what still fails;
-        // k  > 24: certified passes of 20 results with exclusion lists, each followed by its own wide-list pass and the
-        // exhaustive kernel.  Results are written with LOCAL ids; the caller applies the id offset.
-        auto rerank_rows = [&](const int32_t* rows, int64_t n_sel) {
-            init_rows_kernel<<<grid_for(n_sel * k_out, 256), 256, 0, st>>>(c.o_ids, c.o_scores, c.o_counts, rows, n_sel, k_out);
-            CK(cudaGetLastError());
-            S.n_launches++;
-            const int k_pass = k_out <= 24 ? k_out : 20;
-            const int kc_pass = k_out <= 24 ? 32 : (c.bf16 ? 30 : 25);
-            for (int k0 = 0; k0 < k_out; k0 += k_pass) {
-                const int kp = std::min(k_pass, k_out - k0);
-                if (k0 > 0) {
-                    build_exclusion_kernel<<<grid_for(n_sel * 32, 256), 256, 0, st>>>(c.o_ids, rows, n_sel, k_out, k0, (int32_t)E->id_offset,
-                                                                                     E->excl.as<int32_t>());
-                    CK(cudaGetLastError());
-                    S.n_launches++;
-                }
-                CK(cudaMemsetAsync(cnt + 2, 0, 2 * sizeof(int32_t), st));
-                TcPass t;
-                t.rows_dev = rows;
-                t.n_sel = n_sel;
-                t.sub32 = c.sub32;
-                t.rowmap = c.rowmap;
-                t.indptr = c.indptr;
-                t.o_ids = c.o_ids;
-                t.o_scores = c.o_scores;
-                t.o_counts = c.o_counts;
-                t.nw = 8;
-                t.kc = std::min(32, std::max(kc_pass - (k_pass - kp), kp));
-                t.k0 = k0;
-                t.kp = kp;
-                t.fb_list = fbA;
-                t.fb_count = cnt + 2;
-                run_tc(c, t);
-                int64_t n_fb = read_counter(c, cnt + 2);
-                const int32_t* f = fbA;
-                if (n_fb > 0 && t.kc < 32) {  // the pass's own second chance: widest lists
-                    TcPass t2 = t;
-                    t2.rows_dev = fbA;
-                    t2.n_sel = n_fb;
-                    t2.kc = 32;
-                    t2.fb_list = fbB;
-                    t2.fb_count = cnt + 3;
-                    run_tc(c, t2);
-                    n_fb = read_counter(c, cnt + 3);
-                    f = fbB;
-                }
-                S.n_exact_rows += n_fb;
-                if (n_fb > 0) run_exact(c, f, n_fb, c.sub32, c.rowmap, c.indptr, c.o_ids, c.o_scores, c.o_counts, k0, k0 + kp, false);
-            }
-        };
-
-        // k > 128: rows the wide pass could not certify are ranked by the exhaustive kernels of path 3, over these rows only.
-        auto rerank_exhaustive = [&](const int32_t* rows, int64_t n_sel) {
-            init_rows_kernel<<<grid_for(n_sel * k_out, 256), 256, 0, st>>>(c.o_ids, c.o_scores, c.o_counts, rows, n_sel, k_out);
-            CK(cudaGetLastError());
-            S.n_launches++;
-            run_dense_large_k(c, rows, c.sub32, c.rowmap, c.indptr, n_sel, c.o_ids, c.o_scores, c.o_counts, false);
-            S.n_exact_rows += n_sel;
-        };
+        stage_inputs(c, sp_nnz, f_nnz);
 
         // ---------------- chunk pipeline
-        const bool multipass_main = use_tc && k_out > 24 && !wide && !wide_l;
-        int64_t chunk = n_rows;
-        if (!in_dev && use_tc && !multipass_main) {
-            const int64_t wave = (int64_t)(E->sm_count / 2) * 256;  // subject rows one wave of CTA pairs works on
-            int64_t want = 8 * wave;
-            if (const char* env = getenv("B200_CHUNK_ROWS")) want = std::max<int64_t>(256, atoll(env));  // test hook
-            if (n_rows >= 2 * want) chunk = want;
-        }
-        if (use_tc && wide_l) {
-            // the append lists take lists x cand_stride x 8 B per row (~21 GB for 1M rows at k = 1000): row chunks keep them
-            // within the budget, for device inputs too.  Whole waves of CTA pairs where the budget allows.
-            const int64_t per_row = (int64_t)2 * wide_geom(k_out, 2).cand_stride * 8;
-            const int64_t budget = (int64_t)env_int("B200_WIDE_BUDGET_MB", 2048) << 20;  // test hook
-            const int64_t wave = (int64_t)(E->sm_count / 2) * 256;
-            int64_t fit = std::max<int64_t>(256, budget / per_row / 256 * 256);
-            if (fit >= wave) fit = fit / wave * wave;
-            chunk = std::min(chunk, fit);
-        }
-        const int64_t n_chunks = (n_rows + chunk - 1) / chunk;
+        const int64_t chunk = P.chunk, n_chunks = P.n_chunks;
         cudaStream_t cs = n_chunks > 1 ? E->cs : st;
         S.n_chunks = (int32_t)n_chunks;
         if (n_chunks > 1) {
             CK(cudaEventRecord(E->evp[2], st));  // the copy stream starts after everything queued so far (whitelist, ...)
             CK(cudaStreamWaitEvent(cs, E->evp[2], 0));
         }
-        stage_rows(0, std::min(chunk, n_rows), cs);
+        stage_rows(c, 0, std::min(chunk, c.n_rows), cs);
         CK(cudaEventRecord(E->evp[0], cs));
-        CK(cudaEventRecord(E->ev[1], cs));
-        auto copy_back = [&](int64_t r0, int64_t r1, cudaStream_t s) {
-            CK(cudaMemcpyAsync(q->out_ids + r0 * k_out, c.o_ids + r0 * k_out, sizeof(int32_t) * (r1 - r0) * k_out, cudaMemcpyDeviceToHost, s));
-            CK(cudaMemcpyAsync(q->out_scores + r0 * k_out, c.o_scores + r0 * k_out, sizeof(float) * (r1 - r0) * k_out, cudaMemcpyDeviceToHost, s));
-            CK(cudaMemcpyAsync(q->out_counts + r0, c.o_counts + r0, sizeof(int32_t) * (r1 - r0), cudaMemcpyDeviceToHost, s));
-            S.d2h_bytes += (int64_t)((r1 - r0) * k_out * 8 + (r1 - r0) * 4);
-            if (shared) {
-                CK(cudaMemcpyAsync(q->out_bounds + r0, c.o_bounds + r0, sizeof(float) * (r1 - r0), cudaMemcpyDeviceToHost, s));
-                S.d2h_bytes += (int64_t)(r1 - r0) * 4;
-            }
-        };
+        CK(cudaEventRecord(E->ev_staged, cs));
         for (int64_t ci = 0; ci < n_chunks; ++ci) {
-            const int64_t r0 = ci * chunk, r1 = std::min(n_rows, r0 + chunk);
+            const int64_t r0 = ci * chunk, r1 = std::min(c.n_rows, r0 + chunk);
             if (ci + 1 < n_chunks) {
-                stage_rows(r1, std::min(n_rows, r1 + chunk), cs);
+                stage_rows(c, r1, std::min(c.n_rows, r1 + chunk), cs);
                 CK(cudaEventRecord(E->evp[(ci + 1) & 1], cs));
             }
             if (n_chunks > 1) CK(cudaStreamWaitEvent(st, E->evp[ci & 1], 0));
-            if (multipass_main) {
-                // every row takes the certified multi-pass route (tuning / test hook B200_WIDE=0)
-                S.path = 1;
-                S.tc_dtype = E->tc_dtype;
-                S.k_cand = k_cand;
-                S.epi_warps = 8;
-                iota_kernel<<<grid_for(n_rows, 256), 256, 0, st>>>(fb1, n_rows);
-                CK(cudaGetLastError());
-                rerank_rows(fb1, n_rows);
-                if (E->id_offset != 0) {
-                    add_offset_kernel<<<grid_for(n_rows * k_out, 256), 256, 0, st>>>(c.o_ids, n_rows * k_out, (int32_t)E->id_offset);
-                    CK(cudaGetLastError());
-                }
-            } else {
-                main_pass(r0, r1);
-            }
-            if (ci + 1 == n_chunks) CK(cudaEventRecord(E->ev[4], st));
-            if (!out_dev) {
+            main_pass(c, r0, r1);
+            if (ci + 1 == n_chunks) CK(cudaEventRecord(E->ev_ranked, st));
+            if (!c.out_dev) {
                 if (n_chunks > 1) {
                     CK(cudaEventRecord(E->evp[2], st));
                     CK(cudaStreamWaitEvent(cs, E->evp[2], 0));
                 }
-                copy_back(r0, r1, cs);
+                copy_back(c, r0, r1, cs);
             }
         }
-        // ---------------- rows whose certificate failed in the main pass (all chunks): re-rank, patch the results
-        int64_t n_fb = 0;
-        if (use_tc && !multipass_main && !peers && !sparse_sub) {
-            n_fb = read_counter(c, cnt);
-            S.n_fallback_rows = n_fb;
-            if (n_fb > 0) {
-                if (k_out > 128)
-                    rerank_exhaustive(fb1, n_fb);
-                else
-                    rerank_rows(fb1, n_fb);
-                if (E->id_offset != 0) {
-                    add_offset_rows_kernel<<<grid_for(n_fb * k_out, 256), 256, 0, st>>>(c.o_ids, fb1, n_fb, k_out, (int32_t)E->id_offset);
-                    CK(cudaGetLastError());
-                    S.n_launches++;
-                }
-                if (!out_dev) {
-                    // packed copies of the patched rows: one more small transfer, scattered into the caller's arrays below
-                    const size_t row_bytes = (size_t)k_out * 8 + 8;
-                    E->patch.ensure(row_bytes * n_fb);
-                    int32_t* g_ids = E->patch.as<int32_t>();
-                    float* g_sc = reinterpret_cast<float*>(g_ids + n_fb * k_out);
-                    int32_t* g_cnt = reinterpret_cast<int32_t*>(g_sc + n_fb * k_out);
-                    int32_t* g_rows = g_cnt + n_fb;
-                    gather_rows_kernel<<<grid_for(n_fb * k_out, 256), 256, 0, st>>>(c.o_ids, c.o_scores, c.o_counts, fb1, n_fb, k_out, g_ids,
-                                                                                   g_sc, g_cnt);
-                    CK(cudaGetLastError());
-                    CK(cudaMemcpyAsync(g_rows, fb1, sizeof(int32_t) * n_fb, cudaMemcpyDeviceToDevice, st));
-                    E->h_patch.resize(row_bytes * n_fb);
-                    if (n_chunks > 1) {  // the caller's arrays must hold the chunk copies before they are patched
-                        CK(cudaEventRecord(E->evp[2], cs));
-                        CK(cudaStreamWaitEvent(st, E->evp[2], 0));
-                    }
-                    CK(cudaMemcpyAsync(E->h_patch.data(), E->patch.p, row_bytes * n_fb, cudaMemcpyDeviceToHost, st));
-                    CK(cudaStreamSynchronize(st));
-                    const int32_t* h_ids = reinterpret_cast<const int32_t*>(E->h_patch.data());
-                    const float* h_sc = reinterpret_cast<const float*>(h_ids + n_fb * k_out);
-                    const int32_t* h_cnt = reinterpret_cast<const int32_t*>(h_sc + n_fb * k_out);
-                    const int32_t* h_rows = h_cnt + n_fb;
-                    for (int64_t i = 0; i < n_fb; ++i) {
-                        const int64_t r = h_rows[i];
-                        memcpy(q->out_ids + r * k_out, h_ids + i * k_out, sizeof(int32_t) * k_out);
-                        memcpy(q->out_scores + r * k_out, h_sc + i * k_out, sizeof(float) * k_out);
-                        q->out_counts[r] = h_cnt[i];
-                    }
-                    S.d2h_bytes += (int64_t)(row_bytes * n_fb);
-                }
-            }
-        }
+        if (P.tc() && P.mode != TcMode::MULTI_PASS && !P.peers) rerank_failures(c, cs);
+
+        // ---------------- finish
         if (n_chunks > 1) {  // the main stream (and through it the caller) sees the copies of the last chunks
             CK(cudaEventRecord(E->evp[2], cs));
             CK(cudaStreamWaitEvent(st, E->evp[2], 0));
         }
-        CK(cudaEventRecord(E->ev[5], st));
-        if (user && out_dev) {
-            CK(cudaEventRecord(E->ev[7], st));
-            CK(cudaStreamWaitEvent(user, E->ev[7], 0));
+        CK(cudaEventRecord(E->ev_end, st));
+        if (user && c.out_dev) {
+            CK(cudaEventRecord(E->ev_to_user, st));
+            CK(cudaStreamWaitEvent(user, E->ev_to_user, 0));
         }
         CK(cudaStreamSynchronize(st));
-        CK(cudaEventElapsedTime(&S.ms_total, E->ev[0], E->ev[5]));
-        CK(cudaEventElapsedTime(&S.ms_h2d, E->ev[0], E->ev[1]));  // exposed part: the first chunk's inputs
-        CK(cudaEventElapsedTime(&S.ms_d2h, E->ev[4], E->ev[5]));  // exposed part: the last chunk's results (+ re-ranked rows)
+        CK(cudaEventElapsedTime(&S.ms_total, E->ev_begin, E->ev_end));
+        CK(cudaEventElapsedTime(&S.ms_h2d, E->ev_begin, E->ev_staged));  // exposed part: the first chunk's inputs
+        CK(cudaEventElapsedTime(&S.ms_d2h, E->ev_ranked, E->ev_end));    // exposed part: the last chunk's results (+ re-ranked rows)
         c.collect_times();
     } catch (const CudaError& ce) {
         return fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_topk: %s failed at line %d: %s", ce.what,

@@ -26,6 +26,7 @@
 //
 // Replaces the same reference code as named in tc_common.cuh (rank_implicit.py:264-272 / rank_torch.py:133-152).
 #pragma once
+#include "sizes.h"
 #include "tc_common.cuh"
 
 namespace b200 {
@@ -42,7 +43,7 @@ struct FusedCfg {
     static constexpr int COLS = 1024 / NW;            // accumulator columns per epilogue thread and tile
     static constexpr int NLIST = NW / 4;              // column groups = candidate lists per row
     static constexpr int NQ = COLS / QUART_N;         // staged quarters per epilogue thread and tile
-    static constexpr int SLOTS = 64 / NLIST;          // list capacity (K' <= SLOTS)
+    static constexpr int SLOTS = ROW_SLOTS / NLIST;   // list capacity (K' <= SLOTS)
     static constexpr int Q = NW == 8 ? 8 : 4;         // deferred hits per thread (ring FIFO)
     static constexpr int QSTRIDE = NW * 32 * 8;       // bytes between FIFO slots: [slot][epilogue thread] x (score, position)
     static constexpr int QBYTES = Q * QSTRIDE;

@@ -1,0 +1,221 @@
+// The decision of one b200_rank_topk call: which path ranks it, with which tensor-core mode, epilogue geometry and list
+// size K', in how many row chunks -- or which refusal it gets.  Pure arithmetic on the query shape, the engine's
+// properties and the B200_* environment hooks, in plain C++17 (no CUDA header), so that tests/test_call_plan_cpu.py
+// compiles it with g++ alone and pins it.
+#pragma once
+#include <algorithm>
+#include <cmath>
+#include <cstdint>
+#include <cstdlib>
+#include <optional>
+#include <string>
+
+#include "../../include/b200_rank.h"
+#include "sizes.h"
+
+namespace b200 {
+
+inline int64_t round_up(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
+
+// Tuning, measurement and test variables, read once per call (tests set them between calls, never during one).
+struct Hooks {
+    int wide = 1;               // B200_WIDE: 0 keeps 24 < k <= 1024 off the wide mode (multi-pass route / path 3)
+    std::optional<int> wide_t;  // B200_WIDE_T: the wide mode's expected candidate count T
+    int epi_warps = 8;          // B200_EPI_WARPS: 16 selects the opt-in 16-warp geometry (k <= 24)
+    int tc_kcand = 0;           // B200_TC_KCAND: K' of the main pass (4 .. 32)
+    int tc_splits = 0;          // B200_TC_SPLITS: object splits of a fused-kernel launch (1 .. its maximum)
+    int tc_carousel = 1;        // B200_TC_CAROUSEL: 0 starts every work item at its first object tile
+    int tc_debug = 0;           // B200_TC_DEBUG: fused-kernel measurement modes (TcParams::debug_mode; results are invalid)
+    int64_t chunk_rows = 0;     // B200_CHUNK_ROWS: row chunk of host-input calls (0: 8 waves; at least 256)
+    int wide_budget_mb = 2048;  // B200_WIDE_BUDGET_MB: device memory for the append lists of k > 128
+    int tc_snapshot = 0;        // B200_TC_SNAPSHOT: the fused-kernel launch whose state is kept (0: none)
+};
+
+inline Hooks read_hooks() {
+    auto get = [](const char* name, int dflt) {
+        const char* v = std::getenv(name);
+        return v ? std::atoi(v) : dflt;
+    };
+    Hooks h;
+    h.wide = get("B200_WIDE", h.wide);
+    if (const char* v = std::getenv("B200_WIDE_T")) h.wide_t = std::atoi(v);
+    h.epi_warps = get("B200_EPI_WARPS", h.epi_warps);
+    h.tc_kcand = get("B200_TC_KCAND", h.tc_kcand);
+    h.tc_splits = get("B200_TC_SPLITS", h.tc_splits);
+    h.tc_carousel = get("B200_TC_CAROUSEL", h.tc_carousel);
+    h.tc_debug = get("B200_TC_DEBUG", h.tc_debug);
+    if (const char* v = std::getenv("B200_CHUNK_ROWS")) h.chunk_rows = std::max<int64_t>(256, std::atoll(v));
+    h.wide_budget_mb = get("B200_WIDE_BUDGET_MB", h.wide_budget_mb);
+    h.tc_snapshot = get("B200_TC_SNAPSHOT", h.tc_snapshot);
+    return h;
+}
+
+// Wide mode: T = the candidates a row is expected to collect, and the slots of each of its `nlist` append lists.  The
+// threshold frozen after a fraction q of the stream is about the (lists x K' - 6)-th best of that fraction, i.e. rank
+// ~ (lists x K' - 6) / q overall, so q follows from T.  k <= 128: T = 1.35 k + 40 (K' = 24), at most WIDE_MAX slots per row.
+// k > 128: T = 1.6 k + 64 (K' = 32), at most WIDE_MAX_L slots per row -- the frozen threshold is an order statistic of
+// ~58 samples, and this margin keeps the rows with fewer than k candidates (or an overflowing list) near 0.3 % (DESIGN 3.4).
+struct WideGeom {
+    double T = 0;
+    int cand_stride = 0;
+};
+
+inline WideGeom wide_geom(int kp, int nlist, const Hooks& h) {
+    WideGeom g;
+    g.T = h.wide_t.value_or(kp <= 128 ? (int)(1.35 * kp + 40) : (int)(1.6 * kp + 64));
+    g.cand_stride = std::min((int)round_up((int64_t)(g.T / nlist * 1.5 + 32), 8), (kp <= 128 ? WIDE_MAX : WIDE_MAX_L) / nlist);
+    return g;
+}
+
+// Object splits of a fused-kernel launch: fill the machine when there are few row tiles, even out the last wave
+// otherwise (`n_units` CTA pairs work concurrently).  `forced` (B200_TC_SPLITS) wins when it is in range.
+inline int choose_splits(int n_row_tiles, int n_obj_tiles, int n_units, bool wide, int forced) {
+    int best_splits = 1;
+    double best_eff = -1.0;
+    const int max_splits = wide ? 1 : std::max(1, std::min(16, n_obj_tiles * 2 / 32));
+    for (int s = 1; s <= max_splits; ++s) {
+        const double work = (double)n_row_tiles * s;
+        const double waves = std::ceil(work / n_units);
+        const double eff = work / (waves * n_units) - 0.01 * (s - 1);
+        if (eff > best_eff + 1e-9) {
+            best_eff = eff;
+            best_splits = s;
+        }
+    }
+    if (forced >= 1 && forced <= max_splits) best_splits = forced;
+    return best_splits;
+}
+
+// What a call ranks and what the engine knows about itself.
+struct CallShape {
+    int64_t n_rows = 0;
+    int64_t n_pos = 0;  // object positions: the whitelist, else the catalogue
+    int64_t k = 0;      // requested k
+    int d = 0, d_pad = 0;
+    int sm_count = 0;
+    int tc_dtype = B200_TC_OFF;  // the engine's resolved tensor-core type
+    int n_peers = 0;             // ranks the engine shares thresholds with
+    int32_t flags = 0;           // B200_Q_*
+    bool sparse = false;         // sparse subject rows
+};
+
+enum class Path { EXACT = 0, TC = 1, SPARSE = 2, DENSE_LARGE_K = 3 };  // = b200_rank_stats::path
+
+// How the tensor-core path ranks the rows of the main pass.
+enum class TcMode {
+    NARROW,      // k <= 24: adaptive lists of K' slots
+    WIDE,        // 24 < k <= 128: one pass, frozen threshold + append lists
+    WIDE_L,      // 128 < k <= 1024: the same with longer append lists and the large re-score
+    MULTI_PASS,  // 24 < k without the wide mode: certified passes of 20 results for every row
+};
+
+struct CallPlan {
+    int k_out = 0;
+    Path path = Path::EXACT;
+    TcMode mode = TcMode::NARROW;  // path TC only
+    bool bf16 = false;             // operand type of the tensor-core passes
+    int nw = 8;                    // epilogue warps of the main pass
+    int k_cand = 0;                // K' of the main pass
+    bool peers = false;            // the main pass shares thresholds (B200_Q_SHARED_THRESHOLDS)
+    WideGeom geom;                 // WIDE / WIDE_L
+    int64_t chunk = 0, n_chunks = 0;  // row chunks of the main pass
+    int error = B200_OK;           // otherwise the call is refused with this code and message
+    std::string message;
+
+    bool tc() const { return path == Path::TC; }
+    bool wide() const { return tc() && (mode == TcMode::WIDE || mode == TcMode::WIDE_L); }
+};
+
+inline CallPlan plan_call(const CallShape& s, const Hooks& h) {
+    CallPlan p;
+    const int k = p.k_out = (int)std::min<int64_t>(s.k, s.n_pos);
+    if (s.n_rows == 0 || k <= 0) return p;  // nothing to rank
+    p.bf16 = s.tc_dtype == B200_TC_BF16;
+    const bool shared = s.flags & B200_Q_SHARED_THRESHOLDS;
+    const bool wide = k > 24 && k <= 128 && h.wide != 0;
+    // 128 < k <= 1024: the same single wide pass with longer append lists and a large-k re-score, when the expected
+    // candidate count stays well inside the catalogue (k = None and near-catalogue requests keep path 3).  Item-sharded
+    // calls that share thresholds need k <= 24 and keep path 3 here as well.
+    const bool wide_l = k > 128 && k <= 1024 && h.wide != 0 && !s.sparse && !shared && wide_geom(k, 2, h).T <= 0.5 * (double)s.n_pos;
+    // 16 epilogue warps (B200_EPI_WARPS=16) are opt-in: next to the MMA warp group they get 96 registers a thread and
+    // spill.  The wide mode always runs the 8-warp geometry: four lists per row freeze at a weaker, noisier rank.
+    int nw = (!wide && !wide_l && h.epi_warps == 16) ? 16 : 8;
+
+    // Candidates kept per list by the tensor-core pass (K' >= k / lists; the surplus is the certificate's safety margin).
+    // A row has 2 (8 epilogue warps) or 4 (16) lists, one per column group of the tile stream, so a small surplus per
+    // list already gives ~2k candidates; rows where (nearly) all of the top-k fall into one column group fail the
+    // certificate and take the second-chance pass.  Inserts, the dominant epilogue cost, scale with K'.
+    int k_cand = 0;
+    if (k <= 24) {
+        if (nw == 16) {
+            // four lists per row: a list may be SHORTER than k (the certificate only needs the k-th exact score above every
+            // list's threshold); rows whose top-k crowd into one column quarter take the second-chance pass
+            k_cand = std::min(16, (k <= 10 ? 8 : k <= 16 ? 12 : 16) + (p.bf16 ? 2 : 0));
+        } else {
+            const int surplus = p.bf16 ? std::max(6, k / 2) : std::max(2, k / 4);
+            k_cand = std::min(32, k + surplus);
+        }
+    } else if (k <= 128) {
+        k_cand = wide ? 24 : (p.bf16 ? 30 : 25);  // wide: adaptive lists of phase 1;  else passes of 20
+    } else if (wide_l) {
+        k_cand = 32;  // the full 32 slots: the frozen threshold samples ~58 ranks instead of ~42
+    }
+    if (shared && s.n_peers > 0 && k <= 24) {
+        // Shared thresholds: the pruning bound of a row is the MAXIMUM over all L = ranks x lists list minima, i.e. the
+        // largest K'-th best of L samples of N/L objects -- about global rank L K' - c_L L sqrt(K') (c_L = expected maximum
+        // of L standard normals).  The certificate needs that rank to stay above k plus a margin; everything beyond is
+        // wasted insertions (K' = 12 on 8 ranks sits near rank 100, K' = 6 near rank 27).
+        const int L = (s.n_peers + 1) * (nw / 4);
+        const double cL = L <= 2 ? 0.56 : L <= 4 ? 1.03 : L <= 8 ? 1.42 : L <= 16 ? 1.77 : L <= 32 ? 2.07 : 2.33;
+        const double target = k + std::max(12.0, 0.6 * k) + (p.bf16 ? 20.0 : 0.0);
+        int kc = 4;
+        while (kc < 32 && L * kc - cL * L * std::sqrt((double)kc) < target) ++kc;
+        k_cand = std::min(kc, nw == 16 ? 16 : 32);
+    }
+    const int forced = h.tc_kcand;
+    if (forced >= 4 && forced <= 32 && (forced >= k || nw == 16 || wide || wide_l || shared)) k_cand = forced;
+
+    bool use_tc = !s.sparse && s.tc_dtype != B200_TC_OFF && k_cand > 0 && !(s.flags & B200_Q_FORCE_EXACT) &&
+                  s.n_pos >= (int64_t)k_cand * 4;
+    // tiny problems are cheaper (and exercised) on the exhaustive kernel
+    if (use_tc && !(s.flags & B200_Q_FORCE_TC) && (double)s.n_rows * (double)s.n_pos < 4.0e6) use_tc = false;
+    auto refuse = [&](const std::string& why) {
+        p.error = B200_E_UNSUPPORTED;
+        p.message = "b200_rank_topk: " + why;
+        return p;
+    };
+    if (use_tc && (size_t)SEL_WARPS * s.d * sizeof(float) > 64 * 1024) return refuse("d too large for the re-score kernel");
+    if ((s.flags & B200_Q_FORCE_TC) && !use_tc)
+        return refuse("tensor-core path unavailable (tc_dtype=" + std::to_string(s.tc_dtype) + ", k=" + std::to_string(k) +
+                      ", d_pad=" + std::to_string(s.d_pad) + ", n_pos=" + std::to_string(s.n_pos) + ")");
+    if (shared && use_tc && k > 24) return refuse("B200_Q_SHARED_THRESHOLDS needs k <= 24");
+
+    p.path = s.sparse ? Path::SPARSE : use_tc ? Path::TC : k > 128 ? Path::DENSE_LARGE_K : Path::EXACT;
+    p.chunk = s.n_rows;
+    if (p.tc()) {
+        p.mode = wide ? TcMode::WIDE : wide_l ? TcMode::WIDE_L : k > 24 ? TcMode::MULTI_PASS : TcMode::NARROW;
+        p.peers = shared;  // (zero peers: the same protocol, nothing to adopt)
+        p.nw = p.mode == TcMode::MULTI_PASS ? 8 : nw;
+        p.k_cand = std::min(k_cand, ROW_SLOTS / (p.nw / 4));  // (the n_pos bound above takes K' before this cap)
+        if (p.wide()) p.geom = wide_geom(k, p.nw / 4, h);
+        const int64_t wave = (int64_t)(s.sm_count / 2) * 256;  // subject rows one wave of CTA pairs works on
+        if (!(s.flags & B200_Q_INPUTS_ON_DEVICE) && p.mode != TcMode::MULTI_PASS) {
+            // host inputs: row chunks let the copies of one chunk overlap the ranking of another
+            const int64_t want = h.chunk_rows > 0 ? h.chunk_rows : 8 * wave;
+            if (s.n_rows >= 2 * want) p.chunk = want;
+        }
+        if (p.mode == TcMode::WIDE_L) {
+            // the append lists take lists x cand_stride x 8 B per row (~21 GB for 1M rows at k = 1000): row chunks keep them
+            // within the budget, for device inputs too.  Whole waves of CTA pairs where the budget allows.
+            const int64_t per_row = (int64_t)2 * p.geom.cand_stride * 8;
+            const int64_t budget = (int64_t)h.wide_budget_mb << 20;
+            int64_t fit = std::max<int64_t>(256, budget / per_row / 256 * 256);
+            if (fit >= wave) fit = fit / wave * wave;
+            p.chunk = std::min(p.chunk, fit);
+        }
+    }
+    p.n_chunks = (s.n_rows + p.chunk - 1) / p.chunk;
+    return p;
+}
+
+}  // namespace b200

@@ -5,6 +5,7 @@
 // definition of include/b200_rank.h (fp64-accumulated dot rounded once to fp32; order = score desc, id asc).
 #pragma once
 #include "common.cuh"
+#include "sizes.h"
 
 namespace b200 {
 
@@ -218,8 +219,6 @@ struct SelectParams {
     float* out_bounds;        // rescore: nullable [rows] (exact-score units, already includes eps);  merge: unused
     const float* in_bounds;   // merge: nullable [n_lists][rows]
 };
-
-constexpr int SEL_WARPS = 8;
 
 // the smallest fp32 that is >= x (bounds are compared against fp32 scores)
 __device__ __forceinline__ float round_up_f32(double x) {
@@ -448,10 +447,9 @@ __global__ void __launch_bounds__(SEL_WARPS * 32) rescore_select_kernel(const Se
 //   rescore_wide_kernel       : kp <= 128, up to WIDE_MAX candidates per row, 128 threads, static shared arrays;
 //   rescore_wide_large_kernel : 128 < kp <= 1024, up to WIDE_MAX_L candidates per row, 256 threads, the arrays in dynamic
 //                               shared memory behind the subject row (32 KiB of score / id pairs at full capacity).
+// (WIDE_MAX / WIDE_MAX_L: sizes.h, the host sizes the append lists by them)
 constexpr int WIDE_THREADS = 128;
-constexpr int WIDE_MAX = 512;
 constexpr int WIDE_THREADS_L = 256;
-constexpr int WIDE_MAX_L = 4096;
 
 // best-first bitonic sort of s_sc / s_id [0, n), n a power of two (all threads of the block)
 template <int THREADS>

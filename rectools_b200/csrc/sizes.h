@@ -1,0 +1,11 @@
+// Sizes fixed by the kernels that the host plan (plan.h) also needs.  Plain C++, so that plan.h compiles without CUDA.
+#pragma once
+
+namespace b200 {
+
+constexpr int SEL_WARPS = 8;      // rows (one warp each) per block of the list re-score / merge kernels
+constexpr int WIDE_MAX = 512;     // candidates per row rescore_wide_kernel holds (kp <= 128)
+constexpr int WIDE_MAX_L = 4096;  // candidates per row rescore_wide_large_kernel holds (128 < kp <= 1024)
+constexpr int ROW_SLOTS = 64;     // candidate-list slots per subject row in the fused kernel, split over its lists
+
+}  // namespace b200
