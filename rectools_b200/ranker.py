@@ -335,6 +335,28 @@ def flatten_padded(
     return np.repeat(subject_ids, counts), ids[mask].astype(np.int64), scores[mask]
 
 
+_NEGINF_SCORE = np.uint32(np.float32(-np.finfo(np.float32).max).view(np.uint32) - 1).view(np.float32)
+
+
+def strip_sentinel_tail(ids: np.ndarray, scores: np.ndarray, counts: np.ndarray) -> tp.Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """`_get_mask_for_correct_scores` (rank_implicit.py:107-118) on padded rows, in place: the trailing entries whose score
+    is at most `_get_neginf_score()` (:83-92; -FLT_MAX and its neighbour) leave the row.  The engine drops only -inf, so a
+    real score that low is returned by the kernels and stripped here, as the reference does; its slots become unfilled."""
+    k_out = ids.shape[1] if ids.ndim == 2 else 0
+    if k_out == 0 or len(counts) == 0:
+        return ids, scores, counts
+    rows = np.nonzero(counts > 0)[0]
+    hit = rows[scores[rows, counts[rows] - 1] <= _NEGINF_SCORE]  # (best first: only rows whose last entry is that low)
+    for r in hit:
+        c = int(counts[r])
+        while c > 0 and scores[r, c - 1] <= _NEGINF_SCORE:
+            c -= 1
+        ids[r, c : counts[r]] = -1
+        scores[r, c : counts[r]] = -np.finfo(np.float32).max
+        counts[r] = c
+    return ids, scores, counts
+
+
 class B200Ranker:
     """Ranker backed by the B200 engine.
 
@@ -470,7 +492,7 @@ class B200Ranker:
                 k, sparse_subjects=rows, indptr=indptr, indices=indices, whitelist=whitelist, flags=flags & ~_lib.Q_FORCE_TC
             )
             self.last_stats = self.engine.last_stats
-            return subject_ids, ids, scores, counts
+            return (subject_ids,) + strip_sentinel_tail(ids, scores, counts)
         if getattr(self, "_subjects", None) is not None and self.engine.subjects_owner is not self:
             # another ranker sharing this (cached) engine made its own subject factors resident in the meantime
             self.engine.set_subjects(self._subjects, key=self._subjects_key, owner=self)
@@ -478,7 +500,7 @@ class B200Ranker:
             k, subject_ids=subject_ids, indptr=indptr, indices=indices, whitelist=whitelist, flags=flags
         )
         self.last_stats = self.engine.last_stats
-        return subject_ids, ids, scores, counts
+        return (subject_ids,) + strip_sentinel_tail(ids, scores, counts)
 
     def rank(
         self,

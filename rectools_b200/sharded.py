@@ -26,7 +26,7 @@ import typing as tp
 import numpy as np
 from scipy import sparse
 
-from .ranker import Distance, Engine, _as_distance, _dense_f32, check_whitelist, flatten_padded, prepare_factors
+from .ranker import Distance, Engine, _as_distance, _dense_f32, check_whitelist, flatten_padded, prepare_factors, strip_sentinel_tail
 
 NEG_MAX = -3.4028234663852886e38
 
@@ -510,7 +510,7 @@ class ShardedB200Ranker:
 
     def rank(self, subject_ids, k=None, filter_pairs_csr=None, sorted_object_whitelist=None):
         subject_ids, ids, sc, cnt = self.rank_padded(subject_ids, k, filter_pairs_csr, sorted_object_whitelist)
-        ids, sc, cnt = (t.cpu().numpy() if hasattr(t, "cpu") else np.asarray(t) for t in (ids, sc, cnt))
+        ids, sc, cnt = strip_sentinel_tail(*(t.cpu().numpy() if hasattr(t, "cpu") else np.array(t) for t in (ids, sc, cnt)))
         all_subjects, all_ids, all_scores = flatten_padded(subject_ids, ids, sc, cnt)
         if self.distance == Distance.COSINE:
             all_scores = all_scores / self.subjects_norms[all_subjects]
