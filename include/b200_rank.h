@@ -48,7 +48,7 @@
 extern "C" {
 #endif
 
-#define B200_RANK_ABI_VERSION 4
+#define B200_RANK_ABI_VERSION 5
 
 /* error codes */
 #define B200_OK 0
@@ -251,6 +251,15 @@ typedef struct b200_rank_snapshot {
 
 int b200_rank_get_snapshot(b200_rank_engine* engine, b200_rank_snapshot* meta, float* cand_scores, int32_t* cand_ids,
                            int32_t* cand_counts, float* cand_thr, int32_t* row_exp, int32_t* rows, int32_t* fb_rows);
+
+/* ---- test interface (ABI 5): threshold sharing inside one process.
+ * One process cannot open its own CUDA IPC handles, so b200_rank_peer_import cannot connect engines that live side by
+ * side.  Instead, attach caller-owned device arrays (on the engine's device, uint64 [max_rows] each): `pub` is the array
+ * this engine publishes to, `peers` [n_peers] the arrays it reads.  Each word is (epoch << 32 | fp32 bits) in the
+ * published units, exact score * 2^row_exp (row_exp: the subject row's power-of-two exponent).  The engine never frees
+ * or IPC-closes them.  Refused with more than 8 peers, NULL arrays, arrays that are not device memory of the engine's
+ * device, and on an engine that has exported, imported or attached before. */
+int b200_rank_peer_attach(b200_rank_engine* engine, int64_t max_rows, void* pub, int32_t n_peers, const void* const* peers);
 
 const char* b200_rank_last_error(void);
 int b200_rank_abi_version(void);

@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200_RANK_LIB") or os.path.join(HERE, "libb200rank.so")
 
 # mirrors of the #defines in include/b200_rank.h
-ABI_VERSION = 4
+ABI_VERSION = 5
 OK, E_INVALID, E_CUDA, E_NOMEM, E_UNSUPPORTED = 0, -1, -2, -3, -4
 DIST_DOT, DIST_COSINE = 0, 1
 TC_AUTO, TC_FP16, TC_BF16, TC_OFF = 0, 1, 2, 3
@@ -31,6 +31,7 @@ EXPORTS = (
     "b200_rank_peer_export",
     "b200_rank_peer_import",
     "b200_rank_get_snapshot",
+    "b200_rank_peer_attach",
     "b200_rank_last_error",
     "b200_rank_abi_version",
 )
@@ -179,6 +180,8 @@ def load() -> C.CDLL:
     lib.b200_rank_peer_import.argtypes = [vp, i32, i32, vp]
     lib.b200_rank_get_snapshot.restype = C.c_int
     lib.b200_rank_get_snapshot.argtypes = [vp, C.POINTER(Snapshot), vp, vp, vp, vp, vp, vp, vp]
+    lib.b200_rank_peer_attach.restype = C.c_int
+    lib.b200_rank_peer_attach.argtypes = [vp, i64, vp, i32, C.POINTER(vp)]
     lib.b200_rank_last_error.restype = C.c_char_p
     lib.b200_rank_last_error.argtypes = []
     lib.b200_rank_abi_version.restype = C.c_int

@@ -142,9 +142,11 @@ struct b200_rank_engine {
 
     // threshold sharing with the other ranks of an item-sharded catalogue
     DevBuf peer_pub;
+    unsigned long long* peer_out = nullptr;  // the array this engine publishes to: peer_pub, or the caller's (attached)
     int64_t peer_rows = 0;
     int n_peers = 0;
     void* peer_in[b200::tc::MAX_PEERS] = {nullptr};
+    bool peer_attached = false;  // peer_out / peer_in are caller-owned (b200_rank_peer_attach): never freed or IPC-closed here
 
     // per-call staging / workspace
     DevBuf sub32, sub16, row_exp, rowmap, indptr, indices, wl, obj16_wl;
@@ -177,7 +179,7 @@ struct b200_rank_engine {
     }
     void free_all() {
         for (int i = 0; i < b200::tc::MAX_PEERS; ++i)
-            if (peer_in[i]) cudaIpcCloseMemHandle(peer_in[i]);
+            if (peer_in[i] && !peer_attached) cudaIpcCloseMemHandle(peer_in[i]);
         for (auto* b : all_bufs()) b->release();
         if (h_pinned) cudaFreeHost(h_pinned);
         h_pinned = nullptr;
@@ -662,7 +664,7 @@ void run_tc(Call& c, const TcPass& t) {
         tp.peer_epoch = c.q->peer_epoch;
         tp.peer_exp = E->obj_exp;
         tp.peer_row0 = t.row0;
-        tp.peer_pub = E->peer_pub.as<unsigned long long>();
+        tp.peer_pub = E->peer_out;
         for (int i = 0; i < E->n_peers; ++i) tp.peer_in[i] = reinterpret_cast<const unsigned long long*>(E->peer_in[i]);
     }
     if (t.main) c.S.n_splits = best_splits;
@@ -1232,8 +1234,10 @@ int b200_rank_peer_export(b200_rank_engine* E, int64_t max_rows, void* handle_ou
     try {
         CK(cudaSetDevice(E->device));
         if (E->peer_pub.p) return fail(B200_E_INVALID, "b200_rank_peer_export: already exported (the peers hold the old handle)");
+        if (E->peer_attached) return fail(B200_E_INVALID, "b200_rank_peer_export: the engine has caller-owned arrays attached");
         E->peer_pub.ensure(sizeof(unsigned long long) * max_rows);
         CK(cudaMemset(E->peer_pub.p, 0, E->peer_pub.cap));
+        E->peer_out = E->peer_pub.as<unsigned long long>();
         E->peer_rows = max_rows;
         cudaIpcMemHandle_t h;
         CK(cudaIpcGetMemHandle(&h, E->peer_pub.p));
@@ -1248,8 +1252,7 @@ int b200_rank_peer_import(b200_rank_engine* E, int32_t n_ranks, int32_t self, co
     if (!E || !handles || n_ranks < 1 || self < 0 || self >= n_ranks) return fail(B200_E_INVALID, "b200_rank_peer_import: bad arguments");
     if (n_ranks - 1 > tc::MAX_PEERS) return fail(B200_E_UNSUPPORTED, "b200_rank_peer_import: at most %d ranks", tc::MAX_PEERS + 1);
     std::lock_guard<std::mutex> lock(E->mu);
-    if (!E->peer_pub.p) return fail(B200_E_INVALID, "b200_rank_peer_import: call b200_rank_peer_export first");
-    try {
+    if (!E->peer_pub.p) return fail(B200_E_INVALID, "b200_rank_peer_import: call b200_rank_peer_export first");    try {
         CK(cudaSetDevice(E->device));
         int n = 0;
         for (int r = 0; r < n_ranks; ++r) {
@@ -1264,6 +1267,33 @@ int b200_rank_peer_import(b200_rank_engine* E, int32_t n_ranks, int32_t self, co
     } catch (const CudaError& ce) {
         return fail(B200_E_CUDA, "b200_rank_peer_import: %s failed: %s", ce.what, cudaGetErrorString(ce.e));
     }
+    return B200_OK;
+}
+
+int b200_rank_peer_attach(b200_rank_engine* E, int64_t max_rows, void* pub, int32_t n_peers, const void* const* peers) {
+    if (!E || !pub || !peers || max_rows <= 0 || n_peers < 1) return fail(B200_E_INVALID, "b200_rank_peer_attach: bad arguments");
+    if (n_peers > tc::MAX_PEERS) return fail(B200_E_UNSUPPORTED, "b200_rank_peer_attach: at most %d peers", tc::MAX_PEERS);
+    std::lock_guard<std::mutex> lock(E->mu);
+    if (E->peer_pub.p || E->n_peers > 0)
+        return fail(B200_E_INVALID, "b200_rank_peer_attach: the engine already shares thresholds (b200_rank_peer_export / _import)");
+    try {
+        CK(cudaSetDevice(E->device));
+        for (int i = -1; i < n_peers; ++i) {  // every array must be device memory of the engine's device
+            const void* a = i < 0 ? pub : peers[i];
+            cudaPointerAttributes at{};
+            if (!a || cudaPointerGetAttributes(&at, a) != cudaSuccess || at.type != cudaMemoryTypeDevice || at.device != E->device) {
+                cudaGetLastError();
+                return fail(B200_E_INVALID, "b200_rank_peer_attach: array %d is not device memory of device %d", i + 1, E->device);
+            }
+        }
+    } catch (const CudaError& ce) {
+        return fail(B200_E_CUDA, "b200_rank_peer_attach: %s failed: %s", ce.what, cudaGetErrorString(ce.e));
+    }
+    E->peer_attached = true;
+    E->peer_out = reinterpret_cast<unsigned long long*>(pub);
+    E->peer_rows = max_rows;
+    for (int i = 0; i < tc::MAX_PEERS; ++i) E->peer_in[i] = i < n_peers ? const_cast<void*>(peers[i]) : nullptr;
+    E->n_peers = n_peers;
     return B200_OK;
 }
 

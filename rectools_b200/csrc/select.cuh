@@ -425,9 +425,12 @@ __global__ void __launch_bounds__(SEL_WARPS * 32) rescore_select_kernel(const Se
 
     const double thr = ldexp((double)thr_max, -ex);
     if (p.out_bounds) {
-        // one fp32 ulp of slack: a discarded object whose exact score rounds up to e_k could tie with a smaller id
-        if (lane == 0)
-            p.out_bounds[lrow] = overflow ? INFINITY : (thr_max > -INFINITY ? round_up_f32((thr + eps) * (1.0 + 2.4e-7) + 1e-37) : -INFINITY);
+        // one fp32 ulp of slack: a discarded object whose exact score rounds up to e_k could tie with a smaller id.  The
+        // slack is relative to |thr + eps|: a factor (1 + 2.4e-7) would move a negative bound DOWN, below thr + eps.
+        if (lane == 0) {
+            const double b = thr + eps;
+            p.out_bounds[lrow] = overflow ? INFINITY : (thr_max > -INFINITY ? round_up_f32(b + 2.4e-7 * fabs(b) + 1e-37) : -INFINITY);
+        }
         return;
     }
     if (thr_max > -INFINITY || overflow) {

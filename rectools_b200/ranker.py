@@ -179,6 +179,13 @@ class Engine:
         assert len(blob) == 64 * len(handles)
         _lib.check(self._lib.b200_rank_peer_import(self._h, len(handles), int(self_index), blob))
 
+    def peer_attach(self, pub: tp.Any, peers: tp.Sequence[tp.Any]) -> None:
+        """Test interface: share thresholds inside one process through caller-owned device arrays (torch int64 / uint64
+        tensors of `max_rows` words on the engine's device): `pub` is published to, `peers` are read.  The caller keeps the
+        tensors alive for as long as the engine ranks with B200_Q_SHARED_THRESHOLDS."""
+        ptrs = (C.c_void_p * max(1, len(peers)))(*[t.data_ptr() for t in peers])
+        _lib.check(self._lib.b200_rank_peer_attach(self._h, int(pub.numel()), pub.data_ptr(), len(peers), ptrs))
+
     def candidate_snapshot(self) -> tp.Optional[tp.Dict[str, tp.Any]]:
         """Test interface: the tensor-core pass the last call captured with B200_TC_SNAPSHOT=n set (None: nothing was
         captured).  The metadata of `b200_rank_snapshot` plus numpy arrays: `cand_scores` / `cand_ids`

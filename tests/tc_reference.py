@@ -10,6 +10,12 @@ A row that breaks either premise can be certified with a wrong answer; a list th
 makes rows fail their certificate and take the (exact, slow) re-rank, which no end-to-end comparison notices.
 `check_snapshot` tests the premises, the list contents and the verdict on every row and list of a pass captured with
 B200_TC_SNAPSHOT (`Engine.candidate_snapshot`).  Nothing here calls the engine: it is numpy, in fp64 where it matters.
+
+A pass of an item-sharded call that shares thresholds (B200_Q_SHARED_THRESHOLDS) gives no verdict: it reports a bound
+per row instead, and its lists may prune with the other shards' published thresholds.  With `shared=SharedPass(...)`
+the checker also tests that every threshold is justified by some shard's lists or a valid peer value (I6), restates
+the bound in fp64 (I7) and checks what the pass published for the other shards (I8).  Published words are
+(epoch << 32 | fp32 bits) in units of exact score * 2^row_exp, i.e. a shard's approximate units times 2^-obj_exp.
 """
 from __future__ import annotations
 
@@ -134,7 +140,7 @@ def list_of_positions(n_pos: int, lists_per_row: int, tiles_per_split: int) -> n
 class Report:
     """Violations per invariant (a few examples each) and the observed margins."""
 
-    CLASSES = ("const", "I1", "I2", "I3", "I4", "I5")
+    CLASSES = ("const", "I1", "I2", "I3", "I4", "I5", "I6", "I7", "I8")
 
     def __init__(self) -> None:
         self.violations: tp.Dict[str, tp.List[str]] = {c: [] for c in self.CLASSES}
@@ -144,6 +150,10 @@ class Report:
         self.i3_margin = -np.inf  # max (best discarded A_ref - tau) / accumulation bound
         self.n_rows = self.n_lists = self.n_overflow = self.n_fb = self.n_rejected = self.n_tolerated = 0
         self.rejected: tp.List[int] = []  # batch rows the restated verdict rejects
+        # shared mode: lists of rows with a valid peer value / of those, lists whose final tau IS that value (converted);
+        # rows of the pass whose published slot was written
+        self.n_peer_lists = self.n_adopted = self.n_published = 0
+        self.adopted_rows: tp.List[int] = []  # batch rows with at least one list that adopted the peer value
 
     def add(self, cls: str, msg: str, n: int = 1) -> None:
         self.counts[cls] += n
@@ -159,8 +169,81 @@ class Report:
         return (
             f"rows={self.n_rows} lists={self.n_lists} frac_acc={self.frac_acc:.3g} frac_eps={self.frac_eps:.3g} "
             f"i3_margin={self.i3_margin:.3g} overflow={self.n_overflow} fb={self.n_fb} rejected={self.n_rejected} "
-            f"tolerated={self.n_tolerated}" + (f" VIOLATIONS={bad} {self.violations}" if bad else "")
+            f"tolerated={self.n_tolerated} adopted={self.n_adopted}/{self.n_peer_lists} published={self.n_published}"
+            + (f" VIOLATIONS={bad} {self.violations}" if bad else "")
         )
+
+
+class SharedPass(tp.NamedTuple):
+    """What a threshold-sharing pass adds to its snapshot (all rows in the pass's batch order).
+
+    bounds      [n_sel] fp32   the pass's `out_bounds`
+    epoch                      the call's peer_epoch
+    peer_words  [n_peers, n_sel] uint64  each peer's word of the row, as the pass could read it (arrays are static while
+                               a pass runs when shards run one after another)
+    justify     [n_sel] fp64   published units: the largest `list_justification` of the OTHER shards of the call (-inf: none)
+    pub_before / pub_after  [max_rows] uint64  this shard's published array before / after the call (None: not checked)
+    n_call_rows                rows of the whole call (slots [0, n_call_rows) may be written, the rest must stay untouched)
+    """
+
+    bounds: np.ndarray
+    epoch: int
+    peer_words: np.ndarray
+    justify: np.ndarray
+    pub_before: tp.Optional[np.ndarray] = None
+    pub_after: tp.Optional[np.ndarray] = None
+    n_call_rows: int = 0
+
+
+def peer_word(epoch: int, value: np.ndarray) -> np.ndarray:
+    """(epoch << 32 | fp32 bits) words of published values."""
+    bits = np.asarray(value, np.float32).view(np.uint32).astype(np.uint64)
+    return (np.uint64(epoch) << np.uint64(32)) | bits
+
+
+def split_words(words: np.ndarray) -> tp.Tuple[np.ndarray, np.ndarray]:
+    """(epochs uint32, fp32 values) of published words."""
+    w = np.asarray(words, np.uint64)
+    return (w >> np.uint64(32)).astype(np.uint32), (w & np.uint64(0xFFFFFFFF)).astype(np.uint32).view(np.float32)
+
+
+def round_up_f32(x: np.ndarray) -> np.ndarray:
+    """Smallest fp32 >= x (fp64 in), elementwise; +inf above the fp32 range."""
+    x = np.asarray(x, np.float64)
+    with np.errstate(over="ignore"):
+        f = x.astype(np.float32)
+    low = f.astype(np.float64) < x
+    return np.where(low, np.nextafter(f, np.float32(np.inf)), f).astype(np.float32)
+
+
+def _kth_per_list(A: np.ndarray, elig: np.ndarray, pos_of_list: tp.List[np.ndarray], kc: int) -> np.ndarray:
+    """[rows] max over lists of the kc-th best eligible A of the list (-inf where no list has kc eligible positions)."""
+    out = np.full(A.shape[0], -np.inf)
+    for cols in pos_of_list:
+        if len(cols) < kc:
+            continue
+        v = np.where(elig[:, cols], A[:, cols], -np.inf)
+        out = np.maximum(out, -np.partition(-v, kc - 1, axis=1)[:, kc - 1])
+    return out
+
+
+def list_justification(snap: tp.Dict[str, tp.Any], cat: "Catalogue", sub32: np.ndarray, viewed: sparse.csr_matrix, block: int = 256) -> np.ndarray:
+    """[n_sel] in published units: per row, the largest (K'-th best eligible A_ref of a list + accumulation bound) over the
+    pass's lists, times 2^-obj_exp.  No list of the pass can hold a threshold above it without a peer's help."""
+    n_sel = int(snap["n_sel"])
+    sub32 = np.ascontiguousarray(sub32, dtype=np.float32)
+    lpr = int(snap["nw"]) // 4
+    lop = list_of_positions(cat.n_pos, lpr, max(1, int(snap["tiles_per_split"])))
+    pos_of_list = [np.nonzero(lop == l)[0] for l in range(int(snap["n_lists"]))]
+    _, u16 = subject_operands(sub32, cat.bf16)
+    acc_bound = cat.d_pad * ACC_REL * np.sqrt(np.einsum("ij,ij->i", u16, u16)) * cat.i16_norm_max
+    out = np.empty(n_sel)
+    for r0 in range(0, n_sel, block):
+        r1 = min(n_sel, r0 + block)
+        A = u16[r0:r1] @ cat.i16_pos.T
+        elig = viewed[r0:r1].toarray() == 0
+        out[r0:r1] = _kth_per_list(A, elig, pos_of_list, int(snap["k_cand"])) + acc_bound[r0:r1]
+    return np.ldexp(out, -cat.obj_exp)
 
 
 def _sorted_kth(scores: np.ndarray, ids: np.ndarray, k: int) -> float:
@@ -176,10 +259,12 @@ def check_snapshot(
     excluded: tp.Optional[sparse.csr_matrix] = None,
     prev: tp.Optional[tp.Tuple[np.ndarray, np.ndarray, np.ndarray]] = None,
     block: int = 256,
+    shared: tp.Optional[SharedPass] = None,
 ) -> Report:
     """Check one pass.  `sub32` [n_sel, d] fp32 subject rows and `viewed` [n_sel, n_pos] (Catalogue.viewed_positions) in
     the pass's batch order; `excluded` [n_sel, n_pos]: positions returned by earlier passes (k0 > 0); `prev` (k0 > 0):
-    per batch row (score, LOCAL id, rows with at least k0 results) of output entry k0 - 1, the bound of this pass."""
+    per batch row (score, LOCAL id, rows with at least k0 results) of output entry k0 - 1, the bound of this pass;
+    `shared`: the pass shared thresholds (I5 becomes "no verdict", I6-I8 apply)."""
     rep = Report()
     n_sel, n_pos = int(snap["n_sel"]), cat.n_pos
     nl, stride, kc = int(snap["n_lists"]), int(snap["cand_stride"]), int(snap["k_cand"])
@@ -231,6 +316,7 @@ def check_snapshot(
 
     # exact fp32 scores of every listed candidate (input of the restated verdict)
     cand_rows: tp.List[tp.List[tp.Tuple[np.ndarray, np.ndarray]]] = [[] for _ in range(n_sel)]
+    justify = np.full(n_sel, -np.inf)  # approximate units: the largest K'-th best eligible A_ref of a list + accumulation bound
 
     for r0 in range(0, n_sel, block):
         r1 = min(n_sel, r0 + block)
@@ -291,6 +377,7 @@ def check_snapshot(
         for i in range(r1 - r0):
             sel = order[splits[i] : splits[i + 1]]
             cand_rows[r0 + i].append((exact32[sel], ids[sel]))
+        justify[r0:r1] = _kth_per_list(A, ~(vmask | xmask), pos_of_list, kc) + acc_bound[r0:r1]
         # I3 (P2) and I4: every discarded eligible position lies below the list's final threshold
         elig = ~(vmask | xmask | listed)
         for l in range(nl):
@@ -321,6 +408,10 @@ def check_snapshot(
                     mn = float(np.asarray(snap["cand_scores"])[l, r0 + i, :k].min())
                     if not thr[l, r0 + i] >= mn:
                         rep.add("I4", f"row {r0 + i} list {l}: full list with tau {thr[l, r0 + i]} < its minimum {mn}")
+
+    if shared is not None:
+        _check_shared(rep, snap, shared, thr, overflow, justify, row_exp, eps)
+        return rep
 
     # ---- I5: the verdict of rescore_select_kernel / rescore_wide_kernel, restated in fp64
     pass_row = {int(r): i for i, r in enumerate(np.asarray(snap["rows"]))}
@@ -368,12 +459,79 @@ def check_snapshot(
     return rep
 
 
+def _check_shared(rep: Report, snap: tp.Dict[str, tp.Any], sh: SharedPass, thr: np.ndarray, overflow: np.ndarray, justify: np.ndarray,
+                  row_exp: np.ndarray, eps: np.ndarray) -> None:
+    """I5-I8 of a threshold-sharing pass (see SharedPass); `thr` [lists, n_sel] final thresholds, `justify` / `thr` in
+    approximate units, `eps` in exact units."""
+    n_sel, obj_exp = int(snap["n_sel"]), int(snap["obj_exp"])
+    rows = np.asarray(snap["rows"], np.int64)[:n_sel]
+    # I5: no local verdict in this mode -- the merge's global certificate decides
+    if len(snap["fb_rows"]):
+        rep.add("I5", f"{len(snap['fb_rows'])} rows sent to the fallback by a pass that shares thresholds", len(snap["fb_rows"]))
+    # I6: every threshold is justified by a list of some shard of the call or by a valid peer value
+    ep, val = split_words(np.asarray(sh.peer_words, np.uint64).reshape(-1, n_sel))
+    valid = (ep == np.uint32(sh.epoch)) & ~np.isnan(val)
+    peer = np.where(valid, val.astype(np.float64), -np.inf).max(axis=0) if len(ep) else np.full(n_sel, -np.inf)
+    peer_conv = np.ldexp(peer, obj_exp)  # the pass's approximate units (ldexpf in the kernel: exact in the fp32 range)
+    allowed = np.maximum(np.maximum(justify, np.ldexp(np.asarray(sh.justify, np.float64), obj_exp)), peer_conv)
+    over = thr > allowed[None, :]
+    if over.any():
+        l, i = (int(v[0]) for v in np.nonzero(over))
+        rep.add("I6", f"row {i} list {l}: tau {thr[l, i]:.9g} above every justification {allowed[i]:.9g} (own lists "
+                f"{justify[i]:.9g}, other shards {np.ldexp(sh.justify[i], obj_exp):.9g}, peers {peer_conv[i]:.9g})", int(over.sum()))
+    has_peer = np.isfinite(peer_conv)
+    adopted = has_peer[None, :] & (thr == peer_conv.astype(np.float32)[None, :])
+    rep.n_peer_lists = int(has_peer.sum()) * thr.shape[0]
+    rep.n_adopted = int(adopted.sum())
+    rep.adopted_rows = np.nonzero(adopted.any(axis=0))[0].tolist()
+    # I7: the bound, restated in fp64: smallest fp32 >= x = max tau (exact units) + eps, at most a few ulps above it
+    bounds = np.asarray(sh.bounds, np.float32)[:n_sel]
+    tmax = thr.max(axis=0) if thr.shape[0] else np.full(n_sel, -np.inf)
+    row_over = overflow.any(axis=0)
+    with np.errstate(invalid="ignore", over="ignore"):
+        x = np.ldexp(tmax, -(row_exp + obj_exp)) + eps
+        lo = round_up_f32(x - 1e-12 * np.abs(x))  # (eps: the kernel sums |u|^2 in another order)
+        hi = round_up_f32(x + 2.0**-21 * np.abs(x) + 1e-36)
+    none = ~row_over & (tmax == -np.inf)
+    expect_inf = row_over | (~none & (lo == np.inf))
+    bad = np.zeros(n_sel, bool)
+    bad |= none & (bounds != -np.inf)
+    bad |= expect_inf & (bounds != np.inf)
+    live = ~none & ~expect_inf
+    bad |= live & ~((bounds >= lo) & (bounds <= hi))
+    for i in np.nonzero(bad)[0][:1]:
+        rep.add("I7", f"row {i}: bound {bounds[i]!r}, expected [{lo[i]!r}, {hi[i]!r}] (max tau {tmax[i]!r}, x = {x[i]!r})", int(bad.sum()))
+    # I8: the published array -- the call's epoch, at the absolute row, never above the row's final max tau * 2^-obj_exp
+    if sh.pub_after is None:
+        return
+    before, after = np.asarray(sh.pub_before, np.uint64), np.asarray(sh.pub_after, np.uint64)
+    touched = after != before
+    outside = touched.copy()
+    outside[: sh.n_call_rows] = False
+    if outside.any():
+        rep.add("I8", f"slot {int(np.nonzero(outside)[0][0])} outside the call's {sh.n_call_rows} rows was written", int(outside.sum()))
+    t_ep, t_val = split_words(after)
+    wrong_ep = touched & (t_ep != np.uint32(sh.epoch))
+    if wrong_ep.any():
+        rep.add("I8", f"slot {int(np.nonzero(wrong_ep)[0][0])} written with epoch {int(t_ep[np.nonzero(wrong_ep)[0][0]])}", int(wrong_ep.sum()))
+    mine = touched[rows]
+    rep.n_published = int(mine.sum())
+    with np.errstate(invalid="ignore"):
+        above = mine & ~(t_val[rows].astype(np.float64) <= np.ldexp(tmax, -obj_exp))
+    if above.any():
+        i = int(np.nonzero(above)[0][0])
+        rep.add("I8", f"row {i} (slot {rows[i]}): published {t_val[rows[i]]!r} > max tau * 2^-obj_exp {np.ldexp(tmax[i], -obj_exp)!r}", int(above.sum()))
+
+
 def model_snapshot(
-    cat: Catalogue, sub32: np.ndarray, viewed: sparse.csr_matrix, k_cand: int, kp: int, k_out: int, nw: int = 8, n_splits: int = 1
+    cat: Catalogue, sub32: np.ndarray, viewed: sparse.csr_matrix, k_cand: int, kp: int, k_out: int, nw: int = 8, n_splits: int = 1,
+    peer_floor: tp.Optional[np.ndarray] = None,
 ) -> tp.Dict[str, tp.Any]:
     """What a correct adaptive pass may leave behind, built without the engine: the same partition of the stream, each list
     holding its K' best eligible positions by A_ref, every list's threshold the maximum of the row's full-list minima,
-    the failure rows those of the restated verdict.  Input of the checker's own tests."""
+    the failure rows those of the restated verdict.  `peer_floor` [n_sel] (approximate units, -inf: none): a shared pass
+    whose lists adopted a peer threshold from the start -- lists keep only positions above it, thresholds are at least
+    it, and there is no verdict.  Input of the checker's own tests."""
     n_sel = len(sub32)
     row_exp, u16 = subject_operands(sub32, cat.bf16)
     lpr = nw // 4
@@ -391,6 +549,8 @@ def model_snapshot(
         minima = []
         for l in range(nl):
             cols = np.nonzero((lop == l) & ~vm[r])[0]
+            if peer_floor is not None:
+                cols = cols[A[r, cols] > peer_floor[r]]
             top = cols[np.argsort(-A[r, cols], kind="stable")[:k_cand]]
             counts[l, r] = len(top)
             scores[l, r, : len(top)] = A[r, top]
@@ -398,6 +558,8 @@ def model_snapshot(
             if len(top) == k_cand:
                 minima.append(np.float32(A[r, top].min()))
         thr[:, r] = max(minima) if minima else -np.inf
+        if peer_floor is not None:
+            thr[:, r] = np.maximum(thr[:, r], np.float32(peer_floor[r]))
     snap = {
         "valid": 1, "launch": 1, "nw": nw, "n_lists": nl, "n_splits": n_splits, "tiles_per_split": tps, "n_obj_tiles": n_obj_tiles,
         "cand_stride": stride, "n_pos": cat.n_pos, "rows_pad": rows_pad, "n_sel": n_sel, "k_out": k_out, "k_cand": k_cand, "k0": 0,
@@ -405,6 +567,7 @@ def model_snapshot(
         "max_obj_norm": cat.max_obj_norm, "id_off": cat.id_off, "cand_scores": scores, "cand_ids": ids, "cand_counts": counts,
         "cand_thr": thr, "row_exp": row_exp, "rows": np.arange(n_sel, dtype=np.int32), "fb_rows": np.empty(0, np.int32),
     }
-    snap["fb_rows"] = np.asarray(check_snapshot(snap, cat, sub32, viewed).rejected, dtype=np.int32)
+    if peer_floor is None:
+        snap["fb_rows"] = np.asarray(check_snapshot(snap, cat, sub32, viewed).rejected, dtype=np.int32)
     snap["n_fb"] = len(snap["fb_rows"])
     return snap
