@@ -24,6 +24,7 @@
 #include "prep.cuh"
 #include "select.cuh"
 #include "sparse.cuh"
+#include "large_k_select.cuh"
 #include "fused_topk.cuh"
 
 namespace {
@@ -155,6 +156,7 @@ struct b200_rank_engine {
     DevBuf cand_scores, cand_ids, cand_counts, cand_thr;
     DevBuf part_scores, part_ids;
     DevBuf fb_rows, scratch, excl, carousel, patch;
+    DevBuf lk_scratch;            // sort scratch of the radix selection (k_out > LK_SMEM_PAIRS)
     int32_t* h_pinned = nullptr;  // small pinned scratch (counters)
     std::vector<char> h_patch;    // host copy of re-ranked rows (host-output calls)
 
@@ -168,7 +170,7 @@ struct b200_rank_engine {
     std::vector<DevBuf*> all_bufs() {
         return {&obj32, &obj16, &obj_norms, &objT, &sub32_res, &peer_pub, &sub32, &sub16, &row_exp, &rowmap, &indptr, &indices, &wl,
                 &obj16_wl, &sp_indptr, &sp_indices, &sp_data, &sp_scores, &out_ids, &out_scores, &out_counts, &out_bounds, &cand_scores,
-                &cand_ids, &cand_counts, &cand_thr, &part_scores, &part_ids, &fb_rows, &scratch, &excl, &carousel, &patch,
+                &cand_ids, &cand_counts, &cand_thr, &part_scores, &part_ids, &fb_rows, &scratch, &excl, &carousel, &patch, &lk_scratch,
                 &snap_scores, &snap_ids, &snap_counts, &snap_thr, &snap_row_exp, &snap_rows, &snap_fb};
     }
     std::vector<cudaEvent_t*> call_events() { return {&ev_begin, &ev_staged, &ev_ranked, &ev_end, &ev_from_user, &ev_to_user}; }
@@ -367,6 +369,9 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
         CK(cudaFuncSetAttribute(rescore_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
         CK(cudaFuncSetAttribute(rescore_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
         CK(cudaFuncSetAttribute(rescore_wide_large_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+        // the largest launch of any call (k_out >= LK_SMEM_PAIRS); a fixed maximum: the attribute is shared by every engine
+        // on the device, and smaller launches stay within it
+        CK(cudaFuncSetAttribute(large_k_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lk_smem_bytes(LK_SMEM_PAIRS)));
     } catch (const CudaError& ce) {
         int rc = fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_create: %s failed at line %d: %s",
                       ce.what, ce.line, cudaGetErrorString(ce.e));
@@ -741,9 +746,46 @@ void run_tc(Call& c, const TcPass& t) {
     if (snap) take_snapshot(c, t, tp, t.nw, sp.eps_rel);
 }
 
-// Sparse subjects (EASE): SpMM score rows for bounded row chunks + streaming top-k (sparse.cuh).
+// Radix selection of the nb score rows in sp_scores (large_k_select.cuh): the filter mask, then one CTA per row.  The
+// same row / filter / output conventions as scores_topk_kernel; two launches whatever k is.
+void select_radix(Call& c, const int32_t* rows, int64_t nb, const int64_t* f_indptr, int32_t* o_ids, float* o_scores, int32_t* o_counts,
+                  bool timed) {
+    b200_rank_engine* E = c.E;
+    cudaStream_t st = c.st;
+    if (timed) c.time_begin(1);
+    if (f_indptr) {
+        filter_mask_kernel<<<grid_for(nb * 32, 256), 256, 0, st>>>(E->sp_scores.as<float>(), rows, nb, c.n_pos, c.wl, f_indptr, c.indices,
+                                                                   (int32_t)E->id_offset);
+        CK(cudaGetLastError());
+        c.S.n_launches++;
+    }
+    LargeKParams lp{};
+    lp.scores = E->sp_scores.as<float>();
+    lp.rows = rows;
+    lp.n_rows = nb;
+    lp.n_pos = c.n_pos;
+    lp.pos2obj = c.wl;
+    lp.k_out = c.k_out;
+    lp.smem_pairs = std::min(c.k_out, LK_SMEM_PAIRS);
+    lp.scratch = c.k_out > LK_SMEM_PAIRS ? E->lk_scratch.as<uint32_t>() : nullptr;
+    lp.out_ids = o_ids;
+    lp.out_scores = o_scores;
+    lp.out_counts = o_counts;
+    const size_t smem = lk_smem_bytes(c.k_out);
+    large_k_select_kernel<<<(unsigned)nb, LK_THREADS, smem, st>>>(lp);
+    CK(cudaGetLastError());
+    if (timed) c.time_end();
+    c.S.n_launches++;
+}
+
+// Score rows per chunk of paths 2 / 3: select_row_bytes each within SELECT_CHUNK_BYTES (at least one row).
+int64_t select_chunk_rows(const Call& c, int64_t nr, Select sel) {
+    return std::max<int64_t>(1, std::min<int64_t>(nr, SELECT_CHUNK_BYTES / std::max<int64_t>(select_row_bytes(c.n_pos, c.k_out, sel), 1)));
+}
+
+// Sparse subjects (EASE): SpMM score rows for bounded row chunks + the plan's selection (sparse.cuh, large_k_select.cuh).
 void run_sparse(Call& c, const int64_t* sp_indptr, const int32_t* sp_indices, const float* sp_data, int64_t nr, const int64_t* f_indptr,
-                int32_t* o_ids, float* o_scores, int32_t* o_counts) {
+                int32_t* o_ids, float* o_scores, int32_t* o_counts, Select sel) {
     b200_rank_engine* E = c.E;
     cudaStream_t st = c.st;
     if (!E->objT.p && E->n_obj > 0) {  // transposed master copy, built once
@@ -753,8 +795,9 @@ void run_sparse(Call& c, const int64_t* sp_indptr, const int32_t* sp_indices, co
         CK(cudaGetLastError());
         c.S.n_launches++;
     }
-    const int64_t rows_max = std::max<int64_t>(1, std::min<int64_t>(nr, ((int64_t)1 << 30) / std::max<int64_t>(4 * c.n_pos, 1)));
+    const int64_t rows_max = select_chunk_rows(c, nr, sel);
     E->sp_scores.ensure(sizeof(float) * (size_t)rows_max * c.n_pos);
+    if (sel == Select::RADIX && c.k_out > LK_SMEM_PAIRS) E->lk_scratch.ensure((size_t)16 * rows_max * c.k_out);
     for (int64_t b0 = 0; b0 < nr; b0 += rows_max) {
         const int64_t nb = std::min(rows_max, nr - b0);
         c.time_begin(0);
@@ -763,6 +806,10 @@ void run_sparse(Call& c, const int64_t* sp_indptr, const int32_t* sp_indices, co
         CK(cudaGetLastError());
         c.time_end();
         c.S.n_launches++;
+        if (sel == Select::RADIX) {
+            select_radix(c, nullptr, nb, f_indptr ? f_indptr + b0 : nullptr, o_ids + b0 * c.k_out, o_scores + b0 * c.k_out, o_counts + b0, true);
+            continue;
+        }
         for (int k0 = 0; k0 < c.k_out; k0 += 32) {
             c.time_begin(1);
             scores_topk_kernel<<<grid_for(nb * 32, 256), 256, 0, st>>>(E->sp_scores.as<float>(), nullptr, nb, c.n_pos, c.wl, f_indptr ? f_indptr + b0 : nullptr,
@@ -775,15 +822,17 @@ void run_sparse(Call& c, const int64_t* sp_indptr, const int32_t* sp_indices, co
     }
 }
 
-// Dense subjects with k > 128: one exhaustive scoring of bounded row chunks into HBM + k / 32 streaming selection passes.
+// Dense subjects with k > 128: one exhaustive scoring of bounded row chunks into HBM + the plan's selection (k / 32
+// streaming passes, or the radix selection).
 // rows == nullptr: rows [0, nr) of the given base pointers (a chunk's slices);  otherwise the nr logical rows listed in
 // `rows` (absolute rows of the call, whole-call base pointers): the re-rank of rows a k > 128 wide pass could not certify.
 void run_dense_large_k(Call& c, const int32_t* rows, const float* sub32, const int64_t* rowmap, const int64_t* f_indptr, int64_t nr,
-                       int32_t* o_ids, float* o_scores, int32_t* o_counts, bool timed) {
+                       int32_t* o_ids, float* o_scores, int32_t* o_counts, bool timed, Select sel) {
     b200_rank_engine* E = c.E;
     cudaStream_t st = c.st;
-    const int64_t rows_max = std::max<int64_t>(32, std::min<int64_t>(nr, ((int64_t)1 << 30) / std::max<int64_t>(4 * c.n_pos, 1)) / 32 * 32);
+    const int64_t rows_max = std::max<int64_t>(32, select_chunk_rows(c, nr, sel) / 32 * 32);
     E->sp_scores.ensure(sizeof(float) * (size_t)rows_max * c.n_pos);
+    if (sel == Select::RADIX && c.k_out > LK_SMEM_PAIRS) E->lk_scratch.ensure((size_t)16 * rows_max * c.k_out);
     for (int64_t b0 = 0; b0 < nr; b0 += rows_max) {
         const int64_t nb = std::min(rows_max, nr - b0);
         const int blocks_x = grid_for(nb, 32);
@@ -798,6 +847,10 @@ void run_dense_large_k(Call& c, const int32_t* rows, const float* sub32, const i
         if (timed) c.time_end();
         c.S.n_launches++;
         const int64_t ob = rows ? 0 : b0;  // outputs / filter rows: listed rows are absolute
+        if (sel == Select::RADIX) {
+            select_radix(c, rl, nb, f_indptr ? f_indptr + ob : nullptr, o_ids + ob * c.k_out, o_scores + ob * c.k_out, o_counts + ob, timed);
+            continue;
+        }
         for (int k0 = 0; k0 < c.k_out; k0 += 32) {
             if (timed) c.time_begin(1);
             scores_topk_kernel<<<grid_for(nb * 32, 256), 256, 0, st>>>(E->sp_scores.as<float>(), rl, nb, c.n_pos, c.wl,
@@ -1059,9 +1112,9 @@ void main_pass(Call& c, int64_t r0, int64_t r1) {
         CK(cudaGetLastError());
         c.S.n_launches++;
         if (P.path == Path::SPARSE) {
-            run_sparse(c, c.sp_indptr + r0, c.sp_indices, c.sp_data, nr, ip, oi, os, oc);
-        } else if (P.path == Path::DENSE_LARGE_K) {  // materialised exhaustive scores + streaming selection passes
-            run_dense_large_k(c, nullptr, sub, rm, ip, nr, oi, os, oc, true);
+            run_sparse(c, c.sp_indptr + r0, c.sp_indices, c.sp_data, nr, ip, oi, os, oc, P.select);
+        } else if (P.path == Path::DENSE_LARGE_K) {  // materialised exhaustive scores + the plan's selection
+            run_dense_large_k(c, nullptr, sub, rm, ip, nr, oi, os, oc, true, P.select);
         } else if (P.path == Path::EXACT) {
             run_exact(c, nullptr, nr, sub, rm, ip, oi, os, oc, 0, k_out, true);
         } else {
@@ -1111,7 +1164,7 @@ void rerank_failures(Call& c, cudaStream_t cs) {
         init_rows_kernel<<<grid_for(n_fb * k_out, 256), 256, 0, c.st>>>(c.o_ids, c.o_scores, c.o_counts, c.fb_main, n_fb, k_out);
         CK(cudaGetLastError());
         c.S.n_launches++;
-        run_dense_large_k(c, c.fb_main, c.sub32, c.rowmap, c.indptr, n_fb, c.o_ids, c.o_scores, c.o_counts, false);
+        run_dense_large_k(c, c.fb_main, c.sub32, c.rowmap, c.indptr, n_fb, c.o_ids, c.o_scores, c.o_counts, false, Select::PASSES);
         c.S.n_exact_rows += n_fb;
     } else {
         rerank_rows(c, c.fb_main, n_fb);

@@ -29,6 +29,8 @@ struct Hooks {
     int64_t chunk_rows = 0;     // B200_CHUNK_ROWS: row chunk of host-input calls (0: 8 waves; at least 256)
     int wide_budget_mb = 2048;  // B200_WIDE_BUDGET_MB: device memory for the append lists of k > 128
     int tc_snapshot = 0;        // B200_TC_SNAPSHOT: the fused-kernel launch whose state is kept (0: none)
+    int select = 1;             // B200_SELECT: paths 2 / 3 select with 0 the streaming passes for every k, 2 the radix
+                                // selection for every k (cross-checks); 1 the radix selection for k > 1024 only
 };
 
 inline Hooks read_hooks() {
@@ -47,6 +49,7 @@ inline Hooks read_hooks() {
     if (const char* v = std::getenv("B200_CHUNK_ROWS")) h.chunk_rows = std::max<int64_t>(256, std::atoll(v));
     h.wide_budget_mb = get("B200_WIDE_BUDGET_MB", h.wide_budget_mb);
     h.tc_snapshot = get("B200_TC_SNAPSHOT", h.tc_snapshot);
+    h.select = get("B200_SELECT", h.select);
     return h;
 }
 
@@ -109,9 +112,23 @@ enum class TcMode {
     MULTI_PASS,  // 24 < k without the wide mode: certified passes of 20 results for every row
 };
 
+// How paths 2 and 3 select from their materialised score rows.
+enum class Select {
+    PASSES,  // ceil(k_out / 32) streaming passes of scores_topk_kernel over every row
+    RADIX,   // large_k_select_kernel: radix select + one sort of the k_out survivors (k_out > 1024)
+};
+
+// Bytes per row of a path-2 / path-3 row chunk: the fp32 score row and, when the radix selection sorts more survivors than
+// its shared memory holds, the sort's global scratch (4 words per entry).  Chunks keep within 1 GiB of these.
+inline int64_t select_row_bytes(int64_t n_pos, int64_t k_out, Select sel) {
+    return 4 * n_pos + (sel == Select::RADIX && k_out > LK_SMEM_PAIRS ? 16 * k_out : 0);
+}
+constexpr int64_t SELECT_CHUNK_BYTES = (int64_t)1 << 30;
+
 struct CallPlan {
     int k_out = 0;
     Path path = Path::EXACT;
+    Select select = Select::PASSES;  // paths SPARSE / DENSE_LARGE_K (the re-rank of rows a wide pass rejects: PASSES)
     TcMode mode = TcMode::NARROW;  // path TC only
     bool bf16 = false;             // operand type of the tensor-core passes
     int nw = 8;                    // epilogue warps of the main pass
@@ -191,6 +208,8 @@ inline CallPlan plan_call(const CallShape& s, const Hooks& h) {
     if (shared && use_tc && k > 24) return refuse("B200_Q_SHARED_THRESHOLDS needs k <= 24");
 
     p.path = s.sparse ? Path::SPARSE : use_tc ? Path::TC : k > 128 ? Path::DENSE_LARGE_K : Path::EXACT;
+    if ((p.path == Path::SPARSE || p.path == Path::DENSE_LARGE_K) && (h.select == 2 || (h.select != 0 && k > 1024)))
+        p.select = Select::RADIX;
     p.chunk = s.n_rows;
     if (p.tc()) {
         p.mode = wide ? TcMode::WIDE : wide_l ? TcMode::WIDE_L : k > 24 ? TcMode::MULTI_PASS : TcMode::NARROW;
