@@ -149,7 +149,7 @@ typedef struct b200_rank_stats {
     int64_t d2h_bytes;
     int32_t n_chunks;        /* row chunks of the copy / compute pipeline (1: call not chunked) */
     int32_t n_tc_launches;   /* launches of the fused tensor-core kernel summed in ms_main (main pass, second chance, re-rank passes) */
-    int32_t epi_warps;       /* epilogue warps per CTA of the fused kernel (8 or 16) */
+    int32_t epi_warps;       /* epilogue warps per CTA of the fused kernel: always 8 */
     int32_t wide;            /* 1: single-pass wide mode (24 < k <= 1024) */
     float ms_select;         /* CUDA-event time of the fp64 re-score / selection kernels */
     int32_t reserved;
@@ -215,7 +215,7 @@ int b200_rank_peer_import(b200_rank_engine* engine, int32_t n_ranks, int32_t sel
  * than one row chunk counts one main-pass launch per chunk, so n = 1 snapshots the first chunk.  Unset (or 0), nothing
  * is copied and nothing is allocated.  The state of a pass:
  *   cand_scores / cand_ids  [n_lists][rows_pad][cand_stride]  approximate scores (units of 2^(row_exp + obj_exp)) and
- *                           LOCAL object ids; list l = split * (nw / 4) + column group; entries beyond the count unused
+ *                           LOCAL object ids; list l = split * 2 + column group; entries beyond the count unused
  *   cand_counts / cand_thr  [n_lists][rows_pad]  entries produced (wide mode: > cand_stride = overflow) and the list's
  *                           final pruning threshold
  *   row_exp                 [rows_pad]  power-of-two exponent of each subject row (batch order of the pass)
@@ -226,8 +226,8 @@ int b200_rank_peer_import(b200_rank_engine* engine, int32_t n_ranks, int32_t sel
 typedef struct b200_rank_snapshot {
     int32_t valid;
     int32_t launch;          /* n of B200_TC_SNAPSHOT */
-    int32_t nw;              /* epilogue warps of the pass (8 or 16): nw / 4 candidate lists per row and object split */
-    int32_t n_lists;         /* n_splits * nw / 4 */
+    int32_t nw;              /* epilogue warps of the pass: always 8, two candidate lists per row and object split */
+    int32_t n_lists;         /* n_splits * 2 */
     int32_t n_splits;        /* object splits: split s streams tiles [s * tiles_per_split, (s + 1) * tiles_per_split) */
     int32_t tiles_per_split;
     int32_t n_obj_tiles;     /* tiles of 256 object positions */

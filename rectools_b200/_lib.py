@@ -81,7 +81,7 @@ class Stats(C.Structure):
         ("d2h_bytes", C.c_int64),
         ("n_chunks", C.c_int32),
         ("n_tc_launches", C.c_int32),
-        ("epi_warps", C.c_int32),
+        ("epi_warps", C.c_int32),  # always 8 (one fused-kernel geometry)
         ("wide", C.c_int32),
         ("ms_select", C.c_float),
         ("reserved", C.c_int32),
@@ -113,7 +113,7 @@ class Snapshot(C.Structure):
     _fields_ = [
         ("valid", C.c_int32),
         ("launch", C.c_int32),
-        ("nw", C.c_int32),
+        ("nw", C.c_int32),  # always 8: two lists per row and object split
         ("n_lists", C.c_int32),
         ("n_splits", C.c_int32),
         ("tiles_per_split", C.c_int32),

@@ -245,17 +245,16 @@ void prepare_objects(b200_rank_engine* E, int tc_mode) {
     CK(cudaStreamSynchronize(E->st));
 }
 
-// Shared-memory plan of the fused kernel: subject blocks + object ring + the fixed part of FusedCfg<NW>.
+// Shared-memory plan of the fused kernel: subject blocks + object ring + the fixed part of FusedCfg.
 struct TcPlan {
     int kblocks, n_stages, smem_bytes;
     bool ok;
 };
 
-template <int NW>
 TcPlan plan_fused(int d_pad) {
     TcPlan pl{};
     pl.kblocks = d_pad / tc::KBLK;
-    const int fixed = pl.kblocks * tc::BLK_BYTES + tc::FusedCfg<NW>::FIXED_BYTES;
+    const int fixed = pl.kblocks * tc::BLK_BYTES + tc::FusedCfg::FIXED_BYTES;
     int stages = (tc::SMEM_LIMIT - fixed) / tc::OBJ_BLK_BYTES;
     if (stages > tc::MAX_STAGES) stages = tc::MAX_STAGES;
     pl.ok = stages >= 2;
@@ -265,32 +264,31 @@ TcPlan plan_fused(int d_pad) {
 }
 
 // The instantiations of the fused kernel: the function (for its attributes) and a launcher.
-template <int NW, bool WIDE, bool PEERS, bool BF16>
+template <bool WIDE, bool PEERS, bool BF16>
 void launch_fused(int grid, int smem, cudaStream_t st, const CUtensorMap& tm_sub, const CUtensorMap& tm_obj, const tc::TcParams& tp) {
-    tc::fused_topk_kernel<NW, WIDE, PEERS, BF16><<<grid, tc::FusedCfg<NW>::threads(PEERS), smem, st>>>(tm_sub, tm_obj, tp);
+    tc::fused_topk_kernel<WIDE, PEERS, BF16><<<grid, tc::FusedCfg::threads(PEERS), smem, st>>>(tm_sub, tm_obj, tp);
 }
 
 struct FusedKernel {
     const void* fn;
-    decltype(&launch_fused<8, false, false, false>) launch;
+    decltype(&launch_fused<false, false, false>) launch;
 };
 
-template <int NW, bool WIDE, bool PEERS, bool BF16>
+template <bool WIDE, bool PEERS, bool BF16>
 FusedKernel fused_entry() {
-    return {(const void*)tc::fused_topk_kernel<NW, WIDE, PEERS, BF16>, launch_fused<NW, WIDE, PEERS, BF16>};
+    return {(const void*)tc::fused_topk_kernel<WIDE, PEERS, BF16>, launch_fused<WIDE, PEERS, BF16>};
 }
 
-// [nw == 16][bf16][plain, wide, peers]
-const FusedKernel FUSED_KERNELS[2][2][3] = {
-    {{fused_entry<8, false, false, false>(), fused_entry<8, true, false, false>(), fused_entry<8, false, true, false>()},
-     {fused_entry<8, false, false, true>(), fused_entry<8, true, false, true>(), fused_entry<8, false, true, true>()}},
-    {{fused_entry<16, false, false, false>(), fused_entry<16, true, false, false>(), fused_entry<16, false, true, false>()},
-     {fused_entry<16, false, false, true>(), fused_entry<16, true, false, true>(), fused_entry<16, false, true, true>()}},
+// [bf16][plain, wide, peers]
+const FusedKernel FUSED_KERNELS[2][3] = {
+    {fused_entry<false, false, false>(), fused_entry<true, false, false>(), fused_entry<false, true, false>()},
+    {fused_entry<false, false, true>(), fused_entry<true, false, true>(), fused_entry<false, true, true>()},
 };
+static_assert(CallPlan::nw == tc::FusedCfg::EPILOGUE_WARPS, "the plan reports the fused kernel's epilogue warps");
 
 // Wide wins over peers: no kernel has both (threshold sharing needs k <= 24, the wide mode k > 24).
-const FusedKernel& fused_kernel(int nw, bool wide, bool peers, bool bf16) {
-    return FUSED_KERNELS[nw == 16][bf16][wide ? 1 : peers ? 2 : 0];
+const FusedKernel& fused_kernel(bool wide, bool peers, bool bf16) {
+    return FUSED_KERNELS[bf16][wide ? 1 : peers ? 2 : 0];
 }
 
 int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int64_t n_objects, int32_t d, int32_t distance,
@@ -356,14 +354,13 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
         if (tc_mode == B200_TC_AUTO && dtype == B200_DT_BF16) tc_mode = B200_TC_BF16;  // bf16 factors: the tensor-core copy is exact
         prepare_objects(E, tc_mode);
         if (E->tc_dtype != B200_TC_OFF) {
-            const TcPlan p8 = plan_fused<8>(E->d_pad), p16 = plan_fused<16>(E->d_pad);
-            if (!p8.ok || !p16.ok) {
+            const TcPlan pl = plan_fused(E->d_pad);
+            if (!pl.ok) {
                 E->tc_dtype = B200_TC_OFF;
             } else {
-                for (int w = 0; w < 2; ++w)
-                    for (const auto& by_type : FUSED_KERNELS[w])
-                        for (const FusedKernel& k : by_type)
-                            CK(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (w ? p16 : p8).smem_bytes));
+                for (const auto& by_type : FUSED_KERNELS)
+                    for (const FusedKernel& k : by_type)
+                        CK(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, pl.smem_bytes));
             }
         }
         CK(cudaFuncSetAttribute(rescore_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
@@ -516,7 +513,6 @@ struct TcPass {
     float* o_scores = nullptr;
     int32_t* o_counts = nullptr;
     float* o_bounds = nullptr;  // shared-threshold mode: bounds out, no verdict
-    int nw = 8;                 // epilogue warps
     int kc = 12;                // K' per list (<= the kernel's list capacity)
     int k0 = 0, kp = 0;         // this pass produces entries [k0, k0 + kp)
     TcMode mode = TcMode::NARROW;  // WIDE / WIDE_L: the plan's single wide pass (frozen threshold + global append)
@@ -529,9 +525,9 @@ struct TcPass {
 
 // B200_TC_SNAPSHOT: copy the state the fused kernel and the re-score of this pass left behind (after both launches,
 // before the next pass reuses the buffers).  The failure counter was saved before the pass (snap_fb[0]).
-void take_snapshot(Call& c, const TcPass& t, const tc::TcParams& tp, int nw, float eps_rel) {
+void take_snapshot(Call& c, const TcPass& t, const tc::TcParams& tp, float eps_rel) {
     b200_rank_engine* E = c.E;
-    const int n_lists = tp.n_splits * (nw / 4);
+    const int n_lists = tp.n_splits * tc::FusedCfg::NLIST;
     const size_t n_lr = (size_t)n_lists * tp.rows_pad, n_cand = n_lr * tp.cand_stride;
     auto d2d = [&](DevBuf& dst, const void* src, size_t bytes) {
         dst.ensure(std::max<size_t>(bytes, 16));
@@ -552,7 +548,7 @@ void take_snapshot(Call& c, const TcPass& t, const tc::TcParams& tp, int nw, flo
     m = b200_rank_snapshot{};
     m.valid = 1;
     m.launch = c.n_tc;
-    m.nw = nw;
+    m.nw = tc::FusedCfg::EPILOGUE_WARPS;
     m.n_lists = n_lists;
     m.n_splits = tp.n_splits;
     m.tiles_per_split = tp.tiles_per_split;
@@ -581,8 +577,8 @@ void run_tc(Call& c, const TcPass& t) {
     const bool bf16 = c.plan.bf16;
     const bool wide = t.mode != TcMode::NARROW;
     const int d = c.d;
-    const int nlist = t.nw / 4;
-    const TcPlan pl = t.nw == 8 ? plan_fused<8>(E->d_pad) : plan_fused<16>(E->d_pad);
+    const int nlist = tc::FusedCfg::NLIST;
+    const TcPlan pl = plan_fused(E->d_pad);
     const int64_t rows_pad = round_up(t.n_sel, 2 * tc::TILE_M);
     // subjects -> 16-bit, per-row power-of-two scale
     E->sub16.ensure((size_t)rows_pad * E->d_pad * 2);
@@ -693,7 +689,7 @@ void run_tc(Call& c, const TcPass& t) {
         CK(cudaMemcpyAsync(E->snap_fb.p, t.fb_count, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
     }
     c.time_begin(0);
-    fused_kernel(t.nw, wide, t.peers && tp.n_peers > 0, bf16).launch(grid, pl.smem_bytes, st, tm_sub, tm_obj, tp);
+    fused_kernel(wide, t.peers && tp.n_peers > 0, bf16).launch(grid, pl.smem_bytes, st, tm_sub, tm_obj, tp);
     CK(cudaGetLastError());
     c.time_end();
     c.S.n_launches++;
@@ -743,7 +739,7 @@ void run_tc(Call& c, const TcPass& t) {
     CK(cudaGetLastError());
     c.time_end();
     c.S.n_launches++;
-    if (snap) take_snapshot(c, t, tp, t.nw, sp.eps_rel);
+    if (snap) take_snapshot(c, t, tp, sp.eps_rel);
 }
 
 // Radix selection of the nb score rows in sp_scores (large_k_select.cuh): the filter mask, then one CTA per row.  The
@@ -1065,7 +1061,6 @@ void rerank_rows(Call& c, const int32_t* rows, int64_t n_sel) {
         t.o_ids = c.o_ids;
         t.o_scores = c.o_scores;
         t.o_counts = c.o_counts;
-        t.nw = 8;
         t.kc = std::min(32, std::max(kc_pass - (k_pass - kp), kp));
         t.k0 = k0;
         t.kp = kp;
@@ -1127,7 +1122,6 @@ void main_pass(Call& c, int64_t r0, int64_t r1) {
             t.o_scores = os;
             t.o_counts = oc;
             t.o_bounds = c.o_bounds ? c.o_bounds + r0 : nullptr;
-            t.nw = P.nw;
             t.kc = P.k_cand;
             t.mode = P.mode;
             t.peers = P.peers;

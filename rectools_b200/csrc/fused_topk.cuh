@@ -8,11 +8,10 @@
 //   -> deferred, bounded steps: filter_pairs_csr lookup through a prefetched 4-entry window, candidate-list insertion.
 // Score rows never reach HBM: only the K' best (score, id) pairs per row and column group are written.
 //
-// NW = epilogue warps per CTA; column group g of a tile is made of the quarters g, g + NW / 4, ...:
-//   8  : two quarters (128 columns) per warp and tile, two candidate lists per row (32 slots each)
-//   16 : one quarter (64 columns) per warp and tile, four lists per row (16 slots each)
-// Warps 0-3: the MMA warp group (thread 0 also issues every TMA load); warps 4 .. 4 + NW - 1: epilogue; with PEERS two
-// more warps poll the other ranks' published thresholds over NVLink and publish this rank's.
+// Warps 0-3: the MMA warp group (thread 0 also issues every TMA load); warps 4-11: the eight epilogue warps; with PEERS
+// two more warps poll the other ranks' published thresholds over NVLink and publish this rank's.  Epilogue warp w reads
+// the row quarter w & 3 of column group w >> 2: group g of a tile is made of its quarters g and g + 2 (128 columns), and
+// each group has its own candidate list per row (two lists of 32 slots).
 // The two CTAs of a pair work on the same object tiles in the same order; the odd CTA waits for the start tile the even
 // one publishes through global memory, so the pair is launched as a cluster of two (co-scheduled by the hardware).
 //
@@ -34,20 +33,19 @@ namespace tc {
 
 constexpr uint32_t TAG_NONE = 0xffffffffu, TAG_DONE = 0xfffffffeu;  // exchange-slot tags no work item carries
 
-template <int NW>
 struct FusedCfg {
-    static_assert(NW == 8 || NW == 16, "8 or 16 epilogue warps");
     static constexpr int EPI0 = 4;                    // first epilogue warp; (warp & 3) is its row quarter
+    static constexpr int EPILOGUE_WARPS = 8;          // epilogue warps
     static constexpr int HELPERS = 2;                 // peer-threshold warps behind the epilogue (PEERS kernels only)
-    static constexpr int threads(bool peers) { return (EPI0 + NW + (peers ? HELPERS : 0)) * 32; }
-    static constexpr int COLS = 1024 / NW;            // accumulator columns per epilogue thread and tile
-    static constexpr int NLIST = NW / 4;              // column groups = candidate lists per row
+    static constexpr int threads(bool peers) { return (EPI0 + EPILOGUE_WARPS + (peers ? HELPERS : 0)) * 32; }
+    static constexpr int COLS = 128;                  // accumulator columns per epilogue thread and tile
+    static constexpr int NLIST = 2;                   // column groups = candidate lists per row
     static constexpr int NQ = COLS / QUART_N;         // staged quarters per epilogue thread and tile
-    static constexpr int SLOTS = ROW_SLOTS / NLIST;   // list capacity (K' <= SLOTS)
-    static constexpr int Q = NW == 8 ? 8 : 4;         // deferred hits per thread (ring FIFO)
-    static constexpr int QSTRIDE = NW * 32 * 8;       // bytes between FIFO slots: [slot][epilogue thread] x (score, position)
+    static constexpr int SLOTS = LIST_SLOTS;          // list capacity (K' <= SLOTS)
+    static constexpr int Q = 8;                       // deferred hits per thread (ring FIFO)
+    static constexpr int QSTRIDE = EPILOGUE_WARPS * 32 * 8;  // bytes between FIFO slots: [slot][epilogue thread] x (score, position)
     static constexpr int QBYTES = Q * QSTRIDE;
-    static constexpr int BACKLOG = NW == 8 ? 4 : 2;   // a row with this many pending hits gets a step at once
+    static constexpr int BACKLOG = 4;                 // a row with this many pending hits gets a step at once
     static constexpr int PERIOD = 16;                 // otherwise deferred work runs every PERIOD-th tile (power of two)
     static constexpr int LIST_BYTES = NLIST * TILE_M * SLOTS * 4;  // one of the two arrays (scores / ids): 32 KiB
     static constexpr int THR_BYTES = (NLIST + 1) * TILE_M * 8;     // (tag, threshold) per list + one slot for the peers' maximum
@@ -184,10 +182,10 @@ __device__ __forceinline__ void store_half(const uint32_t (&d)[32], uint32_t stg
 // scores + ids | FIFOs | thresholds [NLIST + 1][128] | barriers.
 // WIDE / PEERS compile the wide mode (threshold freeze + global append) and the peer-threshold exchange in; the plain
 // instantiation carries neither in its tile loop.  BF16 selects the MMA operand type.
-template <int NW, bool WIDE, bool PEERS, bool BF16>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(FusedCfg<NW>::threads(PEERS), 1)
+template <bool WIDE, bool PEERS, bool BF16>
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(FusedCfg::threads(PEERS), 1)
 fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_constant__ CUtensorMap tm_obj, const TcParams p) {
-    using Cfg = FusedCfg<NW>;
+    using Cfg = FusedCfg;
     constexpr int NLIST = Cfg::NLIST, SLOTS = Cfg::SLOTS, NQ = Cfg::NQ, QN = Cfg::Q, QS = Cfg::QSTRIDE;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -290,10 +288,9 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
         // the hand-off of one half overlaps the MMAs of the other --
         //   G0(q), G1(q) | wait<1>, store half 0 of q, G0(q + 1) | wait<1>, release q's blocks, store half 1 of q,
         //   G1(q + 1) | ...
-        // The ring slots of quarter q are refilled once G1(q), their second reader, has retired.  (The 16-warp geometry
-        // leaves the MMA warp group 80-96 registers: it keeps the per-k-block schedule below, which spills less there.)
+        // The ring slots of quarter q are refilled once G1(q), their second reader, has retired.
         constexpr int PKB = 2;
-        const bool pipelined = NW == 8 && KB == PKB && 2 * PKB <= NS;
+        const bool pipelined = KB == PKB && 2 * PKB <= NS;
         auto advance = [&]() {  // ring position of the next quarter's first block
             stage += (uint32_t)PKB;
             if (stage >= (uint32_t)NS) {
@@ -384,7 +381,7 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
                 }
             }
         }
-    } else if (warp < Cfg::EPI0 + NW) {
+    } else if (warp < Cfg::EPI0 + Cfg::EPILOGUE_WARPS) {
         // ===================================================================== epilogue: select candidates
         const int ew = warp - Cfg::EPI0;
         const int colg = ew >> 2, quarter = warp & 3;  // column group of the tile / row quarter of the CTA's 128 rows
@@ -404,7 +401,7 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
         const int kc = p.k_cand;  // (<= SLOTS, guaranteed by the host; a visible bound makes the compiler unroll the list scans fully and spill)
         const bool dbg_skip = p.debug_mode == 2;
         const bool peers = PEERS && p.n_peers > 0;
-        const uint32_t other_thr = pin(thr_row + (uint32_t)(colg ^ 1) * (TILE_M * 8));  // two lists per row: the other one's slot
+        const uint32_t other_thr = pin(thr_row + (uint32_t)(colg ^ 1) * (TILE_M * 8));  // the other list of the row
         uint32_t tpar = 0, work_tag = 0;  // parity of the quarter barriers (one phase per tile)
         for (int w = pair; w < n_work; w += n_pairs, ++work_tag) {
             const int split = w / p.n_row_tiles, rt = w - split * p.n_row_tiles;
@@ -446,24 +443,16 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
             int t = ts;
             uint32_t pos_t = (uint32_t)ts * TILE_N + (uint32_t)(colg * QUART_N);
             for (int it = 0; it < nt; ++it) {
-                // exchange thresholds with the threads that own the other column groups of this row and with the other
+                // exchange thresholds with the thread that owns the other column group of this row and with the other
                 // ranks (monotone, racy by design: a stale value is only a weaker bound; the tag keeps a value of the
                 // previous work item out)
                 {
                     sts_thr(my_thr, work_tag, rs.thr);
-                    if constexpr (NLIST == 2) {
+                    {
                         uint32_t ptag;
                         float pthr;
                         lds_thr(other_thr, ptag, pthr);
                         if (ptag == work_tag) rs.thr = fmaxf(rs.thr, pthr);
-                    } else {
-#pragma unroll
-                        for (int l = 0; l < NLIST; ++l) {  // (reading the own slot back is cheaper than a branch)
-                            uint32_t ptag;
-                            float pthr;
-                            lds_thr(thr_row + (uint32_t)l * (TILE_M * 8), ptag, pthr);
-                            if (ptag == work_tag) rs.thr = fmaxf(rs.thr, pthr);
-                        }
                     }
                     if constexpr (PEERS) {
                         if (peers) {
@@ -559,7 +548,7 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
         // slots, publish their maximum to this rank's global array, read the other ranks' published values (NVLink peer
         // loads, latency irrelevant here), leave their maximum in the row's extra exchange slot.  All values are monotone
         // lower bounds of the row's final threshold: a stale one is only weaker, never wrong.
-        const int h = (warp - Cfg::EPI0 - NW) * 32 + lane;
+        const int h = (warp - Cfg::EPI0 - Cfg::EPILOGUE_WARPS) * 32 + lane;
         float published[2] = {-INFINITY, -INFINITY};
         uint32_t pub_tag[2] = {0xffffffffu, 0xffffffffu};
         bool done[2] = {false, false};

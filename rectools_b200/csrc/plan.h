@@ -1,7 +1,7 @@
-// The decision of one b200_rank_topk call: which path ranks it, with which tensor-core mode, epilogue geometry and list
-// size K', in how many row chunks -- or which refusal it gets.  Pure arithmetic on the query shape, the engine's
-// properties and the B200_* environment hooks, in plain C++17 (no CUDA header), so that tests/test_call_plan_cpu.py
-// compiles it with g++ alone and pins it.
+// The decision of one b200_rank_topk call: which path ranks it, with which tensor-core mode and list size K', in how
+// many row chunks -- or which refusal it gets.  Pure arithmetic on the query shape, the engine's properties and the
+// B200_* environment hooks, in plain C++17 (no CUDA header), so that tests/test_call_plan_cpu.py compiles it with g++
+// alone and pins it.
 #pragma once
 #include <algorithm>
 #include <cmath>
@@ -21,7 +21,6 @@ inline int64_t round_up(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
 struct Hooks {
     int wide = 1;               // B200_WIDE: 0 keeps 24 < k <= 1024 off the wide mode (multi-pass route / path 3)
     std::optional<int> wide_t;  // B200_WIDE_T: the wide mode's expected candidate count T
-    int epi_warps = 8;          // B200_EPI_WARPS: 16 selects the opt-in 16-warp geometry (k <= 24)
     int tc_kcand = 0;           // B200_TC_KCAND: K' of the main pass (4 .. 32)
     int tc_splits = 0;          // B200_TC_SPLITS: object splits of a fused-kernel launch (1 .. its maximum)
     int tc_carousel = 1;        // B200_TC_CAROUSEL: 0 starts every work item at its first object tile
@@ -41,7 +40,6 @@ inline Hooks read_hooks() {
     Hooks h;
     h.wide = get("B200_WIDE", h.wide);
     if (const char* v = std::getenv("B200_WIDE_T")) h.wide_t = std::atoi(v);
-    h.epi_warps = get("B200_EPI_WARPS", h.epi_warps);
     h.tc_kcand = get("B200_TC_KCAND", h.tc_kcand);
     h.tc_splits = get("B200_TC_SPLITS", h.tc_splits);
     h.tc_carousel = get("B200_TC_CAROUSEL", h.tc_carousel);
@@ -53,7 +51,7 @@ inline Hooks read_hooks() {
     return h;
 }
 
-// Wide mode: T = the candidates a row is expected to collect, and the slots of each of its `nlist` append lists.  The
+// Wide mode: T = the candidates a row is expected to collect, and the slots of each of its two append lists.  The
 // threshold frozen after a fraction q of the stream is about the (lists x K' - 6)-th best of that fraction, i.e. rank
 // ~ (lists x K' - 6) / q overall, so q follows from T.  k <= 128: T = 1.35 k + 40 (K' = 24), at most WIDE_MAX slots per row.
 // k > 128: T = 1.6 k + 64 (K' = 32), at most WIDE_MAX_L slots per row -- the frozen threshold is an order statistic of
@@ -63,19 +61,23 @@ struct WideGeom {
     int cand_stride = 0;
 };
 
-inline WideGeom wide_geom(int kp, int nlist, const Hooks& h) {
+inline WideGeom wide_geom(int kp, const Hooks& h) {
     WideGeom g;
     g.T = h.wide_t.value_or(kp <= 128 ? (int)(1.35 * kp + 40) : (int)(1.6 * kp + 64));
-    g.cand_stride = std::min((int)round_up((int64_t)(g.T / nlist * 1.5 + 32), 8), (kp <= 128 ? WIDE_MAX : WIDE_MAX_L) / nlist);
+    g.cand_stride = std::min((int)round_up((int64_t)(g.T / 2 * 1.5 + 32), 8), (kp <= 128 ? WIDE_MAX : WIDE_MAX_L) / 2);
     return g;
 }
 
 // Object splits of a fused-kernel launch: fill the machine when there are few row tiles, even out the last wave
 // otherwise (`n_units` CTA pairs work concurrently).  `forced` (B200_TC_SPLITS) wins when it is in range.
+// At most MAX_SPLITS, so a row has at most 2 x 16 = 32 lists: rescore_select_kernel keeps one list per lane.
+constexpr int MAX_SPLITS = 16;
+static_assert(2 * MAX_SPLITS <= 32, "rescore_select_kernel holds one candidate list per lane of a warp");
+
 inline int choose_splits(int n_row_tiles, int n_obj_tiles, int n_units, bool wide, int forced) {
     int best_splits = 1;
     double best_eff = -1.0;
-    const int max_splits = wide ? 1 : std::max(1, std::min(16, n_obj_tiles * 2 / 32));
+    const int max_splits = wide ? 1 : std::max(1, std::min(MAX_SPLITS, n_obj_tiles * 2 / 32));
     for (int s = 1; s <= max_splits; ++s) {
         const double work = (double)n_row_tiles * s;
         const double waves = std::ceil(work / n_units);
@@ -131,7 +133,7 @@ struct CallPlan {
     Select select = Select::PASSES;  // paths SPARSE / DENSE_LARGE_K (the re-rank of rows a wide pass rejects: PASSES)
     TcMode mode = TcMode::NARROW;  // path TC only
     bool bf16 = false;             // operand type of the tensor-core passes
-    int nw = 8;                    // epilogue warps of the main pass
+    static constexpr int nw = 8;   // epilogue warps of the fused kernel: one geometry (b200_rank_stats::epi_warps)
     int k_cand = 0;                // K' of the main pass
     bool peers = false;            // the main pass shares thresholds (B200_Q_SHARED_THRESHOLDS)
     WideGeom geom;                 // WIDE / WIDE_L
@@ -153,25 +155,16 @@ inline CallPlan plan_call(const CallShape& s, const Hooks& h) {
     // 128 < k <= 1024: the same single wide pass with longer append lists and a large-k re-score, when the expected
     // candidate count stays well inside the catalogue (k = None and near-catalogue requests keep path 3).  Item-sharded
     // calls that share thresholds need k <= 24 and keep path 3 here as well.
-    const bool wide_l = k > 128 && k <= 1024 && h.wide != 0 && !s.sparse && !shared && wide_geom(k, 2, h).T <= 0.5 * (double)s.n_pos;
-    // 16 epilogue warps (B200_EPI_WARPS=16) are opt-in: next to the MMA warp group they get 96 registers a thread and
-    // spill.  The wide mode always runs the 8-warp geometry: four lists per row freeze at a weaker, noisier rank.
-    int nw = (!wide && !wide_l && h.epi_warps == 16) ? 16 : 8;
+    const bool wide_l = k > 128 && k <= 1024 && h.wide != 0 && !s.sparse && !shared && wide_geom(k, h).T <= 0.5 * (double)s.n_pos;
 
     // Candidates kept per list by the tensor-core pass (K' >= k / lists; the surplus is the certificate's safety margin).
-    // A row has 2 (8 epilogue warps) or 4 (16) lists, one per column group of the tile stream, so a small surplus per
-    // list already gives ~2k candidates; rows where (nearly) all of the top-k fall into one column group fail the
-    // certificate and take the second-chance pass.  Inserts, the dominant epilogue cost, scale with K'.
+    // A row has two lists, one per column group of the tile stream, so a small surplus per list already gives ~2k
+    // candidates; rows where (nearly) all of the top-k fall into one column group fail the certificate and take the
+    // second-chance pass.  Inserts, the dominant epilogue cost, scale with K'.
     int k_cand = 0;
     if (k <= 24) {
-        if (nw == 16) {
-            // four lists per row: a list may be SHORTER than k (the certificate only needs the k-th exact score above every
-            // list's threshold); rows whose top-k crowd into one column quarter take the second-chance pass
-            k_cand = std::min(16, (k <= 10 ? 8 : k <= 16 ? 12 : 16) + (p.bf16 ? 2 : 0));
-        } else {
-            const int surplus = p.bf16 ? std::max(6, k / 2) : std::max(2, k / 4);
-            k_cand = std::min(32, k + surplus);
-        }
+        const int surplus = p.bf16 ? std::max(6, k / 2) : std::max(2, k / 4);
+        k_cand = std::min(32, k + surplus);
     } else if (k <= 128) {
         k_cand = wide ? 24 : (p.bf16 ? 30 : 25);  // wide: adaptive lists of phase 1;  else passes of 20
     } else if (wide_l) {
@@ -182,15 +175,15 @@ inline CallPlan plan_call(const CallShape& s, const Hooks& h) {
         // largest K'-th best of L samples of N/L objects -- about global rank L K' - c_L L sqrt(K') (c_L = expected maximum
         // of L standard normals).  The certificate needs that rank to stay above k plus a margin; everything beyond is
         // wasted insertions (K' = 12 on 8 ranks sits near rank 100, K' = 6 near rank 27).
-        const int L = (s.n_peers + 1) * (nw / 4);
+        const int L = (s.n_peers + 1) * 2;
         const double cL = L <= 2 ? 0.56 : L <= 4 ? 1.03 : L <= 8 ? 1.42 : L <= 16 ? 1.77 : L <= 32 ? 2.07 : 2.33;
         const double target = k + std::max(12.0, 0.6 * k) + (p.bf16 ? 20.0 : 0.0);
         int kc = 4;
         while (kc < 32 && L * kc - cL * L * std::sqrt((double)kc) < target) ++kc;
-        k_cand = std::min(kc, nw == 16 ? 16 : 32);
+        k_cand = kc;
     }
     const int forced = h.tc_kcand;
-    if (forced >= 4 && forced <= 32 && (forced >= k || nw == 16 || wide || wide_l || shared)) k_cand = forced;
+    if (forced >= 4 && forced <= 32 && (forced >= k || wide || wide_l || shared)) k_cand = forced;
 
     bool use_tc = !s.sparse && s.tc_dtype != B200_TC_OFF && k_cand > 0 && !(s.flags & B200_Q_FORCE_EXACT) &&
                   s.n_pos >= (int64_t)k_cand * 4;
@@ -214,9 +207,10 @@ inline CallPlan plan_call(const CallShape& s, const Hooks& h) {
     if (p.tc()) {
         p.mode = wide ? TcMode::WIDE : wide_l ? TcMode::WIDE_L : k > 24 ? TcMode::MULTI_PASS : TcMode::NARROW;
         p.peers = shared;  // (zero peers: the same protocol, nothing to adopt)
-        p.nw = p.mode == TcMode::MULTI_PASS ? 8 : nw;
-        p.k_cand = std::min(k_cand, ROW_SLOTS / (p.nw / 4));  // (the n_pos bound above takes K' before this cap)
-        if (p.wide()) p.geom = wide_geom(k, p.nw / 4, h);
+        // every route above keeps K' within a list: the kernel's lists have no room for more
+        if (k_cand > LIST_SLOTS) return refuse("K' = " + std::to_string(k_cand) + " exceeds the candidate-list capacity");
+        p.k_cand = k_cand;
+        if (p.wide()) p.geom = wide_geom(k, h);
         const int64_t wave = (int64_t)(s.sm_count / 2) * 256;  // subject rows one wave of CTA pairs works on
         if (!(s.flags & B200_Q_INPUTS_ON_DEVICE) && p.mode != TcMode::MULTI_PASS) {
             // host inputs: row chunks let the copies of one chunk overlap the ranking of another

@@ -342,24 +342,21 @@ __global__ void __launch_bounds__(SEL_WARPS * 32) rescore_select_kernel(const Se
         for (int o = 16; o > 0; o >>= 1) unorm2 += __shfl_xor_sync(B200_FULL_MASK, unorm2, o);
         __syncwarp();
     }
-    // list lengths and thresholds: lane l holds lists l and l + 32 (n_lists <= 64)
-    int cnt0 = 0, cnt1 = 0;
+    // list lengths and thresholds: lane l holds list l (at most 16 object splits x two lists: n_lists <= 32)
+    int cnt = 0;
     float thr_max = -INFINITY;
     bool overflow = false;
-    for (int l = lane; l < p.n_lists; l += 32) {
-        const int64_t o = (int64_t)l * p.list_stride_rows + sel;
+    if (lane < p.n_lists) {
+        const int64_t o = (int64_t)lane * p.list_stride_rows + sel;
         const int c = p.in_counts[o];
-        overflow |= c > p.L;
-        if (l < 32)
-            cnt0 = min(c, p.L);
-        else
-            cnt1 = min(c, p.L);
+        overflow = c > p.L;
+        cnt = min(c, p.L);
         thr_max = fmaxf(thr_max, p.in_thr[o]);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) thr_max = fmaxf(thr_max, __shfl_xor_sync(B200_FULL_MASK, thr_max, o));
     overflow = __any_sync(B200_FULL_MASK, overflow);
-    int total = cnt0 + cnt1;
+    int total = cnt;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(B200_FULL_MASK, total, o);
 
@@ -375,7 +372,7 @@ __global__ void __launch_bounds__(SEL_WARPS * 32) rescore_select_kernel(const Se
         const int ci = base + lane;
         int list = -1, e = 0, acc = 0;
         for (int l = 0; l < p.n_lists; ++l) {
-            const int c = __shfl_sync(B200_FULL_MASK, l < 32 ? cnt0 : cnt1, l & 31);
+            const int c = __shfl_sync(B200_FULL_MASK, cnt, l);
             if (list < 0 && ci < acc + c) {
                 list = l;
                 e = ci - acc;

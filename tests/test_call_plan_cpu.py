@@ -134,23 +134,13 @@ def test_shared_thresholds_k_cand(driver):
     assert (p["k_cand"], p["peers"]) == (12, 1)
 
 
-def test_sixteen_epilogue_warps(driver):
-    # four lists per row: K' = 8 for k <= 10, + 2 in bf16
-    for tc, kc in ((FP16, 8), (BF16, 10)):
-        p = plan(driver, n_rows=M, n_pos=M, k=10, tc_dtype=tc, B200_EPI_WARPS=16)
-        assert (p["nw"], p["k_cand"]) == (16, kc)
-    # the wide and multi-pass routes keep 8 warps
-    assert plan(driver, n_rows=M, n_pos=M, k=100, B200_EPI_WARPS=16)["nw"] == 8
-    assert plan(driver, n_rows=M, n_pos=M, k=100, B200_EPI_WARPS=16, B200_WIDE=0)["nw"] == 8
-
-
 def test_hooks(driver):
     # B200_TC_KCAND below k is taken only where lists may be shorter than k
     assert plan(driver, n_rows=M, n_pos=M, k=10, B200_TC_KCAND=20)["k_cand"] == 20
     assert plan(driver, n_rows=M, n_pos=M, k=10, B200_TC_KCAND=8)["k_cand"] == 12
     assert plan(driver, n_rows=M, n_pos=M, k=100, B200_TC_KCAND=8)["k_cand"] == 8
-    # the 16-warp lists hold 16 slots
-    assert plan(driver, n_rows=M, n_pos=M, k=10, B200_EPI_WARPS=16, B200_TC_KCAND=32)["k_cand"] == 16
+    # a list holds 32 slots: the largest forced K' is taken whole
+    assert plan(driver, n_rows=M, n_pos=M, k=10, B200_TC_KCAND=32)["k_cand"] == 32
     # B200_WIDE_T: T = 61 at k = 100 -> round_up(int(30.5 * 1.5 + 32), 8) = 80 slots; T = 400 -> 332, capped at
     # WIDE_MAX / 2 = 256.  B200_CHUNK_ROWS (at least 256)
     p = plan(driver, n_rows=M, n_pos=M, k=100, B200_WIDE_T=61)

@@ -99,17 +99,18 @@ def _base(n_rows=N_ROWS, n_obj=N_OBJ, d=D, seed=0, per_user=50):
     "name, env, shape",
     [
         ("nw8", {}, {}),
-        ("nw16", {"B200_EPI_WARPS": "16"}, {}),
+        ("kcand32", {"B200_TC_KCAND": "32"}, {}),  # lists at their full 32 slots
         ("splits1", {"B200_TC_SPLITS": "1"}, {}),
         ("splits3", {"B200_TC_SPLITS": "3"}, {}),
         ("splits_max", {"B200_TC_SPLITS": "16"}, {"n_obj": 80_000, "d": 32, "n_rows": 512}),
         ("rows1", {}, {"n_rows": 1}),
         ("rows255", {}, {"n_rows": 255}),
         ("rows256", {}, {"n_rows": 256}),
-        ("rows257", {"B200_EPI_WARPS": "16"}, {"n_rows": 257}),
+        ("rows257", {}, {"n_rows": 257}),
         ("npos_4kcand", {}, {"n_obj": 48, "n_rows": 300, "per_user": 5}),
         ("npos_256m_plus_1", {}, {"n_obj": 256 * 20 + 1}),
         ("npos_not_64", {}, {"n_obj": 5_037}),
+        ("rows257_splits3", {"B200_TC_SPLITS": "3"}, {"n_rows": 257}),  # six lists per row on a partial row tile
     ],
 )
 def test_geometry(lib, monkeypatch, capsys, name, env, shape):
@@ -121,9 +122,11 @@ def test_geometry(lib, monkeypatch, capsys, name, env, shape):
     eng = Engine(i, cosine=False)
     _, reps = _run(eng, lib, monkeypatch, capsys, name, u, K, i, False, csr.indptr, csr.indices)
     snap = reps[0][0]
-    assert snap["nw"] == int(env.get("B200_EPI_WARPS", 8))
+    assert snap["nw"] == 8
     if "B200_TC_SPLITS" in env:
         assert snap["n_splits"] == int(env["B200_TC_SPLITS"])
+    if name == "kcand32":
+        assert snap["k_cand"] == 32
     if name == "npos_4kcand":
         assert snap["n_pos"] == 4 * snap["k_cand"]
     eng.close()

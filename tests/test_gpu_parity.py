@@ -235,14 +235,15 @@ def test_wide_mode_overflow_and_short_streams(rb, monkeypatch):
 
 
 @pytest.mark.parametrize("splits", [None, "3"])
-@pytest.mark.parametrize("kernel_env", [{}, {"B200_EPI_WARPS": "16"}], ids=["epi8", "epi16"])
-def test_many_work_items_per_cta(rb, monkeypatch, splits, kernel_env):
+@pytest.mark.parametrize("carousel", [True, False], ids=["carousel", "no_carousel"])
+def test_many_work_items_per_cta(rb, monkeypatch, splits, carousel):
     """More subject tiles than CTA pairs (persistent loop, accumulator / list / threshold hand-over between work items) and
-    forced object splits, for both geometries of the fused kernel."""
+    forced object splits, with every work item starting where the reference pair is in the object stream (the carousel)
+    and at its first object tile."""
     from rectools_b200 import _lib
 
-    for k_, v_ in kernel_env.items():
-        monkeypatch.setenv(k_, v_)
+    if not carousel:
+        monkeypatch.setenv("B200_TC_CAROUSEL", "0")
     if splits:
         monkeypatch.setenv("B200_TC_SPLITS", splits)
     n_users, n_items, d, k = 60_000, 12_345, 64, 10
@@ -251,7 +252,7 @@ def test_many_work_items_per_cta(rb, monkeypatch, splits, kernel_env):
     ranker = rb.B200Ranker("dot", u, i)
     sids = np.arange(n_users)
     _, ids, scores, counts = ranker.rank_padded(sids, k, csr, flags=_lib.Q_FORCE_TC)
-    assert ranker.last_stats["path"] == 1 and ranker.last_stats["epi_warps"] == (16 if kernel_env else 8)
+    assert ranker.last_stats["path"] == 1 and ranker.last_stats["epi_warps"] == 8
     sel = np.unique(np.concatenate([np.arange(0, n_users, 29), np.arange(n_users - 300, n_users)]))
     _, oid, osc = rank_oracle("dot", u, i, sel, k, csr[sel], accum="f64")
     np.testing.assert_array_equal(ids[sel].reshape(-1), oid, err_msg=str(ranker.last_stats))
@@ -260,27 +261,6 @@ def test_many_work_items_per_cta(rb, monkeypatch, splits, kernel_env):
     _, ids2, scores2, _ = ranker.rank_padded(sids, k, csr, flags=_lib.Q_FORCE_TC)
     np.testing.assert_array_equal(ids, ids2)
     np.testing.assert_array_equal(scores, scores2)
-
-
-@pytest.mark.parametrize("distance, k, tc_mode", [("dot", 10, "auto"), ("cosine", 20, "auto"), ("dot", 20, "bf16"), ("dot", 5, "auto")])
-def test_random_vs_oracle_16_epilogue_warps(rb, monkeypatch, distance, k, tc_mode):
-    """The 16-warp geometry (four 16-slot lists per row) on the seeded random shapes."""
-    from rectools_b200 import _lib
-
-    monkeypatch.setenv("B200_EPI_WARPS", "16")
-    n_users, n_items, d = 3000, 40_000, 128
-    u, i = synth_factors(n_users, n_items, d, seed=k + 100)
-    csr = synth_viewed_csr(n_users, n_items, 60)
-    ranker = rb.B200Ranker(distance, u, i, tc_mode=tc_mode)
-    sids = np.arange(n_users)
-    _, ids, scores, counts = ranker.rank_padded(sids, k, csr, flags=_lib.Q_FORCE_TC)
-    assert ranker.last_stats["epi_warps"] == 16 and (counts == k).all()
-    _, oid, osc = rank_oracle(distance, u, i, sids, k, csr, accum="f64")
-    if distance == "cosine":
-        osc = osc * ranker.subjects_norms[np.repeat(sids, k)]
-    np.testing.assert_array_equal(ids.reshape(-1), oid, err_msg=str(ranker.last_stats))
-    np.testing.assert_allclose(scores.reshape(-1), osc, rtol=3e-7, atol=1e-9)
-    assert ranker.last_stats["n_fallback_rows"] <= n_users // 20, ranker.last_stats
 
 
 def test_edge_cases(rb):

@@ -28,15 +28,15 @@ def _next_epoch():
     return _EPOCH[0]
 
 
-def shared_kcand(k, n_ranks, nw=8, bf16=False):
-    """K' of a threshold-sharing pass (plan.h `plan_call`; pinned by tests/test_call_plan_cpu.py)."""
-    L = n_ranks * (nw // 4)
+def shared_kcand(k, n_ranks, bf16=False):
+    """K' of a threshold-sharing pass (plan.h `plan_call`; pinned by tests/test_call_plan_cpu.py): two lists per rank."""
+    L = n_ranks * 2
     cL = 0.56 if L <= 2 else 1.03 if L <= 4 else 1.42 if L <= 8 else 1.77 if L <= 16 else 2.07 if L <= 32 else 2.33
     target = k + max(12.0, 0.6 * k) + (20.0 if bf16 else 0.0)
     kc = 4
     while kc < 32 and L * kc - cL * L * np.sqrt(kc) < target:
         kc += 1
-    return min(kc, 16 if nw == 16 else 32)
+    return kc
 
 
 def _torch():
@@ -163,7 +163,7 @@ def run_case(monkeypatch, capsys, name, shards, order, sub, k, csr, objects_all,
         sh = shards[s]
         out, st, snap, peer_before, pub_before = _rank(sh, monkeypatch, sub, k, epoch, indptr, indices, device_inputs, snap_launch)
         assert st["path"] == 1 and st["n_fallback_rows"] == 0, st
-        assert st["k_cand"] == shared_kcand(k, n_ranks, st["epi_warps"], bf16), st
+        assert st["k_cand"] == shared_kcand(k, n_ranks, bf16), st
         assert snap is not None and snap["k_cand"] == st["k_cand"] and snap["launch"] == snap_launch
         runs[s] = (out, st, snap, peer_before, pub_before, _words(sh.pub))
     # each pass's rows, subjects and the lists' own justification (published units)
@@ -326,8 +326,8 @@ def test_negative_rows(monkeypatch, capsys, cosine):
 @pytest.mark.parametrize(
     "name, env, tc_mode, k, whitelist",
     [
-        ("nw16_fp16", {"B200_EPI_WARPS": "16"}, "auto", 10, False),
-        ("nw16_bf16", {"B200_EPI_WARPS": "16"}, "bf16", 10, False),
+        ("bf16_splits3", {"B200_TC_SPLITS": "3"}, "bf16", 10, False),
+        ("bf16_k24", {}, "bf16", 24, False),
         ("nw8_bf16", {}, "bf16", 10, False),
         ("splits3", {"B200_TC_SPLITS": "3"}, "auto", 10, False),
         ("whitelist", {}, "auto", 10, True),
@@ -336,8 +336,8 @@ def test_negative_rows(monkeypatch, capsys, cosine):
     ],
 )
 def test_instantiations_and_options(monkeypatch, capsys, name, env, tc_mode, k, whitelist):
-    """16 epilogue warps with fp16 and bf16, 8 with bf16 (the other three PEERS kernels); three object splits of a row
-    publishing to the same slot; a per-shard whitelist; k = 1 and k = 24."""
+    """bf16 operands (the other PEERS kernel), also with three splits and k = 24; three object splits of a row publishing
+    to the same slot; a per-shard whitelist; k = 1 and k = 24."""
     for key, val in env.items():
         monkeypatch.setenv(key, val)
     n_rows, n_obj, d = 640, 60_000, 64
@@ -348,7 +348,7 @@ def test_instantiations_and_options(monkeypatch, capsys, name, env, tc_mode, k, 
     _, _, runs = run_case(monkeypatch, capsys, name, shards, [0, 1], u, k, csr, i, False, whitelist_all=wl,
                           bf16=tc_mode == "bf16", min_adopt=0.01)
     snap = runs[1][2]
-    assert snap["nw"] == int(env.get("B200_EPI_WARPS", 8)) and snap["bf16"] == (tc_mode == "bf16")
+    assert snap["nw"] == 8 and snap["bf16"] == (tc_mode == "bf16")
     if "B200_TC_SPLITS" in env:
         assert snap["n_splits"] == 3
     if whitelist:
