@@ -48,7 +48,7 @@
 extern "C" {
 #endif
 
-#define B200_RANK_ABI_VERSION 5
+#define B200_RANK_ABI_VERSION 6
 
 /* error codes */
 #define B200_OK 0
@@ -74,7 +74,7 @@ extern "C" {
 #define B200_F_OBJECTS_ON_DEVICE 1 /* `objects` is a device pointer on `device` */
 
 /* query flags */
-#define B200_Q_INPUTS_ON_DEVICE 1  /* subjects / subject_ids / csr_* / whitelist are device pointers */
+#define B200_Q_INPUTS_ON_DEVICE 1  /* subjects / subject_ids / object_rows / csr_* / whitelist are device pointers */
 #define B200_Q_OUTPUTS_ON_DEVICE 2 /* out_* are device pointers */
 #define B200_Q_FORCE_EXACT 4       /* skip the tensor-core pass */
 #define B200_Q_FORCE_TC 8          /* fail with B200_E_UNSUPPORTED instead of silently using the exhaustive kernel */
@@ -125,14 +125,24 @@ typedef struct b200_rank_query {
     const int64_t* sub_indptr; /* [n_rows + 1] or NULL */
     const int32_t* sub_indices;
     const float* sub_data;
-    int64_t reserved[2];
+    /* ---- ABI 6: stored rows as score rows (EASEModel item-to-item: row t of the weight matrix, which the engine holds as
+     * its objects, is the score row of target t, rectools/models/ease.py:163-188).  Batch row r is scored as
+     * score(r, j) = the engine's fp32 master copy [object_rows[r], j], bit for bit; the selection reads the row where it
+     * lies and never writes into it.  Given instead of `subjects` / `subject_ids` / `sub_*`.  Needs d == n_objects (the
+     * row is indexed by object id: else B200_E_INVALID); refused with B200_E_UNSUPPORTED on COSINE engines, engines with a
+     * non-zero id offset, B200_Q_SHARED_THRESHOLDS and B200_Q_FORCE_TC.  Entries must lie in [0, n_objects): checked for
+     * host inputs (B200_E_INVALID), the caller's contract for device inputs, as the CSR arrays are.  The filter,
+     * whitelist, k, outputs and padding mean what they mean for the other paths; stats.path = 4. */
+    const int64_t* object_rows; /* [n_rows] or NULL */
+    int64_t reserved[1];
 } b200_rank_query;
 
 typedef struct b200_rank_stats {
     int32_t path;            /* 0 = exhaustive fp64 kernel, 1 = tensor-core candidates + fp64 re-score, 2 = sparse subjects (SpMM
                               * scores + streaming selection), 3 = k > 128 without the tensor-core path (k > 1024, k = None, a
                               * problem below the tiny-problem size, B200_Q_FORCE_EXACT, B200_WIDE=0, or an expected candidate count
-                              * above half the catalogue): exhaustive scores materialised once + selection passes */
+                              * above half the catalogue): exhaustive scores materialised once + selection passes, 4 = stored
+                              * rows (object_rows): one radix-select launch per row chunk over the rows in place */
     int32_t tc_dtype;        /* B200_TC_FP16 / B200_TC_BF16 when path == 1 */
     int32_t k_out;           /* columns of the output arrays */
     int32_t k_cand;          /* candidates kept per row and item split by the tensor-core pass */

@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200_RANK_LIB") or os.path.join(HERE, "libb200rank.so")
 
 # mirrors of the #defines in include/b200_rank.h
-ABI_VERSION = 5
+ABI_VERSION = 6
 OK, E_INVALID, E_CUDA, E_NOMEM, E_UNSUPPORTED = 0, -1, -2, -3, -4
 DIST_DOT, DIST_COSINE = 0, 1
 TC_AUTO, TC_FP16, TC_BF16, TC_OFF = 0, 1, 2, 3
@@ -59,7 +59,8 @@ class Query(C.Structure):
         ("sub_indptr", C.c_void_p),
         ("sub_indices", C.c_void_p),
         ("sub_data", C.c_void_p),
-        ("reserved", C.c_int64 * 2),
+        ("object_rows", C.c_void_p),  # ABI 6: stored rows as score rows (path 4)
+        ("reserved", C.c_int64 * 1),
     ]
 
 

@@ -25,6 +25,7 @@
 #include "select.cuh"
 #include "sparse.cuh"
 #include "large_k_select.cuh"
+#include "row_select.cuh"
 #include "fused_topk.cuh"
 
 namespace {
@@ -369,6 +370,7 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
         // the largest launch of any call (k_out >= LK_SMEM_PAIRS); a fixed maximum: the attribute is shared by every engine
         // on the device, and smaller launches stay within it
         CK(cudaFuncSetAttribute(large_k_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lk_smem_bytes(LK_SMEM_PAIRS)));
+        CK(cudaFuncSetAttribute(row_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lk_smem_bytes(LK_SMEM_PAIRS)));
     } catch (const CudaError& ce) {
         int rc = fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_create: %s failed at line %d: %s",
                       ce.what, ce.line, cudaGetErrorString(ce.e));
@@ -400,6 +402,7 @@ struct Call {
     const int64_t* sp_indptr = nullptr;  // sparse subjects
     const int32_t* sp_indices = nullptr;
     const float* sp_data = nullptr;
+    const int64_t* obj_rows = nullptr;  // stored rows (path 4)
     int32_t *o_ids = nullptr, *o_counts = nullptr;
     float *o_scores = nullptr, *o_bounds = nullptr;
     // failure lists (absolute rows) of the main pass, of one re-rank pass and of its second chance, and their counters
@@ -860,6 +863,33 @@ void run_dense_large_k(Call& c, const int32_t* rows, const float* sub32, const i
     }
 }
 
+// Stored rows (path 4): one row_select_kernel launch over the nr rows of a chunk, reading the master copy in place.
+void run_rows(Call& c, const int64_t* obj_rows, const int64_t* f_indptr, int64_t nr, int32_t* o_ids, float* o_scores, int32_t* o_counts) {
+    b200_rank_engine* E = c.E;
+    if (c.k_out > LK_SMEM_PAIRS) E->lk_scratch.ensure((size_t)rows_row_bytes(c.k_out) * nr);
+    RowSelectParams rp{};
+    rp.objects = E->obj32_ptr;
+    rp.n_obj = E->n_obj;
+    rp.d = E->d;
+    rp.object_rows = obj_rows;
+    rp.n_rows = nr;
+    rp.n_pos = c.n_pos;
+    rp.pos2obj = c.wl;
+    rp.f_indptr = f_indptr;
+    rp.f_indices = c.indices;
+    rp.k_out = c.k_out;
+    rp.smem_pairs = std::min(c.k_out, LK_SMEM_PAIRS);
+    rp.scratch = c.k_out > LK_SMEM_PAIRS ? E->lk_scratch.as<uint32_t>() : nullptr;
+    rp.out_ids = o_ids;
+    rp.out_scores = o_scores;
+    rp.out_counts = o_counts;
+    c.time_begin(1);
+    row_select_kernel<<<(unsigned)nr, LK_THREADS, lk_smem_bytes(c.k_out), c.st>>>(rp);
+    CK(cudaGetLastError());
+    c.time_end();
+    c.S.n_launches++;
+}
+
 // a device-memory scalar, read after everything queued on the engine stream
 template <typename T>
 T read_scalar(b200_rank_engine* E, const T* dev) {
@@ -881,6 +911,16 @@ int validate_query(const b200_rank_engine* E, const b200_rank_query* q) {
     if (q->n_rows < 0) return fail(B200_E_INVALID, "b200_rank_topk: n_rows < 0");
     if (q->k <= 0) return fail(B200_E_INVALID, "b200_rank_topk: k must be positive");
     const bool sparse_sub = q->sub_indptr != nullptr;
+    if (q->object_rows) {  // stored rows: nothing else describes the batch rows (the plan refuses what path 4 cannot rank)
+        if (q->subjects || q->subject_ids || sparse_sub || q->sub_indices || q->sub_data)
+            return fail(B200_E_INVALID, "b200_rank_topk: object_rows excludes subjects / subject_ids / sparse subjects");
+        if (q->subject_dtype != B200_DT_F32) return fail(B200_E_INVALID, "b200_rank_topk: object_rows takes no subject_dtype");
+        if (q->whitelist && q->n_whitelist < 0) return fail(B200_E_INVALID, "b200_rank_topk: n_whitelist < 0");
+        if (q->n_rows > 0 && (!q->out_ids || !q->out_scores || !q->out_counts))
+            return fail(B200_E_INVALID, "b200_rank_topk: output pointers are NULL");
+        if (q->n_rows >= (1ll << 31) - 64) return fail(B200_E_UNSUPPORTED, "b200_rank_topk: more than 2^31 rows per call");
+        return B200_OK;
+    }
     if (!sparse_sub && !q->subjects && !q->subject_ids) return fail(B200_E_INVALID, "b200_rank_topk: neither subjects nor subject_ids given");
     if (sparse_sub && (q->subjects || q->subject_ids)) return fail(B200_E_INVALID, "b200_rank_topk: sparse subjects exclude subjects / subject_ids");
     if (sparse_sub && E->distance != B200_DIST_DOT)
@@ -926,6 +966,13 @@ void stage_inputs(Call& c, int64_t sp_nnz, int64_t f_nnz) {
         c.sp_indptr = (const int64_t*)stage(E->sp_indptr, q->sub_indptr, sizeof(int64_t) * (n_rows + 1));
         c.sp_indices = (const int32_t*)stage(E->sp_indices, q->sub_indices, sizeof(int32_t) * sp_nnz);
         c.sp_data = (const float*)stage(E->sp_data, q->sub_data, sizeof(float) * sp_nnz);
+    } else if (q->object_rows) {  // chunked (stage_rows)
+        if (c.in_dev) {
+            c.obj_rows = q->object_rows;
+        } else {
+            E->rowmap.ensure(std::max<size_t>(sizeof(int64_t) * n_rows, 16));
+            c.obj_rows = E->rowmap.as<int64_t>();
+        }
     } else if (q->subjects) {
         const int64_t rows_in = q->subject_ids ? q->n_subjects_total : n_rows;
         if (q->subject_dtype != B200_DT_F32) {
@@ -1008,6 +1055,7 @@ void stage_rows(Call& c, int64_t r0, int64_t r1, cudaStream_t s) {
     };
     if (q->subjects && !q->subject_ids) h2d(E->sub32.as<float>() + r0 * c.d, q->subjects + r0 * c.d, sizeof(float) * (r1 - r0) * c.d);
     if (q->subject_ids) h2d(E->rowmap.as<int64_t>() + r0, q->subject_ids + r0, sizeof(int64_t) * (r1 - r0));
+    if (q->object_rows) h2d(E->rowmap.as<int64_t>() + r0, q->object_rows + r0, sizeof(int64_t) * (r1 - r0));
     if (c.indptr) {
         h2d(E->indptr.as<int64_t>() + r0, q->csr_indptr + r0, sizeof(int64_t) * (r1 - r0 + 1));
         const int64_t z0 = q->csr_indptr[r0], z1 = q->csr_indptr[r1];
@@ -1102,6 +1150,8 @@ void main_pass(Call& c, int64_t r0, int64_t r1) {
         iota_kernel<<<grid_for(nr, 256), 256, 0, c.st>>>(c.fb_main, nr);
         CK(cudaGetLastError());
         rerank_rows(c, c.fb_main, nr);
+    } else if (P.path == Path::ROWS) {  // every slot and count written by the selection itself
+        run_rows(c, c.obj_rows + r0, ip, nr, oi, os, oc);
     } else {
         init_outputs_kernel<<<grid_for(std::max<int64_t>(nr * k_out, nr), 256), 256, 0, c.st>>>(oi, os, oc, nr, k_out);
         CK(cudaGetLastError());
@@ -1358,7 +1408,9 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
     c.d = E->d;
     c.in_dev = q->flags & B200_Q_INPUTS_ON_DEVICE;
     c.out_dev = q->flags & B200_Q_OUTPUTS_ON_DEVICE;
-    const CallShape shape{c.n_rows, c.n_pos, q->k, E->d, E->d_pad, E->sm_count, E->tc_dtype, E->n_peers, q->flags, q->sub_indptr != nullptr};
+    const CallShape shape{c.n_rows,    c.n_pos,   q->k,          E->d,           E->d_pad,
+                          E->sm_count, E->tc_dtype, E->n_peers, q->flags,       q->sub_indptr != nullptr,
+                          q->object_rows != nullptr, E->n_obj, E->distance == B200_DIST_COSINE, E->id_offset != 0};
     c.hooks = read_hooks();
     c.plan = plan_call(shape, c.hooks);
     const CallPlan& P = c.plan;
@@ -1367,7 +1419,8 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
         if (stats) *stats = S;
         return B200_OK;
     }
-    if ((q->flags & B200_Q_SHARED_THRESHOLDS) && E->n_peers > 0 && c.n_rows > E->peer_rows)
+    // (path 4 refuses shared thresholds in its plan, with B200_E_UNSUPPORTED, whatever the row count)
+    if (!q->object_rows && (q->flags & B200_Q_SHARED_THRESHOLDS) && E->n_peers > 0 && c.n_rows > E->peer_rows)
         return fail(B200_E_INVALID, "b200_rank_topk: %lld rows exceed the %lld exported for threshold sharing", (long long)c.n_rows,
                     (long long)E->peer_rows);
     try {
@@ -1391,6 +1444,11 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
         if (f_nnz < 0) return fail(B200_E_INVALID, "b200_rank_topk: csr_indptr[n_rows] < 0");
         if (f_nnz > 0 && !q->csr_indices) return fail(B200_E_INVALID, "b200_rank_topk: csr_indices is NULL");
         if (P.error != B200_OK) return fail(P.error, "%s", P.message.c_str());
+        if (q->object_rows && !c.in_dev)
+            for (int64_t r = 0; r < c.n_rows; ++r)
+                if (q->object_rows[r] < 0 || q->object_rows[r] >= E->n_obj)
+                    return fail(B200_E_INVALID, "b200_rank_topk: object_rows[%lld] = %lld is not an object of this engine (n_objects = %lld)",
+                                (long long)r, (long long)q->object_rows[r], (long long)E->n_obj);
         S.path = (int)P.path;
         if (P.tc()) {
             S.tc_dtype = E->tc_dtype;

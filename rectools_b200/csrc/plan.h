@@ -25,7 +25,7 @@ struct Hooks {
     int tc_splits = 0;          // B200_TC_SPLITS: object splits of a fused-kernel launch (1 .. its maximum)
     int tc_carousel = 1;        // B200_TC_CAROUSEL: 0 starts every work item at its first object tile
     int tc_debug = 0;           // B200_TC_DEBUG: fused-kernel measurement modes (TcParams::debug_mode; results are invalid)
-    int64_t chunk_rows = 0;     // B200_CHUNK_ROWS: row chunk of host-input calls (0: 8 waves; at least 256)
+    int64_t chunk_rows = 0;     // B200_CHUNK_ROWS: row chunk of host-input calls and of path 4 (0: 8 waves; at least 256)
     int wide_budget_mb = 2048;  // B200_WIDE_BUDGET_MB: device memory for the append lists of k > 128
     int tc_snapshot = 0;        // B200_TC_SNAPSHOT: the fused-kernel launch whose state is kept (0: none)
     int select = 1;             // B200_SELECT: paths 2 / 3 select with 0 the streaming passes for every k, 2 the radix
@@ -102,9 +102,13 @@ struct CallShape {
     int n_peers = 0;             // ranks the engine shares thresholds with
     int32_t flags = 0;           // B200_Q_*
     bool sparse = false;         // sparse subject rows
+    bool rows = false;           // stored rows as score rows (b200_rank_query.object_rows)
+    int64_t n_objects = 0;       // the engine's objects (path 4: the length of a stored row must be d)
+    bool cosine = false;         // the engine is a COSINE engine
+    bool id_offset = false;      // the engine has a non-zero id offset
 };
 
-enum class Path { EXACT = 0, TC = 1, SPARSE = 2, DENSE_LARGE_K = 3 };  // = b200_rank_stats::path
+enum class Path { EXACT = 0, TC = 1, SPARSE = 2, DENSE_LARGE_K = 3, ROWS = 4 };  // = b200_rank_stats::path
 
 // How the tensor-core path ranks the rows of the main pass.
 enum class TcMode {
@@ -117,7 +121,8 @@ enum class TcMode {
 // How paths 2 and 3 select from their materialised score rows.
 enum class Select {
     PASSES,  // ceil(k_out / 32) streaming passes of scores_topk_kernel over every row
-    RADIX,   // large_k_select_kernel: radix select + one sort of the k_out survivors (k_out > 1024)
+    RADIX,   // large_k_select_kernel: radix select + one sort of the k_out survivors (k_out > 1024);
+             // path 4: row_select_kernel, the same selection over the stored rows, for every k_out
 };
 
 // Bytes per row of a path-2 / path-3 row chunk: the fp32 score row and, when the radix selection sorts more survivors than
@@ -127,10 +132,13 @@ inline int64_t select_row_bytes(int64_t n_pos, int64_t k_out, Select sel) {
 }
 constexpr int64_t SELECT_CHUNK_BYTES = (int64_t)1 << 30;
 
+// Path 4 reads the stored rows in place: a row chunk holds no score row, only the sort scratch above LK_SMEM_PAIRS.
+inline int64_t rows_row_bytes(int64_t k_out) { return k_out > LK_SMEM_PAIRS ? 16 * k_out : 0; }
+
 struct CallPlan {
     int k_out = 0;
     Path path = Path::EXACT;
-    Select select = Select::PASSES;  // paths SPARSE / DENSE_LARGE_K (the re-rank of rows a wide pass rejects: PASSES)
+    Select select = Select::PASSES;  // paths SPARSE / DENSE_LARGE_K (the re-rank of rows a wide pass rejects: PASSES); ROWS: RADIX
     TcMode mode = TcMode::NARROW;  // path TC only
     bool bf16 = false;             // operand type of the tensor-core passes
     static constexpr int nw = 8;   // epilogue warps of the fused kernel: one geometry (b200_rank_stats::epi_warps)
@@ -145,7 +153,37 @@ struct CallPlan {
     bool wide() const { return tc() && (mode == TcMode::WIDE || mode == TcMode::WIDE_L); }
 };
 
+// Path 4: batch row r is the engine's stored row object_rows[r], ranked by row_select_kernel in one launch per row chunk,
+// whatever k is.  Row chunks: 8 waves of CTA pairs (or B200_CHUNK_ROWS) when the call has at least two of them, so that
+// the copies of one chunk overlap the ranking of another, and within SELECT_CHUNK_BYTES of sort scratch.
+inline CallPlan plan_rows(const CallShape& s, const Hooks& h) {
+    CallPlan p;
+    const int k = p.k_out = (int)std::min<int64_t>(s.k, s.n_pos);
+    if (s.n_rows == 0 || k <= 0) return p;  // nothing to rank
+    auto refuse = [&](int code, const std::string& why) {
+        p.error = code;
+        p.message = "b200_rank_topk: object_rows: " + why;
+        return p;
+    };
+    if (s.d != s.n_objects)
+        return refuse(B200_E_INVALID, "a stored row is a score row only when d == n_objects (d=" + std::to_string(s.d) +
+                                          ", n_objects=" + std::to_string(s.n_objects) + ")");
+    if (s.cosine) return refuse(B200_E_UNSUPPORTED, "COSINE engines score through the object norms, not the stored rows");
+    if (s.id_offset) return refuse(B200_E_UNSUPPORTED, "engines with an id offset hold one shard of the catalogue");
+    if (s.flags & B200_Q_SHARED_THRESHOLDS) return refuse(B200_E_UNSUPPORTED, "B200_Q_SHARED_THRESHOLDS has no thresholds to share here");
+    if (s.flags & B200_Q_FORCE_TC) return refuse(B200_E_UNSUPPORTED, "no tensor-core pass ranks stored rows (B200_Q_FORCE_TC)");
+    p.path = Path::ROWS;
+    p.select = Select::RADIX;
+    p.chunk = s.n_rows;
+    const int64_t want = h.chunk_rows > 0 ? h.chunk_rows : 8 * (int64_t)(s.sm_count / 2) * 256;
+    if (s.n_rows >= 2 * want) p.chunk = want;
+    if (const int64_t bytes = rows_row_bytes(k)) p.chunk = std::min(p.chunk, std::max<int64_t>(1, SELECT_CHUNK_BYTES / bytes));
+    p.n_chunks = (s.n_rows + p.chunk - 1) / p.chunk;
+    return p;
+}
+
 inline CallPlan plan_call(const CallShape& s, const Hooks& h) {
+    if (s.rows) return plan_rows(s, h);
     CallPlan p;
     const int k = p.k_out = (int)std::min<int64_t>(s.k, s.n_pos);
     if (s.n_rows == 0 || k <= 0) return p;  // nothing to rank

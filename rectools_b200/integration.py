@@ -4,6 +4,8 @@ Seams (SURVEY.md section 8b):
   * `VectorModel._recommend_u2i/_recommend_i2i` construct `ImplicitRanker(...)` inline (rectools/models/vector.py:66-72,
     :90-96; name imported at vector.py:28) and `EASEModel._recommend_u2i` does the same (rectools/models/ease.py:144,
     import at ease.py:31)  ->  `install()` rebinds that module-level name to `B200ImplicitRanker`.
+  * `EASEModel._recommend_i2i` copies the weight rows of the targets and ranks them with numpy (rectools/models/ease.py:163-188)
+    ->  `install()` rebinds it to `ease_recommend_i2i`, which ranks those rows where the u2i engine already holds them.
   * transformer models take `similarity_module_type` (rectools/models/nn/transformers/base.py:219, :423); their
     `DistanceSimilarityModule._recommend_u2i` builds a `TorchRanker` (rectools/models/nn/transformers/similarity.py:127-132)
     ->  `make_similarity_module()` returns a subclass that builds a `B200TorchRanker` instead.
@@ -19,7 +21,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 from scipy import sparse
 
-from .ranker import B200Ranker, Distance, Engine, _as_distance, _dense_f32
+from .ranker import B200Ranker, Distance, Engine, _as_distance, _dense_f32, flatten_padded, rank_object_rows_padded
 
 _ENGINE_CACHE: "tp.Dict[tp.Tuple, Engine]" = {}
 _ENGINE_CACHE_MAX = 2
@@ -144,10 +146,29 @@ class B200TorchRanker(B200Ranker):
 
 _ORIGINALS: tp.Dict[str, tp.Any] = {}
 _FAST_KEY = "VectorModel.recommend"
+_EASE_I2I_KEY = "EASEModel._recommend_i2i"
+
+
+def ease_recommend_i2i(self, target_ids, dataset, k, sorted_item_ids_to_recommend):
+    """`EASEModel._recommend_i2i` (rectools/models/ease.py:163-188) on the GPU: row t of `self.weight` is the score row of
+    target t, and the engine of `_recommend_u2i` (cached by the content of `self.weight`) holds exactly that matrix, so the
+    rows are ranked where they lie -- no copy of the rows, no extra device memory.  Returns the reference's triplet: best
+    first, ids remapped through the whitelist, `min(k, n_pos)` entries per target for finite weights (what EASE fits).
+    Unlike the reference, -inf and NaN weights are never returned, so a target with such entries may get fewer.  Tie order
+    among equal scores is id ascending (the reference leaves it undefined).  Every call finds the engine through
+    `cached_engine`, i.e. one `content_hash` of the whole weight per call.  A weight that is not a C-contiguous fp32 matrix (a float64 weight
+    ranks in fp64 in the reference) goes to the original method."""
+    weight = getattr(self, "weight", None)
+    if not (isinstance(weight, np.ndarray) and weight.dtype == np.float32 and weight.ndim == 2 and weight.flags.c_contiguous):
+        return _ORIGINALS[_EASE_I2I_KEY](self, target_ids, dataset, k, sorted_item_ids_to_recommend)
+    engine = cached_engine(weight, False, B200ImplicitRanker.default_device, B200ImplicitRanker.default_tc_mode)
+    target_ids, ids, scores, counts = rank_object_rows_padded(engine, target_ids, k, None, sorted_item_ids_to_recommend)
+    return flatten_padded(target_ids, ids, scores, counts)
 
 
 def install(device: int = 0, tc_mode: str = "auto", fast_recommend: bool = True) -> None:
-    """Route `VectorModel` (ALS / PureSVD / LightFM / BPR / DSSM) and `EASEModel` ranking through the B200 engine.
+    """Route `VectorModel` (ALS / PureSVD / LightFM / BPR / DSSM) and `EASEModel` ranking (u2i and i2i) through the B200
+    engine.
 
     `fast_recommend`: also give `VectorModel` the vectorised `recommend()` of `rectools_b200.recommend` (cached viewed-items
     CSR, id maps by array indexing, no per-user Python loop); warm / cold targets and context models still go through
@@ -161,6 +182,11 @@ def install(device: int = 0, tc_mode: str = "auto", fast_recommend: bool = True)
         if modname not in _ORIGINALS:
             _ORIGINALS[modname] = mod.ImplicitRanker
         mod.ImplicitRanker = B200ImplicitRanker
+    if _EASE_I2I_KEY not in _ORIGINALS:
+        from rectools.models.ease import EASEModel
+
+        _ORIGINALS[_EASE_I2I_KEY] = EASEModel._recommend_i2i  # pylint: disable=protected-access
+        EASEModel._recommend_i2i = ease_recommend_i2i  # pylint: disable=protected-access
     if fast_recommend and _FAST_KEY not in _ORIGINALS:
         from rectools.models.base import ModelBase
         from rectools.models.vector import VectorModel
@@ -197,6 +223,10 @@ def uninstall() -> None:
                 delattr(VectorModel, name)
             else:
                 setattr(VectorModel, name, orig)
+    if _EASE_I2I_KEY in _ORIGINALS:
+        from rectools.models.ease import EASEModel
+
+        EASEModel._recommend_i2i = _ORIGINALS.pop(_EASE_I2I_KEY)  # pylint: disable=protected-access
     for modname, orig in list(_ORIGINALS.items()):
         importlib.import_module(modname).ImplicitRanker = orig
         del _ORIGINALS[modname]

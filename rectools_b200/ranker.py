@@ -242,9 +242,11 @@ class Engine:
         out_bounds: int = 0,
         peer_epoch: int = 0,
         subject_dtype: int = _lib.DT_F32,
+        object_rows: int = 0,
     ) -> tp.Dict[str, tp.Any]:
         """Raw-pointer call (host or device addresses according to `flags`); returns the call statistics."""
         q = _lib.Query()
+        q.object_rows = object_rows or None
         q.out_bounds, q.peer_epoch, q.subject_dtype = out_bounds or None, int(peer_epoch), int(subject_dtype)
         q.subjects, q.subject_ids, q.n_rows, q.n_subjects_total = subjects or None, subject_ids or None, n_rows, n_subjects_total
         q.csr_indptr, q.csr_indices = indptr or None, indices or None
@@ -265,11 +267,20 @@ class Engine:
         flags: int = 0,
         out: tp.Optional[tp.Tuple[np.ndarray, np.ndarray, np.ndarray]] = None,
         sparse_subjects: tp.Optional[sparse.csr_matrix] = None,
+        object_rows: tp.Optional[np.ndarray] = None,
     ) -> tp.Tuple[np.ndarray, np.ndarray, np.ndarray]:
         """Host-buffer call: returns padded `(ids [n,k_out] int32, scores [n,k_out] fp32, counts [n] int32)`.
-        `sparse_subjects`: the batch rows as a CSR matrix [n_rows, d] (EASE), instead of `subjects` / `subject_ids`."""
+        `sparse_subjects`: the batch rows as a CSR matrix [n_rows, d] (EASE), instead of `subjects` / `subject_ids`.
+        `object_rows`: batch row r is the engine's own stored object row object_rows[r], used as the score row (EASE
+        item-to-item; needs d == n_objects), instead of any subjects."""
         q = _lib.Query()
         keep = []
+        if object_rows is not None:
+            if subjects is not None or subject_ids is not None or sparse_subjects is not None:
+                raise ValueError("object_rows excludes subjects / subject_ids / sparse_subjects")
+            object_rows = np.ascontiguousarray(object_rows, dtype=np.int64).reshape(-1)
+            q.object_rows = object_rows.ctypes.data
+            keep.append(object_rows)
         if sparse_subjects is not None:
             if subjects is not None or subject_ids is not None:
                 raise ValueError("sparse_subjects excludes subjects / subject_ids")
@@ -294,6 +305,8 @@ class Engine:
             q.n_subjects_total = 0 if subjects is None else subjects.shape[0]
         elif sparse_subjects is not None:
             n_rows = sparse_subjects.shape[0]
+        elif object_rows is not None:
+            n_rows = len(object_rows)
         else:
             if subjects is None:
                 raise ValueError("either subjects or subject_ids is required")
@@ -327,6 +340,45 @@ class Engine:
         self.topk_raw(q)
         del keep
         return ids, scores, counts
+
+
+def rank_object_rows_padded(
+    engine: Engine,
+    target_ids: InternalIds,
+    k: tp.Optional[int] = None,
+    filter_pairs_csr: tp.Optional[sparse.csr_matrix] = None,
+    sorted_object_whitelist: tp.Optional[np.ndarray] = None,
+) -> tp.Tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+    """Rank the engine's stored object rows as score rows: target t scores object j with objects[t, j] (an EASE weight
+    matrix held as the objects of its u2i engine; d == n_objects).  `(target_ids, ids [n,k], scores [n,k], counts [n])`
+    as `B200Ranker.rank_padded` returns them; k = None ranks every position.  Scores are the stored fp32 values, ordered
+    by (score desc, id asc); -inf and NaN are never returned, filtered objects neither."""
+    target_ids = np.asarray(target_ids, dtype=np.int64).reshape(-1)
+    if filter_pairs_csr is not None and filter_pairs_csr.shape[0] != len(target_ids):
+        raise ValueError("Number of rows in `filter_pairs_csr` must be equal to `len(target_ids)`")
+    if len(target_ids) and (target_ids.min() < 0 or target_ids.max() >= engine.n_objects):
+        raise IndexError("target id out of range")
+    whitelist = None
+    n_pos = engine.n_objects
+    if sorted_object_whitelist is not None:
+        whitelist = np.asarray(sorted_object_whitelist, dtype=np.int64).reshape(-1)
+        check_whitelist(whitelist, engine.n_objects)
+        n_pos = len(whitelist)
+    if k is None:
+        k = n_pos
+    if k <= 0:
+        raise ValueError("`k` must be positive")
+    indptr = indices = None
+    if filter_pairs_csr is not None:
+        csr = filter_pairs_csr if sparse.isspmatrix_csr(filter_pairs_csr) else sparse.csr_matrix(filter_pairs_csr)
+        if not csr.has_sorted_indices:
+            csr = csr.sorted_indices()
+        indptr, indices = csr.indptr, csr.indices
+    if n_pos == 0 or len(target_ids) == 0:
+        z = np.empty((len(target_ids), 0))
+        return target_ids, z.astype(np.int32), z.astype(np.float32), np.zeros(len(target_ids), np.int32)
+    ids, scores, counts = engine.topk(k, object_rows=target_ids, indptr=indptr, indices=indices, whitelist=whitelist)
+    return target_ids, ids, scores, counts
 
 
 def flatten_padded(
@@ -508,6 +560,33 @@ class B200Ranker:
         )
         self.last_stats = self.engine.last_stats
         return (subject_ids,) + strip_sentinel_tail(ids, scores, counts)
+
+    def rank_object_rows_padded(
+        self,
+        target_ids: InternalIds,
+        k: tp.Optional[int] = None,
+        filter_pairs_csr: tp.Optional[sparse.csr_matrix] = None,
+        sorted_object_whitelist: tp.Optional[np.ndarray] = None,
+    ) -> tp.Tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+        """`rank_object_rows` without the ragged flattening: `(target_ids, ids [n,k], scores [n,k], counts [n])`."""
+        if self.distance != Distance.DOT:
+            raise NotImplementedError("stored rows are score rows for Distance.DOT only")
+        out = rank_object_rows_padded(self.engine, target_ids, k, filter_pairs_csr, sorted_object_whitelist)
+        self.last_stats = self.engine.last_stats
+        return out
+
+    def rank_object_rows(
+        self,
+        target_ids: InternalIds,
+        k: tp.Optional[int] = None,
+        filter_pairs_csr: tp.Optional[sparse.csr_matrix] = None,
+        sorted_object_whitelist: tp.Optional[np.ndarray] = None,
+    ) -> tp.Tuple[InternalIds, InternalIds, Scores]:
+        """Rank the object factors' own rows as score rows (square object factors, e.g. an EASE weight matrix): target t
+        scores object j with `objects_factors[t, j]`, as `EASEModel._recommend_i2i` does (rectools/models/ease.py:163-188).
+        Flat `(target ids repeated, object ids, scores)`, grouped by target in input order, best first."""
+        target_ids, ids, scores, counts = self.rank_object_rows_padded(target_ids, k, filter_pairs_csr, sorted_object_whitelist)
+        return flatten_padded(target_ids, ids, scores, counts)
 
     def rank(
         self,
