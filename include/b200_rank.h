@@ -111,8 +111,9 @@ typedef struct b200_rank_query {
     float* out_scores;
     int32_t* out_counts; /* [n_rows] */
     void* stream;        /* cudaStream_t the device buffers are produced / consumed on; the call is ordered after the work
-                          * queued on it and it waits for the results.  NULL = the (legacy) default stream.  Ignored when
-                          * every buffer is a host buffer. */
+                          * queued on it and it waits for the results.  NULL = the (legacy) default stream.  Resident
+                          * subjects set with on_device = 1 count as device inputs of the calls that read them (subject_ids
+                          * without `subjects`).  Ignored when every buffer is a host buffer. */
     /* ---- ABI 3 */
     float* out_bounds;   /* B200_Q_SHARED_THRESHOLDS: [n_rows] upper bound on the exact score of every object of this shard that
                           * is NOT among the row's returned candidates (-inf: nothing was discarded); same memory space as out_* */
@@ -183,10 +184,16 @@ int b200_rank_create(b200_rank_engine** out, const float* objects, int64_t n_obj
                      int32_t device, int32_t tc_mode, int32_t flags);
 /* The same with an explicit element type: fp16 / bf16 object factors (transformer id-embedding scorers keep `item_embs`
  * in the model dtype, rectools/models/nn/transformers/lightning.py:391-398).  16-bit matrices must be device pointers
- * (B200_F_OBJECTS_ON_DEVICE); they are widened once into the engine's fp32 master copy, which is exact. */
+ * (B200_F_OBJECTS_ON_DEVICE); they are widened once into the engine's fp32 master copy, which is exact.
+ * With B200_F_OBJECTS_ON_DEVICE (any dtype) create reads the device matrix after all work queued on the device, so
+ * the caller's producer stream needs no synchronisation.  The object matrix must not change after create: the row norms,
+ * eps and the tensor-core copy are derived from it once (an fp32 device matrix stays the engine's master copy and must
+ * outlive the engine). */
 int b200_rank_create_ex(b200_rank_engine** out, const void* objects, int32_t dtype, int64_t n_objects, int32_t d,
                         int32_t distance, int32_t device, int32_t tc_mode, int32_t flags);
 int b200_rank_destroy(b200_rank_engine* engine);
+/* on_device = 1: `subjects` is a device matrix the engine references (not copied); calls that gather it are ordered
+ * after the work queued on query.stream (NULL = the legacy default stream), as device inputs are. */
 int b200_rank_set_subjects(b200_rank_engine* engine, const float* subjects, int64_t n_subjects, int32_t on_device);
 /* Item-sharded catalogues: the engine holds objects [offset, offset + n_objects) of a larger catalogue.  CSR column ids
  * and returned ids are GLOBAL (local + offset); whitelist entries stay LOCAL positions into this shard. */

@@ -141,6 +141,7 @@ struct b200_rank_engine {
     DevBuf sub32_res;
     int64_t n_sub_res = 0;
     const float* sub32_res_ptr = nullptr;
+    bool sub_res_on_device = false;  // sub32_res_ptr is the caller's device matrix: calls that read it wait on query.stream
 
     // threshold sharing with the other ranks of an item-sharded catalogue
     DevBuf peer_pub;
@@ -334,6 +335,10 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
         for (auto* e : E->call_events()) CK(cudaEventCreate(e));
         for (auto& e : E->evp) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         CK(cudaMallocHost(&E->h_pinned, 256));
+        // a device matrix was produced on some caller stream, which the engine streams do not wait for: order everything
+        // create reads of it (the widening, the row norms and maxima that feed eps, the tensor-core copy) after all work
+        // queued on the device
+        if (flags & B200_F_OBJECTS_ON_DEVICE) CK(cudaDeviceSynchronize());
         if ((flags & B200_F_OBJECTS_ON_DEVICE) && dtype == B200_DT_F32) {
             E->obj32_ptr = reinterpret_cast<const float*>(objects);
         } else {
@@ -342,8 +347,6 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
                 if (dtype == B200_DT_F32) {
                     CK(cudaMemcpyAsync(E->obj32.p, objects, sizeof(float) * n_objects * d, cudaMemcpyHostToDevice, E->st));
                 } else {
-                    // the caller's stream produced the matrix: order the widening after everything queued on the device
-                    CK(cudaDeviceSynchronize());
                     widen16_kernel<<<grid_for(n_objects * d, 256), 256, 0, E->st>>>(objects, dtype == B200_DT_BF16 ? 1 : 0, n_objects * d,
                                                                                    E->obj32.as<float>());
                     CK(cudaGetLastError());
@@ -1308,6 +1311,7 @@ int b200_rank_set_subjects(b200_rank_engine* E, const float* subjects, int64_t n
             E->sub32_res_ptr = E->sub32_res.as<float>();
         }
         E->n_sub_res = n_subjects;
+        E->sub_res_on_device = on_device != 0;
     } catch (const CudaError& ce) {
         return fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_set_subjects: %s failed: %s", ce.what,
                     cudaGetErrorString(ce.e));
@@ -1429,9 +1433,12 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
         cudaStream_t user = reinterpret_cast<cudaStream_t>(q->stream);
         // device pointers + NULL stream = CUDA's (legacy) default stream, like every CUDA API: producers / consumers of the
         // buffers on that stream are ordered against the engine stream (torch's current stream is the default stream unless
-        // the caller switched it: without this a collective reading the outputs could overlap the next call's kernels)
-        if (!user && (c.in_dev || c.out_dev)) user = cudaStreamLegacy;
-        if (user && (c.in_dev || c.out_dev)) {
+        // the caller switched it: without this a collective reading the outputs could overlap the next call's kernels).
+        // Resident subjects set from a device pointer are the caller's memory too: a call that gathers them waits likewise.
+        const bool res_dev = E->sub_res_on_device && !q->subjects && !q->sub_indptr && !q->object_rows;
+        const bool from_user = c.in_dev || res_dev;
+        if (!user && (from_user || c.out_dev)) user = cudaStreamLegacy;
+        if (user && (from_user || c.out_dev)) {
             CK(cudaEventRecord(E->ev_from_user, user));
             CK(cudaStreamWaitEvent(st, E->ev_from_user, 0));
         }
