@@ -117,7 +117,8 @@ class EngineShard:
 
         torch = self.torch
         flags = int(inputs.pop("flags", 0)) | _lib.Q_OUTPUTS_ON_DEVICE
-        n_pos_local = inputs.get("n_whitelist", 0) if inputs.get("whitelist") else self.engine.n_objects
+        # (a whitelist that leaves this shard no position is still a whitelist: the address of an empty array says nothing)
+        n_pos_local = inputs.get("n_whitelist", 0) if "whitelist" in inputs else self.engine.n_objects
         k_loc = min(k, n_pos_local)  # the engine writes rows of k_out = min(k, local candidates) columns
         if k_loc < k:  # short shard: rank into a narrow scratch, widen into the packed buffer
             out.ids.fill_(-1)
@@ -153,6 +154,8 @@ class EngineShard:
         base = g.data_ptr()
         stride = n * (2 * k + 2)
         fail_count.zero_()
+        if n == 0:  # a subject group without a row (a batch smaller than the grid): empty tensors have no address to hand over
+            return
         args = (self.device.index, torch.cuda.current_stream().cuda_stream, w, n, k, base, base + 4 * n * k, base + 8 * n * k)
         if certified and k <= 32:
             _lib.check(_lib.load().b200_rank_merge_certified(

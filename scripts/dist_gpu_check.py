@@ -1,78 +1,20 @@
-"""torchrun check of the sharded CUDA path (NCCL): ShardedB200Ranker over WORLD_SIZE GPUs == fp64 oracle, with and without
-threshold sharing over NVLink peer memory, host inputs (`rank`) and device inputs (`rank_device`), item sharding and -- with
-4+ ranks -- the item x subject grid.
+"""torchrun check of the sharded CUDA path (NCCL, one GPU per rank): `ShardedB200Ranker` over WORLD_SIZE GPUs == fp64 oracle on
+every row, with and without threshold sharing over NVLink peer memory, host inputs (`rank`) and device inputs
+(`rank_device`), item sharding and -- with 3 or 4 ranks -- subject sharding and the item x subject grid.  The cases are the
+table of tests/sharded_cases.py, which also runs on one GPU (tests/test_gpu_sharded_processes.py).
 
-    python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29511 scripts/dist_gpu_check.py
+    python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port <free port> \\
+        scripts/dist_gpu_check.py [--out DIR]
 """
 import os
 import sys
-
-import numpy as np
-import torch
-import torch.distributed as dist
+import tempfile
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
-from oracle.topk_oracle import rank_oracle  # noqa: E402
-from rectools_b200.sharded import ShardedB200Ranker  # noqa: E402
-from tests.helpers import synth_factors, synth_viewed_csr  # noqa: E402
-
-
-def main():
-    local_rank = int(os.environ.get("LOCAL_RANK", "0"))
-    torch.cuda.set_device(local_rank)
-    dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
-    world, rank = dist.get_world_size(), dist.get_rank()
-    n_users, n_items, d, k = 30_000, 141_003, 64, 10
-    u, i = synth_factors(n_users, n_items, d, seed=21)
-    i[50_000:50_040] = i[50_000]  # ties at the cut for the subjects below: rows the global certificate must reject
-    u[:25] = (u[:25] * 0.05 + 3.0 * i[50_000][None, :]).astype(np.float32)
-    csr = synth_viewed_csr(n_users, n_items, 40)
-    whitelist = np.sort(np.random.default_rng(3).choice(n_items, 60_000, replace=False))
-    ok = True
-
-    def report(name, same, extra=""):
-        nonlocal ok
-        if rank == 0:
-            print(f"{name}: {'OK' if same else 'MISMATCH'} {extra}", flush=True)
-        ok = ok and same
-
-    grids = [None] + ([2] if world >= 4 else [])
-    for item_shards in grids:
-        for share in (True, False):
-            for dist_name in ("dot", "cosine"):
-                ranker = ShardedB200Ranker(dist_name, u, i, item_shards=item_shards, share_thresholds=share)
-                for filt, wl in ((csr, None), (csr, whitelist), (None, None)):
-                    sids = np.arange(n_users)
-                    s, ids, sc = ranker.rank(sids, k, filt, wl)
-                    sel = sids[::29]
-                    es, eid, esc = rank_oracle(dist_name, u, i, sel, k, None if filt is None else filt[sel], wl, accum="f64")
-                    got = np.isin(s, sel)
-                    same = np.array_equal(ids[got], eid) and np.allclose(sc[got], esc, rtol=1e-6, atol=1e-7)
-                    st = ranker.last_stats
-                    report(f"grid={item_shards} share={share} {dist_name} filter={filt is not None} whitelist={wl is not None}", same,
-                           f"uncertified={st.get('n_uncertified_rows')} fallback={st.get('n_fallback_rows')} ms_main={st.get('ms_main', 0):.2f}")
-                    if share and item_shards is None and filt is not None and wl is None:
-                        # the planted ties must have gone through the global re-rank; sharing must be on
-                        report("  sharing active + ties re-ranked", ranker.local.sharing and st.get("n_uncertified_rows", 0) >= 25)
-                del ranker
-    # device inputs / outputs (the bench's resident path)
-    ranker = ShardedB200Ranker("dot", None, i, share_thresholds=True, max_rows=n_users)
-    dev = torch.device("cuda", local_rank)
-    d_u = torch.from_numpy(u).to(dev)
-    d_ip = torch.from_numpy(csr.indptr.astype(np.int64)).to(dev)
-    d_ix = torch.from_numpy(csr.indices.astype(np.int32)).to(dev)
-    for rep in range(3):  # consecutive calls: epochs keep the published thresholds of different calls apart
-        ids, sc, cnt = ranker.rank_device(d_u, k, d_ip, d_ix)
-    torch.cuda.synchronize()
-    sel = np.arange(n_users)[::31]
-    _, eid, esc = rank_oracle("dot", u, i, sel, k, csr[sel], accum="f64")
-    same = np.array_equal(ids.cpu().numpy()[sel].reshape(-1), eid) and np.allclose(sc.cpu().numpy()[sel].reshape(-1), esc, rtol=1e-6, atol=1e-7)
-    report("rank_device (device in / out, 3 consecutive calls)", same, str({k_: ranker.last_stats.get(k_) for k_ in ("ms_main", "n_uncertified_rows")}))
-    dist.barrier()
-    dist.destroy_process_group()
-    if not ok:
-        sys.exit(1)
-
+from tests.sharded_cases import main  # noqa: E402
 
 if __name__ == "__main__":
-    main()
+    args = sys.argv[1:]
+    if "--out" not in args:  # (every rank of the node must name the same directory)
+        args += ["--out", os.path.join(tempfile.gettempdir(), f"dist_gpu_check_{os.environ.get('MASTER_PORT', '0')}")]
+    main(["--backend", "nccl", "--provider", "engine", "--check", *args])

@@ -4,7 +4,8 @@
   per-row bounds out), packed buffers, `b200_rank_merge_certified`, re-rank of the rows the global certificate rejects --
   must equal the unsharded ranking;
 * two or more GPUs: `ShardedB200Ranker` under torchrun (NCCL), with and without threshold sharing over NVLink peer memory,
-  host and device inputs, item sharding / subject sharding / grid (scripts/dist_gpu_check.py)."""
+  host and device inputs, item sharding / subject sharding / grid (scripts/dist_gpu_check.py, the case table of
+  tests/sharded_cases.py).  The same table runs on one GPU in tests/test_gpu_sharded_processes.py."""
 import os
 import subprocess
 import sys
@@ -61,14 +62,17 @@ def test_shared_threshold_protocol_on_one_gpu(rb):
 
 
 @pytest.mark.parametrize("n_gpus", [2])
-def test_sharded_ranker_under_torchrun(n_gpus):
+def test_sharded_ranker_under_torchrun(n_gpus, tmp_path):
     import torch
+
+    from tests.sharded_cases import check_results, free_port
 
     if torch.cuda.device_count() < n_gpus:
         pytest.skip(f"needs {n_gpus} GPUs")
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={n_gpus}", "--master-addr", "127.0.0.1",
-           "--master-port", "29517", os.path.join(ROOT, "scripts", "dist_gpu_check.py")]
+           "--master-port", str(free_port()), os.path.join(ROOT, "scripts", "dist_gpu_check.py"), "--out", str(tmp_path)]
     res = subprocess.run(cmd, cwd=ROOT, capture_output=True, text=True, timeout=900)
     sys.stdout.write(res.stdout[-4000:])
     assert res.returncode == 0, res.stdout[-3000:] + res.stderr[-3000:]
-    assert "MISMATCH" not in res.stdout and res.stdout.count("OK") >= 8
+    report = check_results(str(tmp_path), f"items{n_gpus}", ["edges", "tiny", "certificate"], "engine")
+    assert "bit-identical" in report

@@ -11,58 +11,9 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 from scipy import sparse
 
-from oracle.topk_oracle import implicit_topk
 from rectools_b200.sharded import ShardedB200Ranker, merge_padded_numpy, shard_bounds, split_whitelist
 from tests.helpers import synth_factors, synth_viewed_csr
-
-
-class OracleShard:
-    """Local top-k provider with the EngineShard interface, backed by the numpy oracle (test infrastructure only)."""
-
-    def __init__(self, objects, cosine, lo):
-        self.objects, self.cosine, self.lo = objects, cosine, lo
-        self.subjects = None
-
-    def set_subjects(self, subjects):
-        self.subjects = subjects
-
-    def local_topk(self, subject_ids, k, indptr, indices, whitelist_local):
-        n = len(subject_ids)
-        objs = self.objects if whitelist_local is None else self.objects[whitelist_local]
-        n_pos = objs.shape[0]
-        k_loc = min(k, n_pos)
-        ids = np.full((n, k_loc), -1, dtype=np.int32)
-        sc = np.full((n, k_loc), -np.finfo(np.float32).max, dtype=np.float32)
-        cnt = np.zeros(n, dtype=np.int32)
-        if k_loc == 0 or n == 0:
-            return torch.from_numpy(ids), torch.from_numpy(sc), torch.from_numpy(cnt)
-        filt = None
-        if indptr is not None:
-            # global column ids -> local positions of this shard (and of the whitelist)
-            rows = np.repeat(np.arange(n), np.diff(indptr))
-            cols = np.asarray(indices, dtype=np.int64) - self.lo
-            keep = (cols >= 0) & (cols < self.objects.shape[0])
-            rows, cols = rows[keep], cols[keep]
-            if whitelist_local is not None:
-                pos = np.searchsorted(whitelist_local, cols)
-                ok = (pos < len(whitelist_local)) & (whitelist_local[np.minimum(pos, len(whitelist_local) - 1)] == cols)
-                rows, cols = rows[ok], pos[ok]
-            filt = sparse.csr_matrix((np.ones(len(rows), np.float32), (rows, cols)), shape=(n, n_pos))
-        norms = None
-        if self.cosine:
-            norms = np.sqrt((objs.astype(np.float64) ** 2).sum(1)).astype(np.float32)
-            norms[norms == 0] = 1e-10
-        tid, tsc = implicit_topk(objs, self.subjects[subject_ids], k_loc, norms, filt, accum="f64")
-        valid = tsc > -1e38
-        cnt[:] = valid.sum(1)
-        loc = tid if whitelist_local is None else np.asarray(whitelist_local)[tid]
-        ids[valid] = (loc + self.lo)[valid]
-        sc[valid] = tsc[valid]
-        return torch.from_numpy(ids), torch.from_numpy(sc), torch.from_numpy(cnt)
-
-    def merge(self, ids, sc, cnt, k):
-        o = merge_padded_numpy(ids.numpy(), sc.numpy(), cnt.numpy(), k)
-        return tuple(torch.from_numpy(x) for x in o)
+from tests.sharded_cases import OracleShard
 
 
 def _free_port():
