@@ -278,6 +278,47 @@ int b200_rank_get_snapshot(b200_rank_engine* engine, b200_rank_snapshot* meta, f
  * device, and on an engine that has exported, imported or attached before. */
 int b200_rank_peer_attach(b200_rank_engine* engine, int64_t max_rows, void* pub, int32_t n_peers, const void* const* peers);
 
+/* ---- engine groups: one catalogue on several engines (one process, one or several devices), each call's rows split
+ * between them.  Every member is an ordinary engine holding the whole catalogue; a row's result does not depend on the
+ * engine or path that ranks it, so a group call returns, bit for bit, what one engine returns for the same query.
+ *
+ *   create:  the arguments of b200_rank_create[_ex] plus `devices` [n_devices] (member i runs on devices[i]; duplicates
+ *            make several engines on one device).  devices[0] is the HOME device: device inputs and outputs of group
+ *            calls live there, and with B200_F_OBJECTS_ON_DEVICE so does `objects`.  Members on the home device reference
+ *            a device matrix as b200_rank_create does; members on other devices rank a peer copy made at create.  Every
+ *            member holds a full engine's device memory.
+ *   set_subjects: on_device = 0 uploads the host matrix to every member; on_device = 1 takes a device matrix on the home
+ *            device: home members reference it, members on other devices get a peer copy made here (so, for them, later
+ *            changes of the matrix are not seen).
+ *   topk:    `query` as for b200_rank_topk, device pointers on the home device, ordered after query.stream (NULL: the
+ *            legacy default stream) which waits for the results.  The call is checked once before any member runs (a
+ *            refused call leaves every output untouched, with the code one engine returns); B200_Q_SHARED_THRESHOLDS and
+ *            B200_Q_FORCE_TC are refused with B200_E_UNSUPPORTED (a slice can fall under the tiny-problem rule where the
+ *            whole batch would not), as are calls with B200_TC_SNAPSHOT set.  Rows go out in contiguous slices that the
+ *            members pull from a shared counter on library-owned worker threads (B200_GROUP_SLICE_ROWS=n forces slices of
+ *            n rows).  `total`: counters and bytes summed over every member call, times the maximum over members (each
+ *            member's time summed over its slices), path and the shape fields of the first member that ranked a slice;
+ *            `per_member` [n_devices] (nullable): each member's sums.  Stats do not match one engine's on the same query:
+ *            a slice may take another path than the whole batch.  If a member fails, the call waits for the others and
+ *            returns that member's code, with a message naming the member and its device; the outputs are then
+ *            unspecified.
+ *   Calls on one group are serialised; distinct groups are independent.  Worker threads are started by create and joined
+ *   by destroy.  Threshold sharing, snapshots and id offsets are engine-only (b200_rank_peer_*, b200_rank_get_snapshot,
+ *   b200_rank_set_id_offset). */
+typedef struct b200_rank_group b200_rank_group;
+
+int b200_rank_group_create(b200_rank_group** out, const float* objects, int64_t n_objects, int32_t d, int32_t distance,
+                           const int32_t* devices, int32_t n_devices, int32_t tc_mode, int32_t flags);
+int b200_rank_group_create_ex(b200_rank_group** out, const void* objects, int32_t dtype, int64_t n_objects, int32_t d,
+                              int32_t distance, const int32_t* devices, int32_t n_devices, int32_t tc_mode, int32_t flags);
+int b200_rank_group_destroy(b200_rank_group* group);
+/* member i's engine info in infos[i] (n_devices entries); *hbm_bytes (nullable): device memory of all members and of the
+ * group's peer copies and staging buffers */
+int b200_rank_group_get_info(b200_rank_group* group, b200_rank_info* infos, int64_t* hbm_bytes);
+int b200_rank_group_set_subjects(b200_rank_group* group, const float* subjects, int64_t n_subjects, int32_t on_device);
+int b200_rank_group_topk(b200_rank_group* group, const b200_rank_query* query, b200_rank_stats* total /* nullable */,
+                         b200_rank_stats* per_member /* nullable, [n_devices] */);
+
 const char* b200_rank_last_error(void);
 int b200_rank_abi_version(void);
 

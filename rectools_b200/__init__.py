@@ -5,11 +5,12 @@ Public surface (host-side mirror of `rectools.models.rank`):
   * `B200TorchRanker`                     -- `TorchRanker`-signature adapter (transformer id-embedding scorers)
   * `install()` / `uninstall()`           -- rebind the ranker used by `VectorModel` / `EASEModel` in an installed rectools
   * `recommend()`                         -- vectorised `ModelBase.recommend` around the ranker (cached viewed CSR, id maps, table)
+  * `EngineGroup`                         -- one engine per GPU of the host (`device=[...]` / "all"), rows split between them
   * `ShardedB200Ranker`                   -- item-sharded multi-GPU ranking (one process per GPU, NCCL all-gather + merge)
 The CUDA library is `rectools_b200/libb200rank.so` (C ABI: include/b200_rank.h); build it with
 `python -m rectools_b200.build`.  There is no CPU fallback.
 """
-from .ranker import B200Ranker, Distance, Engine, flatten_padded  # noqa: F401
+from .ranker import B200Ranker, Distance, Engine, EngineGroup, flatten_padded  # noqa: F401
 from .integration import B200ImplicitRanker, B200TorchRanker, install, uninstall  # noqa: F401
 from .recommend import recommend, recommend_to_items  # noqa: F401
 
@@ -19,6 +20,7 @@ __all__ = [
     "B200TorchRanker",
     "Distance",
     "Engine",
+    "EngineGroup",
     "flatten_padded",
     "install",
     "recommend",

@@ -34,6 +34,12 @@ EXPORTS = (
     "b200_rank_peer_attach",
     "b200_rank_last_error",
     "b200_rank_abi_version",
+    "b200_rank_group_create",
+    "b200_rank_group_create_ex",
+    "b200_rank_group_destroy",
+    "b200_rank_group_get_info",
+    "b200_rank_group_set_subjects",
+    "b200_rank_group_topk",
 )
 
 
@@ -187,6 +193,18 @@ def load() -> C.CDLL:
     lib.b200_rank_last_error.argtypes = []
     lib.b200_rank_abi_version.restype = C.c_int
     lib.b200_rank_abi_version.argtypes = []
+    lib.b200_rank_group_create.restype = C.c_int
+    lib.b200_rank_group_create.argtypes = [C.POINTER(vp), vp, i64, i32, i32, vp, i32, i32, i32]
+    lib.b200_rank_group_create_ex.restype = C.c_int
+    lib.b200_rank_group_create_ex.argtypes = [C.POINTER(vp), vp, i32, i64, i32, i32, vp, i32, i32, i32]
+    lib.b200_rank_group_destroy.restype = C.c_int
+    lib.b200_rank_group_destroy.argtypes = [vp]
+    lib.b200_rank_group_get_info.restype = C.c_int
+    lib.b200_rank_group_get_info.argtypes = [vp, C.POINTER(Info), C.POINTER(i64)]
+    lib.b200_rank_group_set_subjects.restype = C.c_int
+    lib.b200_rank_group_set_subjects.argtypes = [vp, vp, i64, i32]
+    lib.b200_rank_group_topk.restype = C.c_int
+    lib.b200_rank_group_topk.argtypes = [vp, C.POINTER(Query), C.POINTER(Stats), C.POINTER(Stats)]
     if lib.b200_rank_abi_version() != ABI_VERSION:
         raise B200RankError("libb200rank.so ABI version mismatch: rebuild with `python -m rectools_b200.build --force`")
     _LIB = lib

@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "../../include/b200_rank.h"
+#include "engine_internal.h"
 #include "plan.h"
 #include "common.cuh"
 #include "prep.cuh"
@@ -949,6 +950,27 @@ int validate_query(const b200_rank_engine* E, const b200_rank_query* q) {
     return B200_OK;
 }
 
+CallShape call_shape(const b200_rank_engine* E, const b200_rank_query* q) {
+    return CallShape{q->n_rows,    q->whitelist ? q->n_whitelist : E->n_obj, q->k, E->d, E->d_pad,
+                     E->sm_count, E->tc_dtype, E->n_peers, q->flags, q->sub_indptr != nullptr,
+                     q->object_rows != nullptr, E->n_obj, E->distance == B200_DIST_COSINE, E->id_offset != 0};
+}
+
+// The refusals that need the CSR sizes (sp_nnz = sub_indptr[n_rows], f_nnz = csr_indptr[n_rows]; 0 without the array),
+// the plan's refusal and the range of host object_rows.
+int check_staged(const b200_rank_engine* E, const b200_rank_query* q, const CallPlan& P, int64_t sp_nnz, int64_t f_nnz) {
+    if (sp_nnz < 0 || (sp_nnz > 0 && (!q->sub_indices || !q->sub_data))) return fail(B200_E_INVALID, "b200_rank_topk: bad sparse subjects");
+    if (f_nnz < 0) return fail(B200_E_INVALID, "b200_rank_topk: csr_indptr[n_rows] < 0");
+    if (f_nnz > 0 && !q->csr_indices) return fail(B200_E_INVALID, "b200_rank_topk: csr_indices is NULL");
+    if (P.error != B200_OK) return fail(P.error, "%s", P.message.c_str());
+    if (q->object_rows && !(q->flags & B200_Q_INPUTS_ON_DEVICE))
+        for (int64_t r = 0; r < q->n_rows; ++r)
+            if (q->object_rows[r] < 0 || q->object_rows[r] >= E->n_obj)
+                return fail(B200_E_INVALID, "b200_rank_topk: object_rows[%lld] = %lld is not an object of this engine (n_objects = %lld)",
+                            (long long)r, (long long)q->object_rows[r], (long long)E->n_obj);
+    return B200_OK;
+}
+
 // Host inputs of a large call are staged in row chunks on a second stream: the copy of chunk c+1 (subject rows / ids,
 // its slice of the CSR filter) and the copy-back of chunk c-1 run while chunk c is being ranked.  Buffers are full-size
 // and addressed by absolute row / nnz offsets, so the kernels see the same layout with or without chunking.
@@ -1254,6 +1276,20 @@ void rerank_failures(Call& c, cudaStream_t cs) {
 
 }  // namespace
 
+int b200_check_query(const b200_rank_engine* E, const b200_rank_query* q, int32_t* k_out) {
+    *k_out = 0;
+    if (const int rc = validate_query(E, q)) return rc;
+    const CallPlan P = plan_call(call_shape(E, q), read_hooks());
+    *k_out = P.k_out;
+    if (q->n_rows == 0 || P.k_out <= 0) return B200_OK;
+    const bool in_dev = q->flags & B200_Q_INPUTS_ON_DEVICE;  // device CSR sizes: checked by the engine that reads them
+    const int64_t sp_nnz = q->sub_indptr && !in_dev ? q->sub_indptr[q->n_rows] : 0;
+    const int64_t f_nnz = q->csr_indptr && !in_dev ? q->csr_indptr[q->n_rows] : 0;
+    return check_staged(E, q, P, sp_nnz, f_nnz);
+}
+
+int b200_set_error(int code, const char* message) { return fail(code, "%s", message); }
+
 extern "C" {
 
 const char* b200_rank_last_error(void) { return g_last_error.c_str(); }
@@ -1412,11 +1448,8 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
     c.d = E->d;
     c.in_dev = q->flags & B200_Q_INPUTS_ON_DEVICE;
     c.out_dev = q->flags & B200_Q_OUTPUTS_ON_DEVICE;
-    const CallShape shape{c.n_rows,    c.n_pos,   q->k,          E->d,           E->d_pad,
-                          E->sm_count, E->tc_dtype, E->n_peers, q->flags,       q->sub_indptr != nullptr,
-                          q->object_rows != nullptr, E->n_obj, E->distance == B200_DIST_COSINE, E->id_offset != 0};
     c.hooks = read_hooks();
-    c.plan = plan_call(shape, c.hooks);
+    c.plan = plan_call(call_shape(E, q), c.hooks);
     const CallPlan& P = c.plan;
     S.k_out = c.k_out = P.k_out;
     if (c.n_rows == 0 || c.k_out <= 0) {
@@ -1446,16 +1479,8 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
 
         // ---------------- validate the CSR arrays, refuse what the plan cannot run, stage
         const int64_t sp_nnz = q->sub_indptr ? read_nnz(E, q->sub_indptr, c.n_rows, c.in_dev) : 0;
-        if (sp_nnz < 0 || (sp_nnz > 0 && (!q->sub_indices || !q->sub_data))) return fail(B200_E_INVALID, "b200_rank_topk: bad sparse subjects");
         const int64_t f_nnz = q->csr_indptr ? read_nnz(E, q->csr_indptr, c.n_rows, c.in_dev) : 0;
-        if (f_nnz < 0) return fail(B200_E_INVALID, "b200_rank_topk: csr_indptr[n_rows] < 0");
-        if (f_nnz > 0 && !q->csr_indices) return fail(B200_E_INVALID, "b200_rank_topk: csr_indices is NULL");
-        if (P.error != B200_OK) return fail(P.error, "%s", P.message.c_str());
-        if (q->object_rows && !c.in_dev)
-            for (int64_t r = 0; r < c.n_rows; ++r)
-                if (q->object_rows[r] < 0 || q->object_rows[r] >= E->n_obj)
-                    return fail(B200_E_INVALID, "b200_rank_topk: object_rows[%lld] = %lld is not an object of this engine (n_objects = %lld)",
-                                (long long)r, (long long)q->object_rows[r], (long long)E->n_obj);
+        if (const int rc = check_staged(E, q, P, sp_nnz, f_nnz)) return rc;
         S.path = (int)P.path;
         if (P.tc()) {
             S.tc_dtype = E->tc_dtype;

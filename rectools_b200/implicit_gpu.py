@@ -66,9 +66,9 @@ def _engine_backend(items, queries, k, item_norms, csr):
     `Matrix` receives a fresh copy each time (models/utils.py:136), so there is no identity to key a cache on here -- the
     `Ranker`-level seam (`install()`, engine cached per factor matrix) is the fast one."""
     from .integration import B200ImplicitRanker
-    from .ranker import Engine
+    from .ranker import new_engine
 
-    eng = Engine(items, cosine=item_norms is not None, device=B200ImplicitRanker.default_device, tc_mode=B200ImplicitRanker.default_tc_mode)
+    eng = new_engine(items, cosine=item_norms is not None, device=B200ImplicitRanker.default_device, tc_mode=B200ImplicitRanker.default_tc_mode)
     try:
         indptr = indices = None
         if csr is not None:

@@ -21,7 +21,9 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 from scipy import sparse
 
-from .ranker import B200Ranker, Distance, Engine, _as_distance, _dense_f32, flatten_padded, rank_object_rows_padded
+from .ranker import (
+    B200Ranker, Devices, Distance, Engine, _as_distance, _dense_f32, flatten_padded, new_engine, parse_devices, rank_object_rows_padded,
+)
 
 _ENGINE_CACHE: "tp.Dict[tp.Tuple, Engine]" = {}
 _ENGINE_CACHE_MAX = 2
@@ -72,17 +74,18 @@ def content_hash(a: np.ndarray) -> bytes:
     return h.digest()
 
 
-def cached_engine(objects: np.ndarray, cosine: bool, device: int, tc_mode: str) -> Engine:
+def cached_engine(objects: np.ndarray, cosine: bool, device: tp.Union[int, tp.Tuple[int, ...]], tc_mode: str) -> Engine:
     """`VectorModel` builds a new ranker on every `recommend()` call (vector.py:66); keep the resident object factors
     across calls instead of re-uploading them (the reference GPU path re-uploads per call, rank_implicit.py:156).
     Keyed by the CONTENT of the matrix.  Evicted engines are only dropped from the cache: a ranker that still holds one
-    keeps it alive, the device memory is released when the last reference goes (`Engine.__del__`)."""
+    keeps it alive, the device memory is released when the last reference goes (`Engine.__del__`).  `device`: an int
+    (one engine) or a tuple of devices (an `EngineGroup`); the two never share an entry, even for one device."""
     key = (content_hash(objects), cosine, device, tc_mode)
     with _CACHE_LOCK:
         eng = _ENGINE_CACHE.get(key)
         if eng is not None:
             return eng
-    eng = Engine(objects, cosine=cosine, device=device, tc_mode=tc_mode)
+    eng = new_engine(objects, cosine=cosine, device=device, tc_mode=tc_mode)
     with _CACHE_LOCK:
         while len(_ENGINE_CACHE) >= _ENGINE_CACHE_MAX:
             _ENGINE_CACHE.pop(next(iter(_ENGINE_CACHE)))
@@ -99,7 +102,7 @@ class B200ImplicitRanker(B200Ranker):
     """`ImplicitRanker(distance, subjects_factors, objects_factors, num_threads=0, use_gpu=False)`-compatible
     constructor (rank_implicit.py:58-65) with a per-process engine cache keyed by the object matrix."""
 
-    default_device: int = 0
+    default_device: tp.Union[int, tp.Tuple[int, ...]] = 0  # a tuple: an engine group (install(device=[...]))
     default_tc_mode: str = "auto"
 
     def __init__(self, distance, subjects_factors, objects_factors, num_threads: int = 0, use_gpu: bool = False) -> None:
@@ -125,16 +128,20 @@ class B200TorchRanker(B200Ranker):
     materialised) and `dtype` other than fp32 is ignored: inputs are cast to fp32 like `_normalize_tensor` does by default.
 
     Difference kept from the reference: `TorchRanker` filters on CSR *values* != 0 (rank_torch.py:143) whereas the
-    implicit path uses the stored structure; explicit zeros are dropped here to keep the torch semantics."""
+    implicit path uses the stored structure; explicit zeros are dropped here to keep the torch semantics.
 
-    def __init__(self, distance, device, subjects_factors, objects_factors, batch_size: int = 128, dtype=None) -> None:
+    `devices` (not in the reference): rank on an engine group over these devices (a sequence or "all"); the factors'
+    device is its home device."""
+
+    def __init__(self, distance, device, subjects_factors, objects_factors, batch_size: int = 128, dtype=None,
+                 devices: tp.Optional[Devices] = None) -> None:
         dev_index = 0
         dev = str(device)
         if dev.startswith("cuda") and ":" in dev:
             dev_index = int(dev.split(":")[1])
         if hasattr(objects_factors, "detach") and dev.startswith("cuda") and not objects_factors.is_cuda:
             objects_factors = objects_factors.to(device)  # `TorchRanker` scores on `device` (rank_torch.py:135)
-        super().__init__(distance, subjects_factors, objects_factors, device=dev_index)
+        super().__init__(distance, subjects_factors, objects_factors, device=dev_index if devices is None else devices)
         self.batch_size = batch_size
 
     def rank(self, subject_ids, k=None, filter_pairs_csr=None, sorted_object_whitelist=None):
@@ -166,16 +173,20 @@ def ease_recommend_i2i(self, target_ids, dataset, k, sorted_item_ids_to_recommen
     return flatten_padded(target_ids, ids, scores, counts)
 
 
-def install(device: int = 0, tc_mode: str = "auto", fast_recommend: bool = True) -> None:
+def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = True) -> None:
     """Route `VectorModel` (ALS / PureSVD / LightFM / BPR / DSSM) and `EASEModel` ranking (u2i and i2i) through the B200
     engine.
+
+    `device`: an int ranks on that GPU; a sequence of ints (`[0, 1, 2, 3]`) or "all" (every visible GPU) ranks on an
+    engine group, one engine per entry, each call's rows split between them (same results; each member holds the whole
+    catalogue).
 
     `fast_recommend`: also give `VectorModel` the vectorised `recommend()` of `rectools_b200.recommend` (cached viewed-items
     CSR, id maps by array indexing, no per-user Python loop); warm / cold targets and context models still go through
     `ModelBase.recommend` (rectools/models/base.py:385-519)."""
     import importlib
 
-    B200ImplicitRanker.default_device = device
+    B200ImplicitRanker.default_device = parse_devices(device)
     B200ImplicitRanker.default_tc_mode = tc_mode
     for modname in ("rectools.models.vector", "rectools.models.ease"):
         mod = importlib.import_module(modname)
@@ -233,21 +244,24 @@ def uninstall() -> None:
     clear_engine_cache()
 
 
-def make_similarity_module(ranker_factory: tp.Optional[tp.Callable[..., tp.Any]] = None) -> type:
+def make_similarity_module(ranker_factory: tp.Optional[tp.Callable[..., tp.Any]] = None, devices: tp.Optional[Devices] = None) -> type:
     """`similarity_module_type` for SASRec / BERT4Rec / HSTU (rectools/models/nn/transformers/base.py:219, :423): the
     reference's `DistanceSimilarityModule` with `B200TorchRanker` as the scorer of `_recommend_u2i`
     (similarity.py:117-140).  `item_embs` stays on its device (and in its dtype: fp16 / bf16 embeddings are handed to the
     engine as they are); the filter stays a CSR (the reference densifies [batch, n_items] per batch, rank_torch.py:138-144).
-    `ranker_factory`: another `TorchRanker`-signature class (the CPU tests plug an oracle-backed stand-in in)."""
+    `ranker_factory`: another `TorchRanker`-signature class (the CPU tests plug an oracle-backed stand-in in).
+    `devices`: rank on an engine group over these devices (a sequence or "all", passed to the factory as `devices=`);
+    None ranks on the device of `item_embs`."""
     from rectools.models.nn.transformers.similarity import DistanceSimilarityModule  # needs torch only
 
     factory = ranker_factory or B200TorchRanker
+    group_kw = {} if devices is None else {"devices": parse_devices(devices)}
 
     class B200DistanceSimilarityModule(DistanceSimilarityModule):
         def _recommend_u2i(self, user_embs, item_embs, user_ids, k, sorted_item_ids_to_recommend, ui_csr_for_filter):
             ranker = factory(
                 distance=self.distance, device=item_embs.device, subjects_factors=user_embs[user_ids],
-                objects_factors=item_embs,
+                objects_factors=item_embs, **group_kw,
             )
             user_ids_indices, all_reco_ids, all_scores = ranker.rank(
                 subject_ids=np.arange(len(user_ids)), k=k, filter_pairs_csr=ui_csr_for_filter,

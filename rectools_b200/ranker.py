@@ -153,7 +153,7 @@ class Engine:
         self._subjects_owner = weakref.ref(owner) if owner is not None else None
         if key is not None and key == getattr(self, "_subjects_key", None):
             return
-        _lib.check(self._lib.b200_rank_set_subjects(self._h, subjects.ctypes.data, subjects.shape[0], 0))
+        self._set_subjects(subjects.ctypes.data, subjects.shape[0], 0)
         self._subjects_key = key
 
     @property
@@ -164,7 +164,10 @@ class Engine:
         return ref() if ref is not None else None
 
     def set_subjects_device(self, ptr: int, n_subjects: int) -> None:
-        _lib.check(self._lib.b200_rank_set_subjects(self._h, ptr, n_subjects, 1))
+        self._set_subjects(ptr, n_subjects, 1)
+
+    def _set_subjects(self, ptr: int, n_subjects: int, on_device: int) -> None:
+        _lib.check(self._lib.b200_rank_set_subjects(self._h, ptr, n_subjects, on_device))
 
     def peer_export(self, max_rows: int) -> bytes:
         """Allocate this engine's published-threshold array (threshold sharing between the ranks of an item-sharded
@@ -342,6 +345,133 @@ class Engine:
         return ids, scores, counts
 
 
+class EngineGroup(Engine):
+    """Owner of one `b200_rank_group*`: an engine per entry of `devices` (duplicates: several engines on one device), each
+    holding the whole catalogue, that rank the row slices of every call.  Results are bit for bit those of one `Engine`.
+    `devices[0]` is the home device: device pointers (objects, subjects, inputs and outputs of `topk_ptrs`) live there.
+    Threshold sharing, snapshots and id offsets are engine-only."""
+
+    def __init__(
+        self,
+        objects: tp.Optional[np.ndarray],
+        cosine: bool,
+        devices: tp.Sequence[int],
+        tc_mode: str = "auto",
+        objects_device_ptr: tp.Optional[int] = None,
+        shape: tp.Optional[tp.Tuple[int, int]] = None,
+        objects_dtype: int = _lib.DT_F32,
+    ) -> None:
+        self._lib = _lib.load()
+        self._h = C.c_void_p()
+        self.devices = tuple(int(d) for d in devices)
+        if not self.devices:
+            raise ValueError("an engine group needs at least one device")
+        if objects_device_ptr is not None:
+            assert shape is not None
+            n, d = shape
+            ptr, flags = objects_device_ptr, _lib.F_OBJECTS_ON_DEVICE
+        else:
+            objects = np.ascontiguousarray(objects, dtype=np.float32)
+            n, d = objects.shape
+            ptr, flags = objects.ctypes.data, 0
+        devs = (C.c_int32 * len(self.devices))(*self.devices)
+        _lib.check(
+            self._lib.b200_rank_group_create_ex(
+                C.byref(self._h), ptr, objects_dtype, n, d, _lib.DIST_COSINE if cosine else _lib.DIST_DOT, devs,
+                len(self.devices), _TC_MODES[tc_mode], flags,
+            )
+        )
+        self.n_objects, self.d, self.device = int(n), int(d), self.devices[0]
+        self.id_offset = 0
+        self.last_stats: tp.Dict[str, tp.Any] = {}
+        self.last_member_stats: tp.List[tp.Dict[str, tp.Any]] = []
+
+    def close(self) -> None:
+        if getattr(self, "_h", None) is not None and self._h.value:
+            self._lib.b200_rank_group_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def info(self) -> tp.Dict[str, tp.Any]:
+        """Member 0's engine info, `hbm_bytes` of the whole group, and `members`: every member's engine info."""
+        infos = (_lib.Info * len(self.devices))()
+        total = C.c_int64()
+        _lib.check(self._lib.b200_rank_group_get_info(self._h, infos, C.byref(total)))
+        members = []
+        for inf in infos:
+            m = {name: getattr(inf, name) for name, _ in inf._fields_}  # pylint: disable=protected-access
+            m["device_name"] = inf.device_name.decode()
+            members.append(m)
+        return {**members[0], "hbm_bytes": int(total.value), "members": members}
+
+    def _set_subjects(self, ptr: int, n_subjects: int, on_device: int) -> None:
+        _lib.check(self._lib.b200_rank_group_set_subjects(self._h, ptr, n_subjects, on_device))
+
+    def topk_raw(self, q: _lib.Query) -> tp.Dict[str, tp.Any]:
+        """`last_stats`: the group's totals (counters summed, times the maximum over members); `last_member_stats`: each
+        member's own."""
+        st = _lib.Stats()
+        per = (_lib.Stats * len(self.devices))()
+        _lib.check(self._lib.b200_rank_group_topk(self._h, C.byref(q), C.byref(st), per))
+        self.last_stats = st.as_dict()
+        self.last_member_stats = [p.as_dict() for p in per]
+        return self.last_stats
+
+    def peer_export(self, max_rows: int) -> bytes:
+        raise NotImplementedError("threshold sharing is for item-sharded engines (ShardedB200Ranker), not engine groups")
+
+    def peer_import(self, handles: tp.Sequence[bytes], self_index: int) -> None:
+        raise NotImplementedError("threshold sharing is for item-sharded engines (ShardedB200Ranker), not engine groups")
+
+    def peer_attach(self, pub: tp.Any, peers: tp.Sequence[tp.Any]) -> None:
+        raise NotImplementedError("threshold sharing is for item-sharded engines (ShardedB200Ranker), not engine groups")
+
+    def candidate_snapshot(self) -> tp.Optional[tp.Dict[str, tp.Any]]:
+        raise NotImplementedError("snapshots are taken by single engines")
+
+
+Devices = tp.Union[int, str, tp.Sequence[int]]
+
+
+def parse_devices(device: tp.Any) -> tp.Union[int, tp.Tuple[int, ...]]:
+    """`device` of `B200Ranker` / `install()`: an int is one engine on that device (returned unchanged); a sequence of
+    ints is an engine group over those devices (duplicates allowed), returned as a tuple; "all" is every visible device."""
+    if isinstance(device, (bool, np.bool_)):
+        raise TypeError(f"device must be an int, a sequence of ints or 'all', not {device!r}")
+    if isinstance(device, (int, np.integer)):
+        if device < 0:
+            raise ValueError(f"device {device} is negative")
+        return int(device)
+    if isinstance(device, str):
+        if device != "all":
+            raise ValueError(f"device must be an int, a sequence of ints or 'all', not {device!r}")
+        import torch
+
+        n = torch.cuda.device_count()
+        if n == 0:
+            raise _lib.B200RankError("device='all': no CUDA device available (the engine has no CPU fallback)")
+        return tuple(range(n))
+    try:
+        devices = tuple(device)
+    except TypeError:
+        raise TypeError(f"device must be an int, a sequence of ints or 'all', not {device!r}") from None
+    if not devices:
+        raise ValueError("device: an empty sequence of devices")
+    for d in devices:
+        if isinstance(d, (bool, np.bool_)) or not isinstance(d, (int, np.integer)):
+            raise TypeError(f"device: {d!r} is not a device ordinal")
+        if d < 0:
+            raise ValueError(f"device {d} is negative")
+    return tuple(int(d) for d in devices)
+
+
+def new_engine(objects: tp.Optional[np.ndarray], cosine: bool, device: tp.Any, tc_mode: str = "auto", **kw: tp.Any) -> Engine:
+    """An `Engine` for an int device, an `EngineGroup` for a sequence of devices or "all" (`parse_devices`)."""
+    dev = parse_devices(device)
+    if isinstance(dev, int):
+        return Engine(objects, cosine=cosine, device=dev, tc_mode=tc_mode, **kw)
+    return EngineGroup(objects, cosine=cosine, devices=dev, tc_mode=tc_mode, **kw)
+
+
 def rank_object_rows_padded(
     engine: Engine,
     target_ids: InternalIds,
@@ -427,7 +557,8 @@ class B200Ranker:
     distance : Distance | str
     subjects_factors : np.ndarray | scipy.sparse.csr_matrix | torch.Tensor, shape (n_subjects, n_factors)
     objects_factors : np.ndarray | torch.Tensor, shape (n_objects, n_factors)
-    device : int, CUDA device ordinal
+    device : int, CUDA device ordinal; or a sequence of ordinals / "all": an engine group that splits every call's rows
+        between one engine per entry (`EngineGroup`, same results)
     tc_mode : "auto" | "fp16" | "bf16" | "off" -- dtype of the tensor-core candidate pass ("off": fp64 kernel only)
     """
 
@@ -438,7 +569,7 @@ class B200Ranker:
         objects_factors: tp.Any,
         num_threads: int = 0,  # pylint: disable=unused-argument
         use_gpu: bool = True,  # pylint: disable=unused-argument
-        device: int = 0,
+        device: Devices = 0,
         tc_mode: str = "auto",
         engine: tp.Optional[Engine] = None,
         subjects_key: tp.Optional[tp.Hashable] = None,
@@ -450,7 +581,7 @@ class B200Ranker:
         if engine is None and self.distance != Distance.EUCLIDEAN and _is_cuda_tensor(objects_factors):
             # embeddings that already live on the GPU (transformer scorers keep `item_embs` on the device,
             # rectools/models/nn/transformers/lightning.py:391, :398): hand the device pointers over, no host round trip
-            self._init_from_device_tensors(subjects_factors, objects_factors, tc_mode)
+            self._init_from_device_tensors(subjects_factors, objects_factors, tc_mode, device)
             return
         objects = _dense_f32(objects_factors)
         if sparse.issparse(subjects_factors):
@@ -463,7 +594,7 @@ class B200Ranker:
             self._subjects_csr = csr.astype(np.float32)
             self.n_subjects, self.n_objects = csr.shape[0], objects.shape[0]
             self.subjects_norms = self.subjects_dots = None
-            self.engine = engine or Engine(objects, cosine=False, device=device, tc_mode=tc_mode)
+            self.engine = engine or new_engine(objects, cosine=False, device=device, tc_mode=tc_mode)
             self._subjects, self._subjects_key = None, None
             self.last_stats = {}
             return
@@ -472,12 +603,12 @@ class B200Ranker:
             raise ValueError("subject and object factors must have the same number of columns")
         self.n_subjects, self.n_objects = subjects.shape[0], objects.shape[0]
         subjects, objects, self.subjects_norms, self.subjects_dots = prepare_factors(self.distance, subjects, objects)
-        self.engine = engine or Engine(objects, cosine=self.distance == Distance.COSINE, device=device, tc_mode=tc_mode)
+        self.engine = engine or new_engine(objects, cosine=self.distance == Distance.COSINE, device=device, tc_mode=tc_mode)
         self._subjects, self._subjects_key = subjects, subjects_key
         self.engine.set_subjects(subjects, key=subjects_key, owner=self)
         self.last_stats: tp.Dict[str, tp.Any] = {}
 
-    def _init_from_device_tensors(self, subjects_factors: tp.Any, objects_factors: tp.Any, tc_mode: str) -> None:
+    def _init_from_device_tensors(self, subjects_factors: tp.Any, objects_factors: tp.Any, tc_mode: str, device: Devices = 0) -> None:
         import torch
 
         # fp16 / bf16 embeddings go to the engine as they are (widened exactly on the device: b200_rank_create_ex)
@@ -503,8 +634,16 @@ class B200Ranker:
             self.subjects_norms = norms.cpu().numpy()
         torch.cuda.current_stream(dev).synchronize()
         self._device_tensors = (subjects, objects)  # the engine references this memory: keep it alive
-        self.engine = Engine(
-            None, cosine=self.distance == Distance.COSINE, device=dev.index or 0, tc_mode=tc_mode,
+        home = dev.index or 0
+        devices = parse_devices(device)
+        if not isinstance(devices, int):  # a group whose home device is the tensors' device
+            if home not in devices:
+                raise ValueError(f"the factors live on cuda:{home}, which is not among the group's devices {devices}")
+            rest = list(devices)
+            rest.remove(home)
+            devices = (home, *rest)
+        self.engine = new_engine(
+            None, cosine=self.distance == Distance.COSINE, device=home if isinstance(devices, int) else devices, tc_mode=tc_mode,
             objects_device_ptr=objects.data_ptr(), shape=(self.n_objects, int(objects.shape[1])), objects_dtype=dtypes[objects.dtype],
         )
         self.engine.set_subjects_device(subjects.data_ptr(), self.n_subjects)
