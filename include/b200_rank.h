@@ -10,7 +10,8 @@
  *       `ImplicitRanker.__init__` object-factor handling (rectools/models/rank/rank_implicit.py:58-81) and the per-call
  *       upload of the whole item matrix by `implicit.gpu.Matrix` (rank_implicit.py:156, rectools/models/utils.py:136);
  *       `TorchRanker.__init__` / `item_embs.to(device)` (rank_torch.py:59-75, :135).  The engine keeps the object
- *       factors resident in HBM (fp32 master copy + fp16/bf16 tensor-core copy + fp32 row norms for COSINE,
+ *       factors resident in HBM (fp32 master copy, or fp16/bf16 with B200_F_OBJECTS_16BIT, + fp16/bf16 tensor-core
+ *       copy + fp32 row norms for COSINE,
  *       rank_implicit.py:98-105, :238-240).
  *   b200_rank_set_subjects
  *       `self.subjects_factors = subjects_factors.astype(np.float32)` (rank_implicit.py:70) -- resident subject
@@ -72,6 +73,7 @@ extern "C" {
 
 /* create flags */
 #define B200_F_OBJECTS_ON_DEVICE 1 /* `objects` is a device pointer on `device` */
+#define B200_F_OBJECTS_16BIT 2     /* fp16 / bf16 objects stay in their own type: no fp32 master copy (b200_rank_create_ex) */
 
 /* query flags */
 #define B200_Q_INPUTS_ON_DEVICE 1  /* subjects / subject_ids / object_rows / csr_* / whitelist are device pointers */
@@ -128,7 +130,8 @@ typedef struct b200_rank_query {
     const float* sub_data;
     /* ---- ABI 6: stored rows as score rows (EASEModel item-to-item: row t of the weight matrix, which the engine holds as
      * its objects, is the score row of target t, rectools/models/ease.py:163-188).  Batch row r is scored as
-     * score(r, j) = the engine's fp32 master copy [object_rows[r], j], bit for bit; the selection reads the row where it
+     * score(r, j) = the engine's master copy [object_rows[r], j] in fp32 (exactly widened when it is kept at 16 bits,
+     * B200_F_OBJECTS_16BIT), bit for bit; the selection reads the row where it
      * lies and never writes into it.  Given instead of `subjects` / `subject_ids` / `sub_*`.  Needs d == n_objects (the
      * row is indexed by object id: else B200_E_INVALID); refused with B200_E_UNSUPPORTED on COSINE engines, engines with a
      * non-zero id offset, B200_Q_SHARED_THRESHOLDS and B200_Q_FORCE_TC.  Entries must lie in [0, n_objects): checked for
@@ -183,12 +186,16 @@ typedef struct b200_rank_info {
 int b200_rank_create(b200_rank_engine** out, const float* objects, int64_t n_objects, int32_t d, int32_t distance,
                      int32_t device, int32_t tc_mode, int32_t flags);
 /* The same with an explicit element type: fp16 / bf16 object factors (transformer id-embedding scorers keep `item_embs`
- * in the model dtype, rectools/models/nn/transformers/lightning.py:391-398).  16-bit matrices must be device pointers
- * (B200_F_OBJECTS_ON_DEVICE); they are widened once into the engine's fp32 master copy, which is exact.
+ * in the model dtype, rectools/models/nn/transformers/lightning.py:391-398).  Without B200_F_OBJECTS_16BIT, 16-bit
+ * matrices must be device pointers (B200_F_OBJECTS_ON_DEVICE); they are widened once into the engine's fp32 master copy,
+ * which is exact.  With B200_F_OBJECTS_16BIT, fp16 / bf16 objects stay in their own type and the engine holds no fp32
+ * copy of them: every exact kernel widens each element on load, so results are bit for bit those of the widened engine.
+ * A 16-bit device matrix is then read in place for the engine's whole life, as an fp32 device matrix is; a 16-bit host
+ * matrix is accepted and uploaded into an owned 16-bit buffer.  The flag changes nothing for fp32 objects.
  * With B200_F_OBJECTS_ON_DEVICE (any dtype) create reads the device matrix after all work queued on the device, so
  * the caller's producer stream needs no synchronisation.  The object matrix must not change after create: the row norms,
- * eps and the tensor-core copy are derived from it once (an fp32 device matrix stays the engine's master copy and must
- * outlive the engine). */
+ * eps and the tensor-core copy are derived from it once.  A device matrix the engine reads in place (fp32, or 16-bit with
+ * B200_F_OBJECTS_16BIT) is its master copy: the caller keeps it alive and unchanged until destroy. */
 int b200_rank_create_ex(b200_rank_engine** out, const void* objects, int32_t dtype, int64_t n_objects, int32_t d,
                         int32_t distance, int32_t device, int32_t tc_mode, int32_t flags);
 int b200_rank_destroy(b200_rank_engine* engine);
@@ -285,8 +292,9 @@ int b200_rank_peer_attach(b200_rank_engine* engine, int64_t max_rows, void* pub,
  *   create:  the arguments of b200_rank_create[_ex] plus `devices` [n_devices] (member i runs on devices[i]; duplicates
  *            make several engines on one device).  devices[0] is the HOME device: device inputs and outputs of group
  *            calls live there, and with B200_F_OBJECTS_ON_DEVICE so does `objects`.  Members on the home device reference
- *            a device matrix as b200_rank_create does; members on other devices rank a peer copy made at create.  Every
- *            member holds a full engine's device memory.
+ *            a device matrix as b200_rank_create does; members on other devices rank a peer copy made at create (with
+ *            B200_F_OBJECTS_16BIT a 16-bit peer copy, which they read in place; without it, 16-bit objects are widened and
+ *            the peer copy is released).  `flags` go to every member.  Every member holds a full engine's device memory.
  *   set_subjects: on_device = 0 uploads the host matrix to every member; on_device = 1 takes a device matrix on the home
  *            device: home members reference it, members on other devices get a peer copy made here (so, for them, later
  *            changes of the matrix are not seen).

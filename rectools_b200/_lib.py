@@ -14,7 +14,7 @@ ABI_VERSION = 6
 OK, E_INVALID, E_CUDA, E_NOMEM, E_UNSUPPORTED = 0, -1, -2, -3, -4
 DIST_DOT, DIST_COSINE = 0, 1
 TC_AUTO, TC_FP16, TC_BF16, TC_OFF = 0, 1, 2, 3
-F_OBJECTS_ON_DEVICE = 1
+F_OBJECTS_ON_DEVICE, F_OBJECTS_16BIT = 1, 2
 Q_INPUTS_ON_DEVICE, Q_OUTPUTS_ON_DEVICE, Q_FORCE_EXACT, Q_FORCE_TC, Q_SHARED_THRESHOLDS = 1, 2, 4, 8, 16
 DT_F32, DT_F16, DT_BF16 = 0, 1, 2
 

@@ -12,6 +12,24 @@
 
 namespace b200 {
 
+// Object factors are read in their stored type (fp32, or fp16 / bf16 kept at 16 bits) and widened on load: every 16-bit
+// value is exact in fp32, so a kernel sees the operand a widened fp32 copy would have given it.
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+
+// The same from the raw 16 bits of one element (elements unpacked from a vector load).
+template <typename T>
+__device__ __forceinline__ float bits_to_f32(unsigned bits);
+template <>
+__device__ __forceinline__ float bits_to_f32<__half>(unsigned bits) {
+    return __half2float(__ushort_as_half((unsigned short)bits));
+}
+template <>
+__device__ __forceinline__ float bits_to_f32<__nv_bfloat16>(unsigned bits) {
+    return __bfloat162float(__ushort_as_bfloat16((unsigned short)bits));
+}
+
 // "a ranks before b": higher score first, ties by smaller object id (the order fixed by the oracle).
 __device__ __forceinline__ bool ranks_before(float as, int ai, float bs, int bi) {
     return as > bs || (as == bs && ai < bi);

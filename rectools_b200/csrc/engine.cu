@@ -67,6 +67,11 @@ struct DevBuf {
         CK(cudaMalloc(&p, want));
         cap = want;
     }
+    void ensure_exact(size_t bytes) {  // buffers that never grow (the resident objects): no slack
+        release();
+        CK(cudaMalloc(&p, bytes));
+        cap = bytes;
+    }
     void release() {
         if (p) cudaFree(p);
         p = nullptr;
@@ -129,14 +134,15 @@ struct b200_rank_engine {
     std::vector<cudaEvent_t> evt;       // timing pairs of the fused-kernel / selection launches of a call
 
     // resident object data
-    DevBuf obj32;     // [n_obj, d] fp32 master copy
+    DevBuf obj_own;   // [n_obj, d] owned master copy: fp32, or the uploaded 16-bit host matrix (B200_F_OBJECTS_16BIT)
     DevBuf obj16;     // [n_obj_pad, d_pad] fp16 / bf16, pre-scaled (and pre-normalised for COSINE)
     DevBuf obj_norms; // [n_obj] fp32 (COSINE)
     DevBuf objT;      // [d, n_obj] fp32 transposed master copy (sparse subjects only, built on first use)
     int obj_exp = 0;
     int64_t id_offset = 0;
     float max_obj_norm = 0.f;
-    const float* obj32_ptr = nullptr;
+    const void* obj_ptr = nullptr;  // the master copy every exact kernel reads: obj_own or the caller's device matrix
+    int obj_dtype = B200_DT_F32;    // its element type: fp32, or fp16 / bf16 kept at 16 bits
 
     // resident subjects (optional)
     DevBuf sub32_res;
@@ -171,7 +177,7 @@ struct b200_rank_engine {
     bool snap_has_rows = false;
 
     std::vector<DevBuf*> all_bufs() {
-        return {&obj32, &obj16, &obj_norms, &objT, &sub32_res, &peer_pub, &sub32, &sub16, &row_exp, &rowmap, &indptr, &indices, &wl,
+        return {&obj_own, &obj16, &obj_norms, &objT, &sub32_res, &peer_pub, &sub32, &sub16, &row_exp, &rowmap, &indptr, &indices, &wl,
                 &obj16_wl, &sp_indptr, &sp_indices, &sp_data, &sp_scores, &out_ids, &out_scores, &out_counts, &out_bounds, &cand_scores,
                 &cand_ids, &cand_counts, &cand_thr, &part_scores, &part_ids, &fb_rows, &scratch, &excl, &carousel, &patch, &lk_scratch,
                 &snap_scores, &snap_ids, &snap_counts, &snap_thr, &snap_row_exp, &snap_rows, &snap_fb};
@@ -207,6 +213,23 @@ using namespace b200;
 
 int grid_for(int64_t n, int block) { return (int)((n + block - 1) / block); }
 
+template <typename T>
+struct TypeTag {
+    using type = T;
+};
+
+// f(TypeTag<TO>{}) with TO the element type of the engine's master copy: every kernel that reads the objects is
+// instantiated for float, __half and __nv_bfloat16 and launched through this.
+template <typename F>
+void with_obj_type(const b200_rank_engine* E, F&& f) {
+    if (E->obj_dtype == B200_DT_F16)
+        f(TypeTag<__half>{});
+    else if (E->obj_dtype == B200_DT_BF16)
+        f(TypeTag<__nv_bfloat16>{});
+    else
+        f(TypeTag<float>{});
+}
+
 // ---- resident objects -------------------------------------------------------------------------------------
 void prepare_objects(b200_rank_engine* E, int tc_mode) {
     const int64_t n = E->n_obj;
@@ -217,8 +240,11 @@ void prepare_objects(b200_rank_engine* E, int tc_mode) {
     const bool cosine = E->distance == B200_DIST_COSINE;
     if (cosine) E->obj_norms.ensure(sizeof(float) * std::max<int64_t>(n, 1));
     if (n > 0)
-        row_stats_kernel<<<grid_for(n * 32, 256), 256, 0, E->st>>>(E->obj32_ptr, n, d, cosine ? 1 : 0,
-                                                                   cosine ? E->obj_norms.as<float>() : nullptr, g, g + 1);
+        with_obj_type(E, [&](auto t) {
+            using TO = typename decltype(t)::type;
+            row_stats_kernel<TO><<<grid_for(n * 32, 256), 256, 0, E->st>>>(static_cast<const TO*>(E->obj_ptr), n, d, cosine ? 1 : 0,
+                                                                           cosine ? E->obj_norms.as<float>() : nullptr, g, g + 1);
+        });
     CK(cudaGetLastError());
     unsigned h[2];
     CK(cudaMemcpyAsync(h, g, 8, cudaMemcpyDeviceToHost, E->st));
@@ -238,12 +264,16 @@ void prepare_objects(b200_rank_engine* E, int tc_mode) {
     E->obj16.ensure((size_t)E->n_obj_pad * E->d_pad * 2);
     const float* norms = cosine ? E->obj_norms.as<float>() : nullptr;
     const int grid = grid_for(E->n_obj_pad * 32, 256);
-    if (E->tc_dtype == B200_TC_FP16)
-        convert_rows_kernel<__half, false><<<grid, 256, 0, E->st>>>(E->obj32_ptr, nullptr, nullptr, n, E->n_obj_pad, d, E->d_pad, norms,
-                                                                    E->obj_exp, E->obj16.as<__half>(), nullptr);
-    else
-        convert_rows_kernel<__nv_bfloat16, false><<<grid, 256, 0, E->st>>>(E->obj32_ptr, nullptr, nullptr, n, E->n_obj_pad, d, E->d_pad,
-                                                                           norms, E->obj_exp, E->obj16.as<__nv_bfloat16>(), nullptr);
+    with_obj_type(E, [&](auto t) {
+        using TO = typename decltype(t)::type;
+        const TO* x = static_cast<const TO*>(E->obj_ptr);
+        if (E->tc_dtype == B200_TC_FP16)
+            convert_rows_kernel<TO, __half, false><<<grid, 256, 0, E->st>>>(x, nullptr, nullptr, n, E->n_obj_pad, d, E->d_pad, norms,
+                                                                            E->obj_exp, E->obj16.as<__half>(), nullptr);
+        else
+            convert_rows_kernel<TO, __nv_bfloat16, false><<<grid, 256, 0, E->st>>>(x, nullptr, nullptr, n, E->n_obj_pad, d, E->d_pad,
+                                                                                   norms, E->obj_exp, E->obj16.as<__nv_bfloat16>(), nullptr);
+    });
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(E->st));
 }
@@ -305,8 +335,9 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
         return fail(B200_E_INVALID, "b200_rank_create: distance must be B200_DIST_DOT or B200_DIST_COSINE");
     if (tc_mode < B200_TC_AUTO || tc_mode > B200_TC_OFF) return fail(B200_E_INVALID, "b200_rank_create: bad tc_mode");
     if (dtype < B200_DT_F32 || dtype > B200_DT_BF16) return fail(B200_E_INVALID, "b200_rank_create: bad dtype");
-    if (dtype != B200_DT_F32 && !(flags & B200_F_OBJECTS_ON_DEVICE))
-        return fail(B200_E_INVALID, "b200_rank_create: 16-bit object factors must be device pointers");
+    const bool keep16 = dtype != B200_DT_F32 && (flags & B200_F_OBJECTS_16BIT);  // the master copy stays at 16 bits
+    if (dtype != B200_DT_F32 && !keep16 && !(flags & B200_F_OBJECTS_ON_DEVICE))
+        return fail(B200_E_INVALID, "b200_rank_create: 16-bit object factors must be device pointers (or B200_F_OBJECTS_16BIT)");
     int n_dev = 0;
     if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0)
         return fail(B200_E_CUDA, "b200_rank_create: no CUDA device available (the engine has no CPU fallback)");
@@ -340,20 +371,22 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
         // create reads of it (the widening, the row norms and maxima that feed eps, the tensor-core copy) after all work
         // queued on the device
         if (flags & B200_F_OBJECTS_ON_DEVICE) CK(cudaDeviceSynchronize());
-        if ((flags & B200_F_OBJECTS_ON_DEVICE) && dtype == B200_DT_F32) {
-            E->obj32_ptr = reinterpret_cast<const float*>(objects);
+        E->obj_dtype = keep16 ? dtype : B200_DT_F32;
+        const size_t elem = keep16 ? 2 : sizeof(float);
+        if ((flags & B200_F_OBJECTS_ON_DEVICE) && (dtype == B200_DT_F32 || keep16)) {
+            E->obj_ptr = objects;  // read in place for the engine's whole life
         } else {
-            E->obj32.ensure(sizeof(float) * std::max<int64_t>(n_objects * d, 1));
+            E->obj_own.ensure_exact(elem * std::max<int64_t>(n_objects * d, 1));
             if (n_objects > 0) {
-                if (dtype == B200_DT_F32) {
-                    CK(cudaMemcpyAsync(E->obj32.p, objects, sizeof(float) * n_objects * d, cudaMemcpyHostToDevice, E->st));
+                if (dtype == B200_DT_F32 || keep16) {
+                    CK(cudaMemcpyAsync(E->obj_own.p, objects, elem * n_objects * d, cudaMemcpyHostToDevice, E->st));
                 } else {
                     widen16_kernel<<<grid_for(n_objects * d, 256), 256, 0, E->st>>>(objects, dtype == B200_DT_BF16 ? 1 : 0, n_objects * d,
-                                                                                   E->obj32.as<float>());
+                                                                                   E->obj_own.as<float>());
                     CK(cudaGetLastError());
                 }
             }
-            E->obj32_ptr = E->obj32.as<float>();
+            E->obj_ptr = E->obj_own.p;
         }
         if (tc_mode != B200_TC_OFF && E->d_pad > 1024) tc_mode = B200_TC_OFF;
         if (tc_mode == B200_TC_AUTO && dtype == B200_DT_BF16) tc_mode = B200_TC_BF16;  // bf16 factors: the tensor-core copy is exact
@@ -368,13 +401,16 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
                         CK(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, pl.smem_bytes));
             }
         }
-        CK(cudaFuncSetAttribute(rescore_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-        CK(cudaFuncSetAttribute(rescore_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
-        CK(cudaFuncSetAttribute(rescore_wide_large_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+        with_obj_type(E, [&](auto t) {
+            using TO = typename decltype(t)::type;
+            CK(cudaFuncSetAttribute(rescore_select_kernel<TO>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+            CK(cudaFuncSetAttribute(rescore_wide_kernel<TO>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
+            CK(cudaFuncSetAttribute(rescore_wide_large_kernel<TO>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+            CK(cudaFuncSetAttribute(row_select_kernel<TO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lk_smem_bytes(LK_SMEM_PAIRS)));
+        });
         // the largest launch of any call (k_out >= LK_SMEM_PAIRS); a fixed maximum: the attribute is shared by every engine
         // on the device, and smaller launches stay within it
         CK(cudaFuncSetAttribute(large_k_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lk_smem_bytes(LK_SMEM_PAIRS)));
-        CK(cudaFuncSetAttribute(row_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lk_smem_bytes(LK_SMEM_PAIRS)));
     } catch (const CudaError& ce) {
         int rc = fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_create: %s failed at line %d: %s",
                       ce.what, ce.line, cudaGetErrorString(ce.e));
@@ -466,7 +502,7 @@ void run_exact(Call& c, const int32_t* rows_dev, int64_t n_sel, const float* sub
         p.rows = rows_dev;
         p.n_sel_dev = nullptr;
         p.n_sel = n_sel;
-        p.objects = E->obj32_ptr;
+        p.objects = E->obj_ptr;
         p.pos2obj = c.wl;
         p.n_pos = c.n_pos;
         p.d = c.d;
@@ -484,7 +520,7 @@ void run_exact(Call& c, const int32_t* rows_dev, int64_t n_sel, const float* sub
         p.part_ids = E->part_ids.as<int32_t>();
         p.part_stride_rows = n_sel;
         if (timed) c.time_begin(0);
-        exact_topk_kernel<<<dim3(blocks_x, n_splits), EX_THREADS, 0, c.st>>>(p);
+        with_obj_type(E, [&](auto t) { exact_topk_kernel<typename decltype(t)::type><<<dim3(blocks_x, n_splits), EX_THREADS, 0, c.st>>>(p); });
         CK(cudaGetLastError());
         if (timed) c.time_end();
         SelectParams sp{};
@@ -593,11 +629,11 @@ void run_tc(Call& c, const TcPass& t) {
     {
         const int grid = grid_for(rows_pad * 32, 256);
         if (!bf16)
-            convert_rows_kernel<__half, true><<<grid, 256, 0, st>>>(t.sub32, t.rowmap, t.rows_dev, t.n_sel, rows_pad, d, E->d_pad, nullptr, 0,
-                                                                    E->sub16.as<__half>(), E->row_exp.as<int32_t>());
+            convert_rows_kernel<float, __half, true><<<grid, 256, 0, st>>>(t.sub32, t.rowmap, t.rows_dev, t.n_sel, rows_pad, d, E->d_pad, nullptr,
+                                                                           0, E->sub16.as<__half>(), E->row_exp.as<int32_t>());
         else
-            convert_rows_kernel<__nv_bfloat16, true><<<grid, 256, 0, st>>>(t.sub32, t.rowmap, t.rows_dev, t.n_sel, rows_pad, d, E->d_pad, nullptr,
-                                                                           0, E->sub16.as<__nv_bfloat16>(), E->row_exp.as<int32_t>());
+            convert_rows_kernel<float, __nv_bfloat16, true><<<grid, 256, 0, st>>>(t.sub32, t.rowmap, t.rows_dev, t.n_sel, rows_pad, d, E->d_pad,
+                                                                                  nullptr, 0, E->sub16.as<__nv_bfloat16>(), E->row_exp.as<int32_t>());
         CK(cudaGetLastError());
         c.S.n_launches++;
     }
@@ -720,7 +756,7 @@ void run_tc(Call& c, const TcPass& t) {
     sp.out_counts = t.o_counts;
     sp.subjects = t.sub32;
     sp.row_map = t.rowmap;
-    sp.objects = E->obj32_ptr;
+    sp.objects = E->obj_ptr;
     sp.obj_norms = c.norms();
     sp.d = d;
     sp.row_exp = E->row_exp.as<int32_t>();
@@ -735,14 +771,17 @@ void run_tc(Call& c, const TcPass& t) {
     sp.fb_row0 = t.rows_dev ? 0 : t.row0;
     sp.out_bounds = t.o_bounds;
     c.time_begin(1);
-    if (t.mode == TcMode::WIDE_L) {
-        rescore_wide_large_kernel<<<(unsigned)t.n_sel, WIDE_THREADS_L, wide_large_smem(d), st>>>(sp);
-    } else if (wide) {
-        rescore_wide_kernel<<<(unsigned)t.n_sel, WIDE_THREADS, (size_t)d * sizeof(float), st>>>(sp);
-    } else {
-        const size_t sel_smem = (size_t)SEL_WARPS * d * sizeof(float);
-        rescore_select_kernel<<<grid_for(t.n_sel, SEL_WARPS), SEL_WARPS * 32, sel_smem, st>>>(sp);
-    }
+    with_obj_type(E, [&](auto tag) {
+        using TO = typename decltype(tag)::type;
+        if (t.mode == TcMode::WIDE_L) {
+            rescore_wide_large_kernel<TO><<<(unsigned)t.n_sel, WIDE_THREADS_L, wide_large_smem(d), st>>>(sp);
+        } else if (wide) {
+            rescore_wide_kernel<TO><<<(unsigned)t.n_sel, WIDE_THREADS, (size_t)d * sizeof(float), st>>>(sp);
+        } else {
+            const size_t sel_smem = (size_t)SEL_WARPS * d * sizeof(float);
+            rescore_select_kernel<TO><<<grid_for(t.n_sel, SEL_WARPS), SEL_WARPS * 32, sel_smem, st>>>(sp);
+        }
+    });
     CK(cudaGetLastError());
     c.time_end();
     c.S.n_launches++;
@@ -791,10 +830,13 @@ void run_sparse(Call& c, const int64_t* sp_indptr, const int32_t* sp_indices, co
                 int32_t* o_ids, float* o_scores, int32_t* o_counts, Select sel) {
     b200_rank_engine* E = c.E;
     cudaStream_t st = c.st;
-    if (!E->objT.p && E->n_obj > 0) {  // transposed master copy, built once
+    if (!E->objT.p && E->n_obj > 0) {  // transposed fp32 master copy, built once
         E->objT.ensure(sizeof(float) * (size_t)E->n_obj * E->d);
-        transpose_kernel<<<dim3((unsigned)grid_for(E->n_obj, 32), (unsigned)grid_for(E->d, 32)), dim3(32, 8), 0, st>>>(E->obj32_ptr, E->n_obj, E->d,
-                                                                                                                  E->objT.as<float>());
+        with_obj_type(E, [&](auto t) {
+            using TO = typename decltype(t)::type;
+            transpose_kernel<TO><<<dim3((unsigned)grid_for(E->n_obj, 32), (unsigned)grid_for(E->d, 32)), dim3(32, 8), 0, st>>>(
+                static_cast<const TO*>(E->obj_ptr), E->n_obj, E->d, E->objT.as<float>());
+        });
         CK(cudaGetLastError());
         c.S.n_launches++;
     }
@@ -843,9 +885,12 @@ void run_dense_large_k(Call& c, const int32_t* rows, const float* sub32, const i
         const int splits = (int)std::max<int64_t>(1, std::min<int64_t>((4 * E->sm_count + blocks_x - 1) / blocks_x, tiles_total));
         const int32_t* rl = rows ? rows + b0 : nullptr;
         if (timed) c.time_begin(0);
-        dense_scores_kernel<<<dim3((unsigned)blocks_x, (unsigned)splits), 256, 0, st>>>(
-            (rowmap || rows) ? sub32 : sub32 + b0 * c.d, (rowmap && !rows) ? rowmap + b0 : rowmap, rl, nb, E->obj32_ptr, c.wl, c.n_pos,
-            c.d, c.norms(), E->sp_scores.as<float>());
+        with_obj_type(E, [&](auto t) {
+            using TO = typename decltype(t)::type;
+            dense_scores_kernel<TO><<<dim3((unsigned)blocks_x, (unsigned)splits), 256, 0, st>>>(
+                (rowmap || rows) ? sub32 : sub32 + b0 * c.d, (rowmap && !rows) ? rowmap + b0 : rowmap, rl, nb,
+                static_cast<const TO*>(E->obj_ptr), c.wl, c.n_pos, c.d, c.norms(), E->sp_scores.as<float>());
+        });
         CK(cudaGetLastError());
         if (timed) c.time_end();
         c.S.n_launches++;
@@ -872,7 +917,7 @@ void run_rows(Call& c, const int64_t* obj_rows, const int64_t* f_indptr, int64_t
     b200_rank_engine* E = c.E;
     if (c.k_out > LK_SMEM_PAIRS) E->lk_scratch.ensure((size_t)rows_row_bytes(c.k_out) * nr);
     RowSelectParams rp{};
-    rp.objects = E->obj32_ptr;
+    rp.objects = E->obj_ptr;
     rp.n_obj = E->n_obj;
     rp.d = E->d;
     rp.object_rows = obj_rows;
@@ -888,7 +933,7 @@ void run_rows(Call& c, const int64_t* obj_rows, const int64_t* f_indptr, int64_t
     rp.out_scores = o_scores;
     rp.out_counts = o_counts;
     c.time_begin(1);
-    row_select_kernel<<<(unsigned)nr, LK_THREADS, lk_smem_bytes(c.k_out), c.st>>>(rp);
+    with_obj_type(E, [&](auto t) { row_select_kernel<typename decltype(t)::type><<<(unsigned)nr, LK_THREADS, lk_smem_bytes(c.k_out), c.st>>>(rp); });
     CK(cudaGetLastError());
     c.time_end();
     c.S.n_launches++;

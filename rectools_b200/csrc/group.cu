@@ -302,7 +302,7 @@ void destroy_group(b200_group* g) {
     for (GroupMember& M : g->m)
         if (M.worker.joinable()) M.worker.join();
     for (GroupMember& M : g->m) {
-        if (M.E) b200_rank_destroy(M.E);  // before the peer copy an fp32 member references
+        if (M.E) b200_rank_destroy(M.E);  // before the peer copy an fp32 (or kept 16-bit) member references
         cudaSetDevice(M.device);
         for (DBuf* b : M.bufs()) b->release();
         if (M.st) cudaStreamDestroy(M.st);
@@ -371,7 +371,7 @@ int group_create(b200_group** out, const void* objects, int32_t dtype, int64_t n
                 destroy_group(g);
                 return ret;
             }
-            if (!M.home && dtype != B200_DT_F32) {  // widened into the engine's own master copy
+            if (!M.home && dtype != B200_DT_F32 && !(flags & B200_F_OBJECTS_16BIT)) {  // widened into the engine's own master copy
                 GCK(cudaSetDevice(M.device));
                 M.objects.release();
             }

@@ -9,7 +9,9 @@ namespace b200 {
 
 // One warp per row: fp32 L2 norm accumulated in fp64 (zero -> 1e-10, rank_implicit.py:103-104), plus the global maxima
 // needed for the fp16 scale and for the certificate bound (non-negative floats order like their bit patterns).
-__global__ void row_stats_kernel(const float* __restrict__ x, int64_t n, int d, int normalise, float* __restrict__ norms,
+// TX: the stored object type (float, __half, __nv_bfloat16), widened on load.
+template <typename TX>
+__global__ void row_stats_kernel(const TX* __restrict__ x, int64_t n, int d, int normalise, float* __restrict__ norms,
                                  unsigned* __restrict__ g_absmax_bits, unsigned* __restrict__ g_maxnorm_bits) {
     const int lane = threadIdx.x & 31;
     const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -17,7 +19,7 @@ __global__ void row_stats_kernel(const float* __restrict__ x, int64_t n, int d, 
     double ss = 0.0;
     float amax = 0.f;
     for (int j = lane; j < d; j += 32) {
-        const float v = x[row * d + j];
+        const float v = to_f32(x[row * d + j]);
         ss = fma((double)v, (double)v, ss);
         amax = fmaxf(amax, fabsf(v));
     }
@@ -62,8 +64,9 @@ __host__ __device__ __forceinline__ int fp16_scale_exp(float amax) {
 
 // One warp per output row: out[row, 0:d_pad] = T( x[src_row, :] (/ norm) * 2^e ), zero padded in rows and columns.
 // PER_ROW_EXP: e is chosen per row (subjects) and written to row_exp; otherwise `fixed_exp` (objects) is used.
-template <typename T, bool PER_ROW_EXP>
-__global__ void convert_rows_kernel(const float* __restrict__ x, const int64_t* __restrict__ row_map,
+// TX: the type of x (fp32 subjects; objects in their stored type), widened on load.
+template <typename TX, typename T, bool PER_ROW_EXP>
+__global__ void convert_rows_kernel(const TX* __restrict__ x, const int64_t* __restrict__ row_map,
                                     const int32_t* __restrict__ sel_rows, int64_t n, int64_t n_pad, int d, int d_pad,
                                     const float* __restrict__ norms, int fixed_exp, T* __restrict__ out,
                                     int32_t* __restrict__ row_exp) {
@@ -77,12 +80,12 @@ __global__ void convert_rows_kernel(const float* __restrict__ x, const int64_t* 
     }
     const int64_t lrow = sel_rows ? (int64_t)sel_rows[row] : row;  // compact batch row -> logical row -> physical row
     const int64_t src = row_map ? row_map[lrow] : lrow;
-    const float* xr = x + src * d;
+    const TX* xr = x + src * d;
     const float inv = norms ? norms[src] : 1.f;
     int e = fixed_exp;
     if (PER_ROW_EXP) {
         float amax = 0.f;
-        for (int j = lane; j < d; j += 32) amax = fmaxf(amax, fabsf(xr[j]));
+        for (int j = lane; j < d; j += 32) amax = fmaxf(amax, fabsf(to_f32(xr[j])));
 #pragma unroll
         for (int o2 = 16; o2 > 0; o2 >>= 1) amax = fmaxf(amax, __shfl_xor_sync(B200_FULL_MASK, amax, o2));
         e = fp16_scale_exp(amax);
@@ -91,7 +94,7 @@ __global__ void convert_rows_kernel(const float* __restrict__ x, const int64_t* 
     for (int j = lane; j < d_pad; j += 32) {
         float v = 0.f;
         if (j < d) {
-            v = xr[j];
+            v = to_f32(xr[j]);
             if (norms) v = v / inv;
             v = ldexpf(v, e);
         }
@@ -128,15 +131,16 @@ __global__ void iota_kernel(int32_t* __restrict__ out, int64_t n) {
     if (i < n) out[i] = (int32_t)i;
 }
 
-// [n, d] row-major -> [d, n] row-major (32 x 32 tiles through shared memory).
-__global__ void transpose_kernel(const float* __restrict__ in, int64_t n, int d, float* __restrict__ out) {
+// [n, d] row-major -> [d, n] row-major fp32 (32 x 32 tiles through shared memory); TX: the stored type, widened on load.
+template <typename TX>
+__global__ void transpose_kernel(const TX* __restrict__ in, int64_t n, int d, float* __restrict__ out) {
     __shared__ float tile[32][33];
     const int64_t r0 = (int64_t)blockIdx.x * 32;
     const int c0 = blockIdx.y * 32;
     for (int i = threadIdx.y; i < 32; i += blockDim.y) {
         const int64_t r = r0 + i;
         const int c = c0 + threadIdx.x;
-        tile[i][threadIdx.x] = (r < n && c < d) ? in[r * d + c] : 0.f;
+        tile[i][threadIdx.x] = (r < n && c < d) ? to_f32(in[r * d + c]) : 0.f;
     }
     __syncthreads();
     for (int i = threadIdx.y; i < 32; i += blockDim.y) {

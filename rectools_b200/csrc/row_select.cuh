@@ -1,5 +1,5 @@
 // Top-k_out selection of rows the engine already holds (path 4, b200_rank_query.object_rows): batch row r is scored as
-// score(r, j) = obj32[object_rows[r], j], the fp32 master row itself (EASE item-to-item: row t of the weight matrix is
+// score(r, j) = obj[object_rows[r], j], the master row itself, widened to fp32 when it is kept at 16 bits (EASE item-to-item: row t of the weight matrix is
 // target t's score row).  One CTA per row reads the stored row where it lies and writes nothing into it, so the filter is
 // applied on the fly instead of by filter_mask_kernel.  Otherwise this is large_k_select_kernel (large_k_select.cuh) with
 // a different row source, built from the same pieces: radix select on order_key, stable compaction of the survivors in
@@ -20,7 +20,7 @@
 namespace b200 {
 
 struct RowSelectParams {
-    const float* objects;       // [n_obj, d] fp32 master copy, d == n_obj
+    const void* objects;        // [n_obj, d] stored objects in the kernel's type TO (fp32, fp16 or bf16), d == n_obj
     int64_t n_obj = 0, d = 0;
     const int64_t* object_rows;  // [n_rows] stored row of each batch row (in range: checked on the host for host inputs)
     int64_t n_rows = 0, n_pos = 0;
@@ -63,7 +63,9 @@ __device__ __forceinline__ bool rs_listed(const int32_t* __restrict__ f, int64_t
     return lo < end && __ldg(f + lo) == id;
 }
 
-// One CTA per batch row; dynamic shared memory lk_smem_bytes(k_out).
+// One CTA per batch row; dynamic shared memory lk_smem_bytes(k_out).  A 16-bit stored row is widened to fp32 before the
+// order key is taken, so its keys and returned scores are those of its widened fp32 copy.
+template <typename TO>
 __global__ void __launch_bounds__(LK_THREADS) row_select_kernel(const RowSelectParams p) {
     extern __shared__ uint32_t lk_smem[];
     __shared__ uint32_t hist[256];
@@ -73,9 +75,9 @@ __global__ void __launch_bounds__(LK_THREADS) row_select_kernel(const RowSelectP
     const int tid = threadIdx.x;
     const int64_t r = blockIdx.x;
     const int64_t n_pos = p.n_pos;
-    const float* srow = p.objects + __ldg(p.object_rows + r) * p.d;
+    const TO* srow = static_cast<const TO*>(p.objects) + __ldg(p.object_rows + r) * p.d;
     const int32_t* wl = p.pos2obj;
-    auto score = [&](int64_t pos) { return __ldg(srow + (wl ? (int64_t)__ldg(wl + pos) : pos)); };
+    auto score = [&](int64_t pos) { return to_f32(__ldg(srow + (wl ? (int64_t)__ldg(wl + pos) : pos))); };
     const int64_t f_lo = p.f_indptr ? __ldg(p.f_indptr + r) : 0, f_hi = p.f_indptr ? __ldg(p.f_indptr + r + 1) : 0;
     constexpr int64_t TILE = (int64_t)LK_THREADS * LK_ITEMS;
 

@@ -4,6 +4,8 @@
 // rectools/models/rank/rank_implicit.py:264-272 (score, /item_norms, CSR mask, per-row top-k), with the result
 // definition of include/b200_rank.h (fp64-accumulated dot rounded once to fp32; order = score desc, id asc).
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 #include "sizes.h"
 
@@ -25,7 +27,7 @@ struct ExactParams {
     const int32_t* rows;     // nullable: compact index -> logical row (re-rank subset)
     const int32_t* n_sel_dev;  // nullable: device-side count overriding n_sel (early exit for unused blocks)
     int64_t n_sel;           // number of compact indices
-    const float* objects;    // fp32 [n_objects, d]
+    const void* objects;     // [n_objects, d] in the kernel's object type TO (fp32, fp16 or bf16)
     const int32_t* pos2obj;  // nullable whitelist: position -> object id (sorted ascending)
     int64_t n_pos;
     int32_t d;
@@ -44,7 +46,9 @@ struct ExactParams {
     int64_t part_stride_rows;  // >= n_sel
 };
 
+template <typename TO>
 __global__ void __launch_bounds__(EX_THREADS) exact_topk_kernel(const ExactParams p) {
+    const TO* objects = static_cast<const TO*>(p.objects);
     __shared__ float s_obj[32][EX_DK + 1];
     __shared__ float s_sub[EX_ROWS][EX_DK];
 
@@ -104,7 +108,7 @@ __global__ void __launch_bounds__(EX_THREADS) exact_topk_kernel(const ExactParam
                 float v = 0.f;
                 if (pos < p.n_pos && dk0 + j < p.d) {
                     const int64_t obj = p.pos2obj ? (int64_t)p.pos2obj[pos] : pos;
-                    v = __ldg(p.objects + obj * p.d + dk0 + j);
+                    v = to_f32(__ldg(objects + obj * p.d + dk0 + j));
                 }
                 s_obj[it][j] = v;
             }
@@ -177,7 +181,8 @@ __global__ void __launch_bounds__(EX_THREADS) exact_topk_kernel(const ExactParam
 //   merge_select_kernel   : lists carry final scores (exhaustive-kernel partial lists, per-shard results of an
 //                           item-sharded catalogue); optional certificate over per-list bounds.
 //   rescore_select_kernel : lists carry approximate (tensor-core) scores; every candidate is re-scored in fp64 from the
-//                           fp32 master copies and the row is certified or queued for a re-rank (kp <= 32).
+//                           master copies (objects: fp32, or fp16 / bf16 widened on load) and the row is certified or
+//                           queued for a re-rank (kp <= 32).
 //   rescore_wide_kernel   : the same for the wide mode (kp <= 128, up to 512 candidates per row), one block per row;
 //   rescore_wide_large_kernel : the wide mode for 128 < kp <= 1024 (up to 4096 candidates per row), one block per row.
 // Certificate: every list reports the final pruning threshold `thr` of its stream -- no discarded object had an
@@ -203,7 +208,7 @@ struct SelectParams {
     // re-scoring inputs
     const float* subjects;
     const int64_t* row_map;
-    const float* objects;
+    const void* objects;       // [n_objects, d] in the re-score kernel's object type TO (fp32, fp16 or bf16)
     const float* obj_norms;
     int32_t d;
     // certificate
@@ -294,27 +299,50 @@ __global__ void __launch_bounds__(SEL_WARPS * 32) merge_select_kernel(const Sele
     }
 }
 
-// fp64-accumulated dot of the staged subject row with object `id` (the result definition of include/b200_rank.h)
+// fp64-accumulated dot of the staged subject row with object `id` (the result definition of include/b200_rank.h).  The
+// elements are summed in index order whatever the load width, so a 16-bit row gives the sum of its widened fp32 copy.
+template <typename TO>
 __device__ __forceinline__ float exact_score(const SelectParams& p, const float* sub, int id) {
     double acc = 0.0;
-    const float* orow = p.objects + (int64_t)id * p.d;
-    if ((p.d & 3) == 0) {
-        const float4* o4 = reinterpret_cast<const float4*>(orow);
-        const float4* s4 = reinterpret_cast<const float4*>(sub);
-        for (int j = 0; j < (p.d >> 2); ++j) {
-            const float4 ov = __ldg(o4 + j);
-            const float4 sv = s4[j];
-            acc = fma((double)ov.x, (double)sv.x, acc);
-            acc = fma((double)ov.y, (double)sv.y, acc);
-            acc = fma((double)ov.z, (double)sv.z, acc);
-            acc = fma((double)ov.w, (double)sv.w, acc);
+    const TO* orow = static_cast<const TO*>(p.objects) + (int64_t)id * p.d;
+    if constexpr (std::is_same<TO, float>::value) {
+        if ((p.d & 3) == 0) {
+            const float4* o4 = reinterpret_cast<const float4*>(orow);
+            const float4* s4 = reinterpret_cast<const float4*>(sub);
+            for (int j = 0; j < (p.d >> 2); ++j) {
+                const float4 ov = __ldg(o4 + j);
+                const float4 sv = s4[j];
+                acc = fma((double)ov.x, (double)sv.x, acc);
+                acc = fma((double)ov.y, (double)sv.y, acc);
+                acc = fma((double)ov.z, (double)sv.z, acc);
+                acc = fma((double)ov.w, (double)sv.w, acc);
+            }
+        } else {
+            for (int j = 0; j < p.d; ++j) acc = fma((double)__ldg(orow + j), (double)sub[j], acc);
         }
-    } else {
-        for (int j = 0; j < p.d; ++j) acc = fma((double)__ldg(orow + j), (double)sub[j], acc);
+    } else if ((p.d & 7) == 0 && (reinterpret_cast<uintptr_t>(orow) & 15) == 0) {
+        // 16-bit rows that start on a 16-byte boundary (d % 8 == 0, aligned matrix): 8 elements per load
+        const uint4* o8 = reinterpret_cast<const uint4*>(orow);
+        const float4* s4 = reinterpret_cast<const float4*>(sub);
+        for (int j = 0; j < (p.d >> 3); ++j) {
+            const uint4 ov = __ldg(o8 + j);
+            const float4 sa = s4[2 * j], sb = s4[2 * j + 1];
+            acc = fma((double)bits_to_f32<TO>(ov.x), (double)sa.x, acc);
+            acc = fma((double)bits_to_f32<TO>(ov.x >> 16), (double)sa.y, acc);
+            acc = fma((double)bits_to_f32<TO>(ov.y), (double)sa.z, acc);
+            acc = fma((double)bits_to_f32<TO>(ov.y >> 16), (double)sa.w, acc);
+            acc = fma((double)bits_to_f32<TO>(ov.z), (double)sb.x, acc);
+            acc = fma((double)bits_to_f32<TO>(ov.z >> 16), (double)sb.y, acc);
+            acc = fma((double)bits_to_f32<TO>(ov.w), (double)sb.z, acc);
+            acc = fma((double)bits_to_f32<TO>(ov.w >> 16), (double)sb.w, acc);
+        }
+    } else {  // any other 16-bit row: element by element (no head / tail to align)
+        for (int j = 0; j < p.d; ++j) acc = fma((double)to_f32(__ldg(orow + j)), (double)sub[j], acc);
     }
     return p.obj_norms ? (float)(acc / (double)__ldg(p.obj_norms + id)) : (float)acc;
 }
 
+template <typename TO>
 __global__ void __launch_bounds__(SEL_WARPS * 32) rescore_select_kernel(const SelectParams p) {
     extern __shared__ float s_sub[];  // [SEL_WARPS][d] subject rows
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -400,7 +428,7 @@ __global__ void __launch_bounds__(SEL_WARPS * 32) rescore_select_kernel(const Se
             skip = valid && (double)approx < (double)a_k - 2.0 * eps_scaled * (1.0 + 1e-6);
         }
         float s = -INFINITY;
-        if (valid && !skip) s = exact_score(p, sub, id);
+        if (valid && !skip) s = exact_score<TO>(p, sub, id);
         valid = valid && !skip && (s < bs || (s == bs && id > bi));
         n_valid += __popc(__ballot_sync(B200_FULL_MASK, skip));  // still candidates of the row (the certificate counts them)
         if (!valid) {
@@ -486,7 +514,7 @@ __device__ __forceinline__ T warp_slots_sum(const T* s_part) {
 }
 
 // The body shared by both wide re-score kernels: s_dyn = subject row [d], s_sc / s_id = MAX candidate slots.
-template <int THREADS, int MAX>
+template <int THREADS, int MAX, typename TO>
 __device__ __forceinline__ void rescore_wide_row(const SelectParams& p, float* s_dyn, float* s_sc, int* s_id) {
     __shared__ int s_off[65];
     __shared__ double s_red[THREADS / 32];
@@ -590,7 +618,7 @@ __device__ __forceinline__ void rescore_wide_row(const SelectParams& p, float* s
         int id = B200_PAD_ID;
         if (c < m) {
             id = s_id[c];
-            s = exact_score(p, s_dyn, id);
+            s = exact_score<TO>(p, s_dyn, id);
             if (!(s < bs || (s == bs && id > bi))) {  // (later passes: at or above the previous pass's last entry)
                 s = -INFINITY;
                 id = B200_PAD_ID;
@@ -631,21 +659,23 @@ __device__ __forceinline__ void rescore_wide_row(const SelectParams& p, float* s
     }
 }
 
+template <typename TO>
 __global__ void __launch_bounds__(WIDE_THREADS) rescore_wide_kernel(const SelectParams p) {
     extern __shared__ float s_dyn[];  // [d] subject row
     __shared__ float s_sc[WIDE_MAX];
     __shared__ int s_id[WIDE_MAX];
-    rescore_wide_row<WIDE_THREADS, WIDE_MAX>(p, s_dyn, s_sc, s_id);
+    rescore_wide_row<WIDE_THREADS, WIDE_MAX, TO>(p, s_dyn, s_sc, s_id);
 }
 
 // dynamic shared memory: [d] subject row (rounded up to 4 floats), [WIDE_MAX_L] scores, [WIDE_MAX_L] ids
 __host__ __device__ constexpr size_t wide_large_smem(int d) { return ((size_t)(d + 3) / 4 * 4 + 2 * WIDE_MAX_L) * 4; }
 
+template <typename TO>
 __global__ void __launch_bounds__(WIDE_THREADS_L) rescore_wide_large_kernel(const SelectParams p) {
     extern __shared__ float s_dyn[];
     float* s_sc = s_dyn + (p.d + 3) / 4 * 4;
     int* s_id = reinterpret_cast<int*>(s_sc + WIDE_MAX_L);
-    rescore_wide_row<WIDE_THREADS_L, WIDE_MAX_L>(p, s_dyn, s_sc, s_id);
+    rescore_wide_row<WIDE_THREADS_L, WIDE_MAX_L, TO>(p, s_dyn, s_sc, s_id);
 }
 
 // Multi-pass ranking: the ids a row has received so far, sorted ascending, become the row's exclusion list for the next

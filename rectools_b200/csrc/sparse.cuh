@@ -72,10 +72,12 @@ __global__ void __launch_bounds__(SP_THREADS) sparse_scores_kernel(const int64_t
 // Block = 32 subjects x 32 positions per step (lane = position), grid (row blocks, position splits).
 // `rows` (nullable): entry r of the batch is logical row rows[r] (the rows a wide pass could not certify); score row r of
 // the output stays compact.
+// TO: the stored object type (fp32, fp16 or bf16), widened on load.
 constexpr int DS_DK = 64;
 
+template <typename TO>
 __global__ void __launch_bounds__(256) dense_scores_kernel(const float* __restrict__ subjects, const int64_t* __restrict__ row_map,
-                                                           const int32_t* __restrict__ rows, int64_t n_rows, const float* __restrict__ objects,
+                                                           const int32_t* __restrict__ rows, int64_t n_rows, const TO* __restrict__ objects,
                                                            const int32_t* __restrict__ pos2obj, int64_t n_pos, int32_t d,
                                                            const float* __restrict__ obj_norms, float* __restrict__ scores) {
     __shared__ float s_obj[32][DS_DK + 1];
@@ -95,7 +97,7 @@ __global__ void __launch_bounds__(256) dense_scores_kernel(const float* __restri
                 float v = 0.f;
                 if (pos < n_pos && dk0 + j < d) {
                     const int64_t obj = pos2obj ? (int64_t)pos2obj[pos] : pos;
-                    v = __ldg(objects + obj * d + dk0 + j);
+                    v = to_f32(__ldg(objects + obj * d + dk0 + j));
                 }
                 s_obj[it][j] = v;
                 const int64_t r = row0 + it;

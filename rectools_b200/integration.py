@@ -79,7 +79,9 @@ def cached_engine(objects: np.ndarray, cosine: bool, device: tp.Union[int, tp.Tu
     across calls instead of re-uploading them (the reference GPU path re-uploads per call, rank_implicit.py:156).
     Keyed by the CONTENT of the matrix.  Evicted engines are only dropped from the cache: a ranker that still holds one
     keeps it alive, the device memory is released when the last reference goes (`Engine.__del__`).  `device`: an int
-    (one engine) or a tuple of devices (an `EngineGroup`); the two never share an entry, even for one device."""
+    (one engine) or a tuple of devices (an `EngineGroup`); the two never share an entry, even for one device.
+    Cached engines are always fp32 engines: `objects` is the fp32 matrix (its dtype is part of `content_hash`), and no
+    engine kept at 16 bits (B200_F_OBJECTS_16BIT) is ever built or returned here."""
     key = (content_hash(objects), cosine, device, tc_mode)
     with _CACHE_LOCK:
         eng = _ENGINE_CACHE.get(key)
@@ -131,17 +133,21 @@ class B200TorchRanker(B200Ranker):
     implicit path uses the stored structure; explicit zeros are dropped here to keep the torch semantics.
 
     `devices` (not in the reference): rank on an engine group over these devices (a sequence or "all"); the factors'
-    device is its home device."""
+    device is its home device.
+
+    `keep_16bit` (not in the reference): fp16 / bf16 `objects_factors` stay at 16 bits in the engine, read in place with
+    no fp32 master copy (the ranker keeps the tensor alive); False widens them into an fp32 copy.  Same results."""
 
     def __init__(self, distance, device, subjects_factors, objects_factors, batch_size: int = 128, dtype=None,
-                 devices: tp.Optional[Devices] = None) -> None:
+                 devices: tp.Optional[Devices] = None, keep_16bit: bool = True) -> None:
         dev_index = 0
         dev = str(device)
         if dev.startswith("cuda") and ":" in dev:
             dev_index = int(dev.split(":")[1])
         if hasattr(objects_factors, "detach") and dev.startswith("cuda") and not objects_factors.is_cuda:
             objects_factors = objects_factors.to(device)  # `TorchRanker` scores on `device` (rank_torch.py:135)
-        super().__init__(distance, subjects_factors, objects_factors, device=dev_index if devices is None else devices)
+        super().__init__(distance, subjects_factors, objects_factors, device=dev_index if devices is None else devices,
+                         keep_16bit=keep_16bit)
         self.batch_size = batch_size
 
     def rank(self, subject_ids, k=None, filter_pairs_csr=None, sorted_object_whitelist=None):
@@ -244,18 +250,25 @@ def uninstall() -> None:
     clear_engine_cache()
 
 
-def make_similarity_module(ranker_factory: tp.Optional[tp.Callable[..., tp.Any]] = None, devices: tp.Optional[Devices] = None) -> type:
+def make_similarity_module(
+    ranker_factory: tp.Optional[tp.Callable[..., tp.Any]] = None, devices: tp.Optional[Devices] = None,
+    keep_16bit: tp.Optional[bool] = None,
+) -> type:
     """`similarity_module_type` for SASRec / BERT4Rec / HSTU (rectools/models/nn/transformers/base.py:219, :423): the
     reference's `DistanceSimilarityModule` with `B200TorchRanker` as the scorer of `_recommend_u2i`
     (similarity.py:117-140).  `item_embs` stays on its device (and in its dtype: fp16 / bf16 embeddings are handed to the
     engine as they are); the filter stays a CSR (the reference densifies [batch, n_items] per batch, rank_torch.py:138-144).
     `ranker_factory`: another `TorchRanker`-signature class (the CPU tests plug an oracle-backed stand-in in).
     `devices`: rank on an engine group over these devices (a sequence or "all", passed to the factory as `devices=`);
-    None ranks on the device of `item_embs`."""
+    None ranks on the device of `item_embs`.
+    `keep_16bit`: passed to the factory as `keep_16bit=` (None: the factory's default, which for `B200TorchRanker` keeps
+    fp16 / bf16 `item_embs` at 16 bits in the engine; False widens them into an fp32 copy)."""
     from rectools.models.nn.transformers.similarity import DistanceSimilarityModule  # needs torch only
 
     factory = ranker_factory or B200TorchRanker
     group_kw = {} if devices is None else {"devices": parse_devices(devices)}
+    if keep_16bit is not None:
+        group_kw["keep_16bit"] = bool(keep_16bit)
 
     class B200DistanceSimilarityModule(DistanceSimilarityModule):
         def _recommend_u2i(self, user_embs, item_embs, user_ids, k, sorted_item_ids_to_recommend, ui_csr_for_filter):

@@ -71,6 +71,20 @@ def check_whitelist(whitelist: np.ndarray, n_objects: int) -> None:
         raise ValueError("`sorted_object_whitelist` must be sorted ascending without duplicates")
 
 
+def object_storage_dtype(distance: tp.Any, dtype: tp.Any, keep_16bit: bool) -> int:
+    """Element type (`_lib.DT_*`) the engine keeps the object factors in.  fp16 / bf16 factors stay at 16 bits with
+    `keep_16bit` (B200_F_OBJECTS_16BIT: results are bit for bit those of the widened engine, at half the master copy's
+    HBM), except for EUCLIDEAN: its augmented objects carry a squared-norm column that is no 16-bit value.  Everything
+    else is an fp32 master copy.  `dtype`: a numpy or torch dtype, or its name."""
+    if isinstance(dtype, str) or str(dtype).startswith("torch."):
+        name = str(dtype).replace("torch.", "")
+    else:
+        name = np.dtype(dtype).name
+    if not keep_16bit or _as_distance(distance) == Distance.EUCLIDEAN:
+        return _lib.DT_F32
+    return {"float16": _lib.DT_F16, "bfloat16": _lib.DT_BF16}.get(name, _lib.DT_F32)
+
+
 def prepare_factors(
     distance: Distance, subjects: np.ndarray, objects: np.ndarray
 ) -> tp.Tuple[np.ndarray, np.ndarray, tp.Optional[np.ndarray], tp.Optional[np.ndarray]]:
@@ -86,8 +100,21 @@ def prepare_factors(
     return subjects, objects, norms, dots
 
 
+def _host_objects(objects: np.ndarray, objects_dtype: int) -> np.ndarray:
+    """A host object matrix as the engine reads it: C-contiguous fp32, or fp16 for `objects_dtype` DT_F16."""
+    if objects_dtype == _lib.DT_BF16:
+        raise TypeError("bf16 object factors must be a CUDA tensor (numpy has no bfloat16)")
+    return np.ascontiguousarray(objects, dtype=np.float16 if objects_dtype == _lib.DT_F16 else np.float32)
+
+
+def _create_flags(on_device: bool, keep_16bit: bool) -> int:
+    return (_lib.F_OBJECTS_ON_DEVICE if on_device else 0) | (_lib.F_OBJECTS_16BIT if keep_16bit else 0)
+
+
 class Engine:
-    """Owner of one `b200_rank_engine*` (resident object factors on one GPU)."""
+    """Owner of one `b200_rank_engine*` (resident object factors on one GPU).  `keep_16bit`: fp16 / bf16 objects stay in
+    their own type (B200_F_OBJECTS_16BIT, no fp32 master copy); a device matrix is then read in place and must stay alive
+    and unchanged until `close()`.  Without it, 16-bit objects must be device pointers and are widened to fp32."""
 
     def __init__(
         self,
@@ -99,18 +126,19 @@ class Engine:
         objects_device_ptr: tp.Optional[int] = None,
         shape: tp.Optional[tp.Tuple[int, int]] = None,
         objects_dtype: int = _lib.DT_F32,
+        keep_16bit: bool = False,
     ) -> None:
         self._lib = _lib.load()
         self._h = C.c_void_p()
         if objects_device_ptr is not None:
             assert shape is not None
             n, d = shape
-            ptr, flags = objects_device_ptr, _lib.F_OBJECTS_ON_DEVICE
+            ptr, flags = objects_device_ptr, _create_flags(True, keep_16bit)
             self._keep = None
         else:
-            objects = np.ascontiguousarray(objects, dtype=np.float32)
+            objects = _host_objects(objects, objects_dtype)
             n, d = objects.shape
-            ptr, flags = objects.ctypes.data, 0
+            ptr, flags = objects.ctypes.data, _create_flags(False, keep_16bit)
             self._keep = objects
         _lib.check(
             self._lib.b200_rank_create_ex(
@@ -349,7 +377,8 @@ class EngineGroup(Engine):
     """Owner of one `b200_rank_group*`: an engine per entry of `devices` (duplicates: several engines on one device), each
     holding the whole catalogue, that rank the row slices of every call.  Results are bit for bit those of one `Engine`.
     `devices[0]` is the home device: device pointers (objects, subjects, inputs and outputs of `topk_ptrs`) live there.
-    Threshold sharing, snapshots and id offsets are engine-only."""
+    `keep_16bit` goes to every member (members on other devices read a 16-bit peer copy).  Threshold sharing, snapshots
+    and id offsets are engine-only."""
 
     def __init__(
         self,
@@ -360,6 +389,7 @@ class EngineGroup(Engine):
         objects_device_ptr: tp.Optional[int] = None,
         shape: tp.Optional[tp.Tuple[int, int]] = None,
         objects_dtype: int = _lib.DT_F32,
+        keep_16bit: bool = False,
     ) -> None:
         self._lib = _lib.load()
         self._h = C.c_void_p()
@@ -369,11 +399,11 @@ class EngineGroup(Engine):
         if objects_device_ptr is not None:
             assert shape is not None
             n, d = shape
-            ptr, flags = objects_device_ptr, _lib.F_OBJECTS_ON_DEVICE
+            ptr, flags = objects_device_ptr, _create_flags(True, keep_16bit)
         else:
-            objects = np.ascontiguousarray(objects, dtype=np.float32)
+            objects = _host_objects(objects, objects_dtype)
             n, d = objects.shape
-            ptr, flags = objects.ctypes.data, 0
+            ptr, flags = objects.ctypes.data, _create_flags(False, keep_16bit)
         devs = (C.c_int32 * len(self.devices))(*self.devices)
         _lib.check(
             self._lib.b200_rank_group_create_ex(
@@ -464,12 +494,15 @@ def parse_devices(device: tp.Any) -> tp.Union[int, tp.Tuple[int, ...]]:
     return tuple(int(d) for d in devices)
 
 
-def new_engine(objects: tp.Optional[np.ndarray], cosine: bool, device: tp.Any, tc_mode: str = "auto", **kw: tp.Any) -> Engine:
-    """An `Engine` for an int device, an `EngineGroup` for a sequence of devices or "all" (`parse_devices`)."""
+def new_engine(
+    objects: tp.Optional[np.ndarray], cosine: bool, device: tp.Any, tc_mode: str = "auto", keep_16bit: bool = False, **kw: tp.Any
+) -> Engine:
+    """An `Engine` for an int device, an `EngineGroup` for a sequence of devices or "all" (`parse_devices`).
+    `keep_16bit`: fp16 / bf16 objects stay at 16 bits (B200_F_OBJECTS_16BIT); no effect on fp32 objects."""
     dev = parse_devices(device)
     if isinstance(dev, int):
-        return Engine(objects, cosine=cosine, device=dev, tc_mode=tc_mode, **kw)
-    return EngineGroup(objects, cosine=cosine, devices=dev, tc_mode=tc_mode, **kw)
+        return Engine(objects, cosine=cosine, device=dev, tc_mode=tc_mode, keep_16bit=keep_16bit, **kw)
+    return EngineGroup(objects, cosine=cosine, devices=dev, tc_mode=tc_mode, keep_16bit=keep_16bit, **kw)
 
 
 def rank_object_rows_padded(
@@ -560,6 +593,9 @@ class B200Ranker:
     device : int, CUDA device ordinal; or a sequence of ordinals / "all": an engine group that splits every call's rows
         between one engine per entry (`EngineGroup`, same results)
     tc_mode : "auto" | "fp16" | "bf16" | "off" -- dtype of the tensor-core candidate pass ("off": fp64 kernel only)
+    keep_16bit : fp16 / bf16 CUDA tensors and numpy fp16 object factors stay at 16 bits in the engine, with no fp32
+        master copy (same results; `object_storage_dtype`).  A CUDA tensor is then read in place for the ranker's life.
+        False: the engine widens them into an fp32 copy.
     """
 
     def __init__(
@@ -573,6 +609,7 @@ class B200Ranker:
         tc_mode: str = "auto",
         engine: tp.Optional[Engine] = None,
         subjects_key: tp.Optional[tp.Hashable] = None,
+        keep_16bit: bool = True,
     ) -> None:
         self.distance = _as_distance(distance)
         self._subjects_csr = None
@@ -581,9 +618,18 @@ class B200Ranker:
         if engine is None and self.distance != Distance.EUCLIDEAN and _is_cuda_tensor(objects_factors):
             # embeddings that already live on the GPU (transformer scorers keep `item_embs` on the device,
             # rectools/models/nn/transformers/lightning.py:391, :398): hand the device pointers over, no host round trip
-            self._init_from_device_tensors(subjects_factors, objects_factors, tc_mode, device)
+            self._init_from_device_tensors(subjects_factors, objects_factors, tc_mode, device, keep_16bit)
             return
-        objects = _dense_f32(objects_factors)
+        objects_dtype = _lib.DT_F32
+        if engine is None and isinstance(objects_factors, np.ndarray):
+            objects_dtype = object_storage_dtype(self.distance, objects_factors.dtype, keep_16bit)
+        if objects_dtype == _lib.DT_F16:  # numpy fp16 objects: uploaded as they are
+            objects = _host_objects(objects_factors, _lib.DT_F16)
+            if objects.ndim != 2:
+                raise ValueError("factor matrices must be 2-dimensional")
+        else:
+            objects = _dense_f32(objects_factors)
+        host_kw = {"objects_dtype": objects_dtype, "keep_16bit": objects_dtype == _lib.DT_F16}
         if sparse.issparse(subjects_factors):
             # EASE: the subjects are the user x item interaction CSR (rectools/models/ease.py:134-161).  The reference keeps the
             # matrix sparse and densifies only the requested rows (rank_implicit.py:236, :157-160); here the rows stay sparse
@@ -594,7 +640,7 @@ class B200Ranker:
             self._subjects_csr = csr.astype(np.float32)
             self.n_subjects, self.n_objects = csr.shape[0], objects.shape[0]
             self.subjects_norms = self.subjects_dots = None
-            self.engine = engine or new_engine(objects, cosine=False, device=device, tc_mode=tc_mode)
+            self.engine = engine or new_engine(objects, cosine=False, device=device, tc_mode=tc_mode, **host_kw)
             self._subjects, self._subjects_key = None, None
             self.last_stats = {}
             return
@@ -603,15 +649,18 @@ class B200Ranker:
             raise ValueError("subject and object factors must have the same number of columns")
         self.n_subjects, self.n_objects = subjects.shape[0], objects.shape[0]
         subjects, objects, self.subjects_norms, self.subjects_dots = prepare_factors(self.distance, subjects, objects)
-        self.engine = engine or new_engine(objects, cosine=self.distance == Distance.COSINE, device=device, tc_mode=tc_mode)
+        self.engine = engine or new_engine(objects, cosine=self.distance == Distance.COSINE, device=device, tc_mode=tc_mode, **host_kw)
         self._subjects, self._subjects_key = subjects, subjects_key
         self.engine.set_subjects(subjects, key=subjects_key, owner=self)
         self.last_stats: tp.Dict[str, tp.Any] = {}
 
-    def _init_from_device_tensors(self, subjects_factors: tp.Any, objects_factors: tp.Any, tc_mode: str, device: Devices = 0) -> None:
+    def _init_from_device_tensors(
+        self, subjects_factors: tp.Any, objects_factors: tp.Any, tc_mode: str, device: Devices = 0, keep_16bit: bool = True
+    ) -> None:
         import torch
 
-        # fp16 / bf16 embeddings go to the engine as they are (widened exactly on the device: b200_rank_create_ex)
+        # fp16 / bf16 embeddings go to the engine as they are: kept at 16 bits and read in place (keep_16bit), or widened
+        # exactly into an fp32 copy on the device (b200_rank_create_ex)
         dtypes = {torch.float32: _lib.DT_F32, torch.float16: _lib.DT_F16, torch.bfloat16: _lib.DT_BF16}
         objects = objects_factors.detach()
         if objects.dtype not in dtypes:
@@ -645,6 +694,7 @@ class B200Ranker:
         self.engine = new_engine(
             None, cosine=self.distance == Distance.COSINE, device=home if isinstance(devices, int) else devices, tc_mode=tc_mode,
             objects_device_ptr=objects.data_ptr(), shape=(self.n_objects, int(objects.shape[1])), objects_dtype=dtypes[objects.dtype],
+            keep_16bit=object_storage_dtype(self.distance, objects.dtype, keep_16bit) != _lib.DT_F32,
         )
         self.engine.set_subjects_device(subjects.data_ptr(), self.n_subjects)
         self._subjects = self._subjects_key = None
