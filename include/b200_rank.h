@@ -195,7 +195,10 @@ int b200_rank_create(b200_rank_engine** out, const float* objects, int64_t n_obj
  * With B200_F_OBJECTS_ON_DEVICE (any dtype) create reads the device matrix after all work queued on the device, so
  * the caller's producer stream needs no synchronisation.  The object matrix must not change after create: the row norms,
  * eps and the tensor-core copy are derived from it once.  A device matrix the engine reads in place (fp32, or 16-bit with
- * B200_F_OBJECTS_16BIT) is its master copy: the caller keeps it alive and unchanged until destroy. */
+ * B200_F_OBJECTS_16BIT) is its master copy: the caller keeps it alive and unchanged until destroy.
+ * Every device pointer the engine reads or writes -- the object matrix here, subjects, index arrays, whitelists and
+ * outputs of a call -- need only be aligned to its element type: a view that starts inside an allocation (a tensor
+ * slice) is read in place, with wide loads only where a row happens to start on a 16-byte boundary. */
 int b200_rank_create_ex(b200_rank_engine** out, const void* objects, int32_t dtype, int64_t n_objects, int32_t d,
                         int32_t distance, int32_t device, int32_t tc_mode, int32_t flags);
 int b200_rank_destroy(b200_rank_engine* engine);

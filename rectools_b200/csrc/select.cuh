@@ -306,7 +306,9 @@ __device__ __forceinline__ float exact_score(const SelectParams& p, const float*
     double acc = 0.0;
     const TO* orow = static_cast<const TO*>(p.objects) + (int64_t)id * p.d;
     if constexpr (std::is_same<TO, float>::value) {
-        if ((p.d & 3) == 0) {
+        // 4 elements per load only where the row starts on a 16-byte boundary: a borrowed matrix (a tensor view, a
+        // C-ABI pointer) need only be element-aligned
+        if ((p.d & 3) == 0 && (reinterpret_cast<uintptr_t>(orow) & 15) == 0) {
             const float4* o4 = reinterpret_cast<const float4*>(orow);
             const float4* s4 = reinterpret_cast<const float4*>(sub);
             for (int j = 0; j < (p.d >> 2); ++j) {
