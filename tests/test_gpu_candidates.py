@@ -2,14 +2,14 @@
 
 Every case ranks on the tensor-core path with B200_TC_SNAPSHOT set, checks the captured pass with tests/tc_reference.py
 on every row and list (list contents I1, premise P1 = I2, premise P2 = I3, thresholds I4, the certificate's verdict I5,
-and the exponents / constants the kernel used), and compares the final ids and scores with the exhaustive fp64 oracle.
+and the exponents / constants the kernel used), and holds the final ids and scores to the rounding-interval checker of tests/score_interval.py on every row.
 Each case prints its largest observed fractions of the I2 bounds and its fallback counts."""
 import numpy as np
 import pytest
 from scipy import sparse
 
-from oracle.topk_oracle import implicit_topk, neginf_score
 from tests.helpers import synth_factors, synth_viewed_csr
+from tests.score_interval import check_topk
 from tests.tc_reference import TILE_N, Catalogue, check_snapshot
 
 pytestmark = pytest.mark.gpu
@@ -31,18 +31,9 @@ def _csr(cols_per_row, n_cols):
     return indptr, indices
 
 
-def _oracle(cat, sub32, k, viewed):
-    """Exhaustive fp64 top-k over the call's positions (score desc, id asc), as GLOBAL ids, padded like the engine."""
-    objs = cat.obj64_pos.astype(np.float32)
-    norms = cat.norms[cat.pos2obj] if cat.cosine else None
-    ids, sc = implicit_topk(objs, sub32, k, norms, viewed, accum="f64")
-    valid = sc > np.float32(neginf_score())
-    return np.where(valid, cat.pos2obj[ids] + cat.id_off, -1), sc, valid.sum(axis=1)
-
-
 def _run(eng, lib, monkeypatch, capsys, name, sub32, k, objects, cosine, indptr=None, indices=None, whitelist=None, id_off=0,
          snaps=(1,), bf16=False, flags=None, min_launches=1):
-    """Rank, compare with the oracle, check the snapshot of each requested launch.  Returns the reports and stats."""
+    """Rank, check every row with the score-interval checker, check the snapshot of each requested launch.  Returns the reports and stats."""
     sub32 = np.ascontiguousarray(sub32, np.float32)
     n_rows = len(sub32)
     cat = Catalogue(objects, cosine=cosine, bf16=bf16, whitelist=whitelist, id_off=id_off)
@@ -50,7 +41,6 @@ def _run(eng, lib, monkeypatch, capsys, name, sub32, k, objects, cosine, indptr=
         viewed = cat.viewed_positions(indptr, indices, n_rows)
     else:
         viewed = sparse.csr_matrix((n_rows, cat.n_pos), dtype=np.float32)
-    oid, osc, ocnt = _oracle(cat, sub32, k, viewed)
     reports = []
     for n in snaps:
         monkeypatch.setenv("B200_TC_SNAPSHOT", str(n))
@@ -58,10 +48,8 @@ def _run(eng, lib, monkeypatch, capsys, name, sub32, k, objects, cosine, indptr=
                                 flags=lib.Q_FORCE_TC if flags is None else flags)
         st = dict(eng.last_stats)
         assert st["path"] == 1 and st["n_tc_launches"] >= min_launches, st
-        np.testing.assert_array_equal(cnt, ocnt, err_msg=f"{name} {st}")
-        valid = np.arange(ids.shape[1])[None, :] < cnt[:, None]
-        np.testing.assert_array_equal(np.where(valid, ids, -1), oid, err_msg=f"{name} {st}")
-        np.testing.assert_allclose(sc[valid], osc[valid], rtol=3e-7, atol=1.5e-45, err_msg=name)
+        check_topk((ids, sc, cnt), sub32, objects, k, cosine=cosine, filter_csr=None if indptr is None else (indptr, indices),
+                   whitelist=whitelist, id_offset=id_off, name=f"{name} {st}")
         snap = eng.candidate_snapshot()
         if n > st["n_tc_launches"]:
             assert snap is None
@@ -186,10 +174,7 @@ def test_d_beyond_the_tensor_core_path(lib, d):
         eng.topk(K, subjects=u, indptr=csr.indptr, indices=csr.indices, flags=lib.Q_FORCE_TC)
     ids, sc, cnt = eng.topk(K, subjects=u, indptr=csr.indptr, indices=csr.indices)
     assert eng.last_stats["path"] == 0
-    cat = Catalogue(i, cosine=False, bf16=False)
-    oid, osc, ocnt = _oracle(cat, u, K, cat.viewed_positions(csr.indptr, csr.indices, 200))
-    np.testing.assert_array_equal(ids, oid)
-    np.testing.assert_allclose(sc, osc, rtol=3e-7)
+    check_topk((ids, sc, cnt), u, i, K, filter_csr=csr, name=f"d={d} exhaustive")
     eng.close()
 
 

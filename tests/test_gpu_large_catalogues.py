@@ -5,11 +5,17 @@ are said to fit on one H100.  At config 4 (10M x 128 fp32) the master copy is 5.
 the fp16 tensor-core copy (2.56 GB) passes 2^31 bytes; at config 5 (5M x 256 bf16 kept at 16 bits) the borrowed matrix and
 the tensor-core copy are 2.56 GB each.  `test_gpu_scale.py` stops at 1M objects.
 
-`rank_oracle` widens the whole catalogue to fp64 at once (10 GB at config 4), so the oracle here scores blocks of 1M
-objects and merges a running top-k by (score desc, id asc); `tests/test_large_catalogue_oracle_cpu.py` pins it against
-`rank_oracle` on small inputs.  The oracle's fp64 sums come from BLAS, in another order than the engine's, so a score can
-round to the neighbouring fp32 value (about one in 10^8): ids are compared exactly on the sampled rows up to k = 1025, and
-the k = None rows (10M entries each) allow such one-ulp neighbours to swap.
+Results are held to the rounding-interval checker of `tests/score_interval.py` (blocks of objects, so that no fp64 copy
+of the catalogue is held): every score one of the fp32 values its fp64 sum can round to, no eligible object left out
+ahead of a row's k-th entry, no tolerance and no swapped neighbours, on sampled rows of the largest k of each route.
+Every engine kernel sums a pair's terms in index order, so the smaller k of the same catalogue must be bit-identical
+prefixes of the checked results, on all rows.
+
+64 sampled rows (spread evenly over the 4096) are checked per route.  Each check scores every object of a row, so one
+row is 10M interval checks at config 4 and a 64-row check costs about 90 s of host time; the rows are not special (one
+subject generator, the same filter density), and the routes' row-dependent decisions -- fallback, row-list re-rank --
+are exercised across all rows by the bit-identical prefix comparisons and, at smaller sizes, by
+`tests/test_gpu_score_bits.py` on every row.  256 rows would multiply the file's run time by about four.
 
 Memory: the config-4 engine reports `hbm_bytes` = 8.00 GB after create (master copy, tensor-core copy, norms, staging);
 engines are closed between tests.  Path 3 cuts at least 32 rows per chunk whatever N is (`run_dense_large_k`): at
@@ -20,139 +26,38 @@ import time
 import numpy as np
 import pytest
 
-from oracle.topk_oracle import NEG_SENTINEL, calc_norms, neginf_score
 from tests.helpers import synth_viewed_csr
+from tests.score_interval import check_topk
 from tests.test_gpu_scale import BLOCK, gen_factors
 
 pytestmark = pytest.mark.gpu
 
-BLOCK_OBJECTS = 1 << 20
 N4, D4 = 10_000_000, 128
 N5, D5 = 5_000_000, 256
 N_SUBJECTS = 4096
-NEG_MAX = np.float32(-np.finfo(np.float32).max)
-
-
-# ------------------------------------------------------------------------------------------------ the blocked oracle
-def _order_keys(scores: np.ndarray, ids: np.ndarray) -> np.ndarray:
-    """uint64 keys whose ascending order is (score desc, id asc): the high word inverts the monotone map of the fp32 bit
-    pattern, the low word is the id."""
-    u = np.ascontiguousarray(scores, np.float32).view(np.uint32)
-    mono = np.where(u >> 31, ~u, u | np.uint32(0x80000000)).astype(np.uint32)  # ascending in the score
-    return ((~mono).astype(np.uint64) << np.uint64(32)) | ids.astype(np.uint64)
-
-
-def _from_keys(keys: np.ndarray) -> tuple:
-    ids = (keys & np.uint64(0xFFFFFFFF)).astype(np.int64)
-    inv = ~(keys >> np.uint64(32)).astype(np.uint32)
-    bits = np.where(inv >> 31, inv & np.uint32(0x7FFFFFFF), ~inv).astype(np.uint32)
-    return ids, bits.view(np.float32)
-
-
-def _rows_f32(objects, sel) -> np.ndarray:
-    """Rows `sel` (a slice or ids) of a numpy matrix or a CPU torch tensor (any float type, widened exactly) as fp32."""
-    if hasattr(objects, "float"):
-        import torch
-
-        return objects[sel if isinstance(sel, slice) else torch.from_numpy(sel)].float().numpy()
-    return np.asarray(objects[sel], np.float32)
-
-
-def blocked_oracle(distance, subjects, objects, k, filter_csr=None, whitelist=None, block=BLOCK_OBJECTS, row_block=64):
-    """The engine's answer in padded form (`ec.expected_padded`'s), computed over blocks of `block` positions: fp64 dot
-    rounded once to fp32 (COSINE: / the fp32 object norm), filtered pairs at -FLT_MAX, a running top-k per row merged by
-    (score desc, id asc), then the trailing sentinel strip as counts (slots beyond: id -1 / score -FLT_MAX).
-    `subjects` [n, d] are the batch rows; `filter_csr` [n, >= ids] filters by object id; `whitelist` (sorted) restricts
-    the positions.  Returns (ids int32 [n, k_out], scores fp32, counts int32)."""
-    subjects = np.asarray(subjects, np.float64)
-    n = subjects.shape[0]
-    wl = None if whitelist is None else np.asarray(whitelist, np.int64)
-    n_pos = objects.shape[0] if wl is None else len(wl)
-    k_out = min(n_pos if k is None else int(k), n_pos)
-    run = np.empty((n, 0), np.uint64)
-    for p0 in range(0, n_pos, block):
-        p1 = min(p0 + block, n_pos)
-        ids = np.arange(p0, p1, dtype=np.int64) if wl is None else wl[p0:p1]
-        blk = _rows_f32(objects, slice(p0, p1) if wl is None else ids)
-        blk64 = blk.astype(np.float64)
-        norms = calc_norms(blk, "f64").astype(np.float64) if distance == "cosine" else None
-        parts = []
-        for r0 in range(0, n, row_block):
-            r1 = min(r0 + row_block, n)
-            s = subjects[r0:r1] @ blk64.T
-            if norms is not None:
-                s = s / norms[None, :]
-            s = s.astype(np.float32) + np.float32(0)  # (-0.0 -> +0.0: the sign of an exact zero is not part of the result)
-            if filter_csr is not None:
-                for r in range(r0, r1):
-                    cols = filter_csr.indices[filter_csr.indptr[r] : filter_csr.indptr[r + 1]]
-                    if wl is None:
-                        s[r - r0, cols[(cols >= p0) & (cols < p1)] - p0] = NEG_SENTINEL
-                    else:
-                        s[r - r0, np.isin(ids, cols)] = NEG_SENTINEL
-            keys = _order_keys(s, np.broadcast_to(ids, s.shape))
-            if k_out < keys.shape[1]:
-                keys = np.partition(keys, k_out - 1, axis=1)[:, :k_out]
-            parts.append(np.sort(keys, axis=1))
-        cand = np.concatenate(parts, axis=0)
-        # two sorted runs per row: the stable sort (timsort) merges them
-        run = np.sort(np.concatenate([run, cand], axis=1), axis=1, kind="stable")[:, :k_out]
-    ids, sc = _from_keys(run)
-    valid = sc > np.float32(neginf_score())
-    counts = valid.sum(axis=1).astype(np.int32)
-    assert (valid == (np.arange(k_out)[None, :] < counts[:, None])).all()
-    return np.where(valid, ids, -1).astype(np.int32), np.where(valid, sc, NEG_MAX).astype(np.float32), counts
 
 
 # ------------------------------------------------------------------------------------------------ comparisons
-def _check(got, exp, name, rtol=3e-7):
-    """Exact ids and counts, scores within fp32 rounding of the oracle's."""
+def _same_prefix(got, ref, name):
+    """`got` (k columns) is the first k columns of `ref`, bit for bit, counts included."""
     ids, sc, cnt = got
-    eids, esc, ecnt = exp
-    assert ids.shape == eids.shape, f"{name}: shape {ids.shape} vs {eids.shape}"
-    np.testing.assert_array_equal(cnt, ecnt, err_msg=f"{name}: counts")
-    np.testing.assert_array_equal(ids, eids, err_msg=f"{name}: ids")
-    np.testing.assert_allclose(sc, esc, rtol=rtol, atol=1e-30, err_msg=f"{name}: scores")
-
-
-def _check_full_rows(got, exp, objects_score, name):
-    """k = None rows: counts exact; at every position the two scores agree to one fp32 rounding; where the ids differ,
-    the engine's id scores (recomputed) what the oracle has there, so only near-equal neighbours swapped."""
-    ids, sc, cnt = got
-    eids, esc, ecnt = exp
-    np.testing.assert_array_equal(cnt, ecnt, err_msg=f"{name}: counts")
-    np.testing.assert_allclose(sc, esc, rtol=3e-7, atol=1e-30, err_msg=f"{name}: scores")
-    swapped = 0
-    for r in range(ids.shape[0]):
-        bad = np.nonzero(ids[r] != eids[r])[0]
-        swapped += len(bad)
-        if len(bad):
-            assert (bad < cnt[r]).all(), f"{name}: row {r} differs in its padding"
-            np.testing.assert_allclose(objects_score(r, ids[r, bad]), esc[r, bad], rtol=3e-7, err_msg=f"{name}: row {r} swapped ids")
-    total = int(cnt.sum())
-    print(f"{name}: {swapped} of {total} positions hold a one-rounding neighbour")
-    assert swapped <= max(16, total // 10**6), f"{name}: {swapped} swapped positions"
+    k = ids.shape[1]
+    np.testing.assert_array_equal(cnt, np.minimum(ref[2], k), err_msg=f"{name}: counts")
+    np.testing.assert_array_equal(ids, ref[0][:, :k], err_msg=f"{name}: ids")
+    np.testing.assert_array_equal(sc.view(np.int32), ref[1][:, :k].view(np.int32), err_msg=f"{name}: scores")
 
 
 # ------------------------------------------------------------------------------------------------ config 4
 @pytest.fixture(scope="module")
 def c4():
-    """10M x 128 fp32 objects (bench's generator), 4096 subjects with 100 viewed objects each, 256 sampled rows and
-    their oracle at k = 1025 (every smaller k is its prefix)."""
+    """10M x 128 fp32 objects (bench's generator), 4096 subjects with 100 viewed objects each, 64 sampled rows."""
     t0 = time.time()
     objects = gen_factors(N4, D4, 1)
     subjects = gen_factors(N_SUBJECTS, D4, 0)
     csr = synth_viewed_csr(N_SUBJECTS, N4, 100)
-    rows = np.unique(np.linspace(0, N_SUBJECTS - 1, 256).astype(np.int64))
-    t1 = time.time()
-    exp = blocked_oracle("dot", subjects[rows], objects, 1025, csr[rows])
-    print(f"config 4: catalogue {t1 - t0:.1f} s, oracle of {len(rows)} rows at k = 1025 {time.time() - t1:.1f} s")
-    yield objects, subjects, csr, rows, exp
-
-
-def _prefix(exp, k, rows=slice(None)):
-    ids, sc, cnt = exp
-    return ids[rows, :k], sc[rows, :k], np.minimum(cnt[rows], k)
+    rows = np.unique(np.linspace(0, N_SUBJECTS - 1, 64).astype(np.int64))
+    print(f"config 4: catalogue {time.time() - t0:.1f} s")
+    yield objects, subjects, csr, rows
 
 
 @pytest.fixture
@@ -167,44 +72,48 @@ def c4_engine(c4):
 
 
 def test_c4_tensor_core_routes(lib_consts, c4, c4_engine):
-    """k = 10 (FORCE_TC), 100 (wide) and 1000 (wide, k > 128) over all 4096 subjects; 256 sampled rows against the
-    oracle."""
-    objects, subjects, csr, rows, exp = c4
+    """k = 10 (FORCE_TC), 100 (wide) and 1000 (wide, k > 128) over all 4096 subjects: k = 1000 on the sampled rows against
+    the score intervals, k = 10 and 100 its bit-identical prefixes on every row."""
+    objects, subjects, csr, rows = c4
     eng = c4_engine
+    res = {}
     for k, flags, wide in ((10, lib_consts.Q_FORCE_TC, 0), (100, 0, 1), (1000, 0, 1)):
         t0 = time.time()
-        got = eng.topk(k, subjects=subjects, indptr=csr.indptr, indices=csr.indices, flags=flags)
+        res[k] = eng.topk(k, subjects=subjects, indptr=csr.indptr, indices=csr.indices, flags=flags)
         st = eng.last_stats
         print(f"config 4 k={k}: path {st['path']} wide {st['wide']} n_fallback_rows {st['n_fallback_rows']} "
               f"n_exact_rows {st.get('n_exact_rows')} ({time.time() - t0:.1f} s)")
         assert (st["path"], st["wide"]) == (1, wide), st
         assert st["n_fallback_rows"] <= N_SUBJECTS // 2, st
-        assert (got[2] == k).all()
-        _check(tuple(a[rows] for a in got), _prefix(exp, k), f"config 4 k={k}")
+        assert (res[k][2] == k).all()
+    t0 = time.time()
+    check_topk(tuple(a[rows] for a in res[1000]), subjects[rows], objects, 1000, filter_csr=csr[rows], name="config 4 k=1000")
+    print(f"config 4 check of {len(rows)} rows: {time.time() - t0:.1f} s")
+    for k in (10, 100):
+        _same_prefix(res[k], res[1000], f"config 4 k={k} against k=1000")
 
 
 def test_c4_exhaustive_and_radix_routes(lib_consts, c4, c4_engine):
-    """64 rows with FORCE_EXACT at k = 10, 64 rows on path 3 at k = 1025, 8 rows at k = None."""
-    objects, subjects, csr, rows, exp = c4
+    """The sampled rows on path 3 at k = 1025 against the score intervals, FORCE_EXACT at k = 10 its prefix; 8 rows at
+    k = None (10M entries each) against the score intervals."""
+    objects, subjects, csr, rows = c4
     eng = c4_engine
-    r64 = np.arange(0, len(rows), len(rows) // 64)[:64]
-    sids = rows[r64]
-    f = csr[sids]
+    f = csr[rows]
+    res = {}
     for k, flags, path in ((10, lib_consts.Q_FORCE_EXACT, 0), (1025, 0, 3)):
-        got = eng.topk(k, subjects=subjects[sids], indptr=f.indptr, indices=f.indices, flags=flags)
+        res[k] = eng.topk(k, subjects=subjects[rows], indptr=f.indptr, indices=f.indices, flags=flags)
         assert eng.last_stats["path"] == path, eng.last_stats
-        _check(got, _prefix(exp, k, r64), f"config 4 path {path} k={k}")
-    s8 = rows[r64[:8]]
+    check_topk(res[1025], subjects[rows], objects, 1025, filter_csr=f, name="config 4 path 3 k=1025")
+    _same_prefix(res[10], res[1025], "config 4 path 0 k=10 against path 3 k=1025")
+    s8 = rows[:8]
     f8 = csr[s8]
     t0 = time.time()
     got = eng.topk(N4, subjects=subjects[s8], indptr=f8.indptr, indices=f8.indices)
     assert eng.last_stats["path"] == 3, eng.last_stats
     print(f"config 4 k=None, 8 rows: {time.time() - t0:.1f} s")
     t0 = time.time()
-    full = blocked_oracle("dot", subjects[s8], objects, None, f8)
-    print(f"config 4 k=None oracle: {time.time() - t0:.1f} s")
-    sub64 = subjects[s8].astype(np.float64)
-    _check_full_rows(got, full, lambda r, ids: (objects[ids].astype(np.float64) @ sub64[r]).astype(np.float32), "config 4 k=None")
+    check_topk(got, subjects[s8], objects, None, filter_csr=f8, name="config 4 k=None")
+    print(f"config 4 k=None check: {time.time() - t0:.1f} s")
 
 
 # ------------------------------------------------------------------------------------------------ config 5
@@ -250,13 +159,13 @@ def lib_consts():
 
 def test_c5_bf16_kept_and_widened(lib_consts, torch, c5):
     """k = 20 over all 4096 rows on the engine that keeps the bf16 matrix at 16 bits (read in place) and on the engine
-    that widens it: bit-identical; 256 rows against the oracle; one call on a 16-bit engine over the matrix at element
-    offset 1 (the element-wise re-score at size)."""
+    that widens it: bit-identical; 64 rows against the score intervals; one call on a 16-bit engine over the matrix at
+    element offset 1 (the element-wise re-score at size), bit-identical on those rows."""
     from rectools_b200 import Engine
 
     items, host, subjects, csr = c5
     kw = dict(objects_device_ptr=items.data_ptr(), shape=(N5, D5), objects_dtype=lib_consts.DT_BF16)
-    rows = np.unique(np.linspace(0, N_SUBJECTS - 1, 256).astype(np.int64))
+    rows = np.unique(np.linspace(0, N_SUBJECTS - 1, 64).astype(np.int64))
     call = dict(subjects=subjects, indptr=csr.indptr, indices=csr.indices)
     kept = Engine(None, cosine=False, keep_16bit=True, **kw)
     try:
@@ -278,9 +187,8 @@ def test_c5_bf16_kept_and_widened(lib_consts, torch, c5):
         np.testing.assert_array_equal(a.view(np.int32) if a.dtype == np.float32 else a,
                                       b.view(np.int32) if b.dtype == np.float32 else b, err_msg=f"config 5 kept vs widened: {what}")
     t0 = time.time()
-    exp = blocked_oracle("dot", subjects[rows], host, 20, csr[rows])
-    print(f"config 5 oracle of {len(rows)} rows: {time.time() - t0:.1f} s")
-    _check(tuple(a[rows] for a in got), exp, "config 5 k=20")
+    check_topk(tuple(a[rows] for a in got), subjects[rows], host, 20, filter_csr=csr[rows], name="config 5 k=20")
+    print(f"config 5 check of {len(rows)} rows: {time.time() - t0:.1f} s")
     # the same matrix one element into a fresh allocation: rows start 2 bytes past 16-byte boundaries
     flat = items.view(-1)
     moved_buf = torch.empty((flat.numel() + 8,), dtype=torch.bfloat16, device=items.device)
@@ -291,11 +199,10 @@ def test_c5_bf16_kept_and_widened(lib_consts, torch, c5):
     odd = Engine(None, cosine=False, keep_16bit=True, objects_device_ptr=moved.data_ptr(), shape=(N5, D5),
                  objects_dtype=lib_consts.DT_BF16)
     try:
-        sub = rows[:64]
-        f = csr[sub]
+        f = csr[rows]
         for k, flags in ((20, 0), (20, lib_consts.Q_FORCE_EXACT)):
-            o = odd.topk(k, subjects=subjects[sub], indptr=f.indptr, indices=f.indices, flags=flags)
-            _check(o, _prefix(exp, k, slice(0, 64)), f"config 5 at offset 1 flags={flags}")
+            o = odd.topk(k, subjects=subjects[rows], indptr=f.indptr, indices=f.indices, flags=flags)
+            _same_prefix(o, tuple(a[rows] for a in got), f"config 5 at offset 1 flags={flags}")
     finally:
         odd.close()
         del moved, moved_buf

@@ -1,4 +1,4 @@
-"""CPU: the blocked fp64 oracle of `test_gpu_large_catalogues.py` against `rank_oracle` and `ec.expected_padded`.
+"""CPU: the blocked fp64 oracle of `tests/blocked_oracle.py` against `rank_oracle` and `ec.expected_padded`.
 
 Integer-valued catalogues (tests/exact_cases.py) make every score exact and tie tens of objects on one value, so ties
 straddle every block edge; blocks of 7, 64 and 1000 objects cut the catalogue at many places, with filters (empty rows,
@@ -8,7 +8,9 @@ import pytest
 
 from oracle.topk_oracle import rank_oracle
 from tests import exact_cases as ec
-from tests.test_gpu_large_catalogues import _from_keys, _order_keys, blocked_oracle
+from tests.blocked_oracle import blocked_oracle
+from tests.score_interval import from_keys as _from_keys
+from tests.score_interval import order_keys as _order_keys
 
 N_OBJ, D, N_ROWS = 3000, 6, 40
 
