@@ -146,7 +146,8 @@ typedef struct b200_rank_stats {
                               * scores + streaming selection), 3 = k > 128 without the tensor-core path (k > 1024, k = None, a
                               * problem below the tiny-problem size, B200_Q_FORCE_EXACT, B200_WIDE=0, or an expected candidate count
                               * above half the catalogue): exhaustive scores materialised once + selection passes, 4 = stored
-                              * rows (object_rows): one radix-select launch per row chunk over the rows in place */
+                              * rows (object_rows): one radix-select launch per row chunk over the rows in place, 5 = candidate
+                              * sets (b200_rank_topk_candidates): ms_main = scoring, ms_select = selection */
     int32_t tc_dtype;        /* B200_TC_FP16 / B200_TC_BF16 when path == 1 */
     int32_t k_out;           /* columns of the output arrays */
     int32_t k_cand;          /* candidates kept per row and item split by the tensor-core pass */
@@ -210,6 +211,28 @@ int b200_rank_set_subjects(b200_rank_engine* engine, const float* subjects, int6
 int b200_rank_set_id_offset(b200_rank_engine* engine, int64_t offset);
 int b200_rank_topk(b200_rank_engine* engine, const b200_rank_query* query, b200_rank_stats* stats /* nullable */);
 int b200_rank_get_info(b200_rank_engine* engine, b200_rank_info* info);
+
+/* Candidate sets (stats.path = 5): batch row r is ranked against its own allow-list, the object ids
+ * cand_indices[cand_indptr[r] .. cand_indptr[r+1]) (host arrays; ids in [0, n_objects), strictly ascending within a row),
+ * minus the row's filter_pairs_csr entries.  Scores are the result definition above, computed by the same fp64 kernel
+ * code as path 1's re-score, so a pair's score bits do not depend on the route; order (score desc, id asc), -inf and NaN
+ * never returned.  Outputs as for b200_rank_topk: [n_rows, k_out] with k_out = min(k, n_objects), unfilled slots
+ * -1 / -FLT_MAX, out_counts = the kept count.  Subjects: `subjects` (with or without subject_ids), or subject_ids over
+ * resident subjects uploaded from the host.  COSINE divides by the stored object norm, as the re-score does.
+ * Refused, with every output untouched:
+ *   B200_E_INVALID      cand_indptr NULL or not monotone, candidate ids out of range or not strictly ascending in a row,
+ *                       and every argument check of b200_rank_topk;
+ *   B200_E_UNSUPPORTED  B200_Q_INPUTS_ON_DEVICE, B200_Q_OUTPUTS_ON_DEVICE, resident subjects set from a device pointer,
+ *                       sub_* and object_rows, a global whitelist (intersect it into the lists), B200_Q_SHARED_THRESHOLDS,
+ *                       B200_Q_FORCE_TC, a non-zero id offset, d > 49152;
+ *   B200_E_NOMEM        a row whose scores (4 B per candidate), sort scratch (16 B per candidate when k_out > 12288) and
+ *                       outputs (8 B x k_out) alone exceed a row chunk's 1 GiB.
+ * B200_Q_FORCE_EXACT is accepted and changes nothing.  Rows are ranked in chunks of whole rows within that 1 GiB
+ * (B200_CHUNK_ROWS=n caps a chunk's rows). */
+int b200_rank_topk_candidates(b200_rank_engine* engine, const b200_rank_query* query,
+                              const int64_t* cand_indptr,  /* [n_rows + 1] */
+                              const int32_t* cand_indices, /* object ids, strictly ascending within a row */
+                              b200_rank_stats* stats /* nullable */);
 
 /* Merge `n_lists` per-shard results (device pointers, each [n_rows, k] / [n_rows], list l at base + l * stride) into
  * the global top-k ordered by (score desc, id asc).  Runs on `stream` of `device`. */

@@ -27,6 +27,7 @@
 #include "sparse.cuh"
 #include "large_k_select.cuh"
 #include "row_select.cuh"
+#include "cand_select.cuh"
 #include "fused_topk.cuh"
 
 namespace {
@@ -411,6 +412,7 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
         // the largest launch of any call (k_out >= LK_SMEM_PAIRS); a fixed maximum: the attribute is shared by every engine
         // on the device, and smaller launches stay within it
         CK(cudaFuncSetAttribute(large_k_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lk_smem_bytes(LK_SMEM_PAIRS)));
+        CK(cudaFuncSetAttribute(cand_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lk_smem_bytes(LK_SMEM_PAIRS)));
     } catch (const CudaError& ce) {
         int rc = fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_create: %s failed at line %d: %s",
                       ce.what, ce.line, cudaGetErrorString(ce.e));
@@ -1319,6 +1321,87 @@ void rerank_failures(Call& c, cudaStream_t cs) {
     c.S.d2h_bytes += (int64_t)(row_bytes * n_fb);
 }
 
+// Path 5: rows [r0, r1) of a candidate-set call, staged, scored, selected and copied back on the engine stream.  The
+// chunk's candidate and filter row pointers are rebased to its first entry; the buffers of the other paths' staging are
+// reused (sp_indptr / sp_indices: candidates, sp_scores: their scores, indptr / indices: the filter, sub32 / rowmap: the
+// subjects, out_*: the chunk's outputs).
+void run_candidates(Call& c, const int64_t* cand_indptr, const int32_t* cand_indices, int64_t r0, int64_t r1,
+                    std::vector<int64_t>& tmp) {
+    b200_rank_engine* E = c.E;
+    const b200_rank_query* q = c.q;
+    cudaStream_t st = c.st;
+    const int64_t nr = r1 - r0, k_out = c.k_out;
+    size_t h2d = 0;
+    auto copy = [&](void* dst, const void* src, size_t bytes) {
+        if (bytes) CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st));
+        h2d += bytes;
+    };
+    auto rebased = [&](const int64_t* indptr) {
+        tmp.resize(nr + 1);
+        for (int64_t i = 0; i <= nr; ++i) tmp[i] = indptr[r0 + i] - indptr[r0];
+        return tmp.data();
+    };
+    CandParams cp{};
+    const int64_t c0 = cand_indptr[r0], nc = cand_indptr[r1] - c0;
+    int64_t max_len = 0;
+    for (int64_t r = r0; r < r1; ++r) max_len = std::max(max_len, cand_indptr[r + 1] - cand_indptr[r]);
+    copy(E->sp_indptr.p, rebased(cand_indptr), sizeof(int64_t) * (nr + 1));
+    copy(E->sp_indices.p, cand_indices + c0, sizeof(int32_t) * nc);
+    cp.c_indptr = E->sp_indptr.as<int64_t>();
+    cp.c_indices = E->sp_indices.as<int32_t>();
+    CK(cudaStreamSynchronize(st));  // tmp is reused below
+    if (q->csr_indptr && q->csr_indptr[q->n_rows] > q->csr_indptr[0]) {
+        const int64_t f0 = q->csr_indptr[r0], nf = q->csr_indptr[r1] - f0;
+        copy(E->indptr.p, rebased(q->csr_indptr), sizeof(int64_t) * (nr + 1));
+        copy(E->indices.p, q->csr_indices + f0, sizeof(int32_t) * nf);
+        cp.f_indptr = E->indptr.as<int64_t>();
+        cp.f_indices = E->indices.as<int32_t>();
+    }
+    if (q->subject_ids) {
+        copy(E->rowmap.p, q->subject_ids + r0, sizeof(int64_t) * nr);
+        cp.row_map = E->rowmap.as<int64_t>();
+        cp.subjects = c.sub32;  // the whole explicit matrix (staged once) or the resident one
+    } else {
+        copy(E->sub32.p, q->subjects + r0 * c.d, sizeof(float) * nr * c.d);
+        cp.subjects = E->sub32.as<float>();
+    }
+    c.S.h2d_bytes += (int64_t)h2d;
+    cp.sp.objects = E->obj_ptr;
+    cp.sp.d = c.d;
+    cp.sp.obj_norms = c.norms();
+    cp.scores = E->sp_scores.as<float>();
+    cp.n_rows = nr;
+    cp.k_out = (int32_t)k_out;
+    cp.smem_pairs = (int32_t)std::min<int64_t>(k_out, LK_SMEM_PAIRS);
+    cp.scratch = k_out > LK_SMEM_PAIRS ? E->lk_scratch.as<uint32_t>() : nullptr;
+    cp.out_ids = E->out_ids.as<int32_t>();
+    cp.out_scores = E->out_scores.as<float>();
+    cp.out_counts = E->out_counts.as<int32_t>();
+    if (max_len > 0) {
+        const unsigned segs = (unsigned)std::min<int64_t>(65535, (max_len + CS_SEG - 1) / CS_SEG);
+        const size_t smem = sizeof(float) * (size_t)c.d;
+        c.time_begin(0);
+        with_obj_type(E, [&](auto t) {
+            using TO = typename decltype(t)::type;
+            if (smem > 48 * 1024) CK(cudaFuncSetAttribute(cand_score_kernel<TO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            cand_score_kernel<TO><<<dim3((unsigned)nr, segs), CS_THREADS, smem, st>>>(cp);
+        });
+        CK(cudaGetLastError());
+        c.time_end();
+        c.S.n_launches++;
+    }
+    c.time_begin(1);
+    cand_select_kernel<<<(unsigned)nr, LK_THREADS, lk_smem_bytes((int)k_out), st>>>(cp);
+    CK(cudaGetLastError());
+    c.time_end();
+    c.S.n_launches++;
+    CK(cudaMemcpyAsync(q->out_ids + r0 * k_out, cp.out_ids, sizeof(int32_t) * nr * k_out, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(q->out_scores + r0 * k_out, cp.out_scores, sizeof(float) * nr * k_out, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(q->out_counts + r0, cp.out_counts, sizeof(int32_t) * nr, cudaMemcpyDeviceToHost, st));
+    c.S.d2h_bytes += nr * k_out * 8 + nr * 4;
+    CK(cudaStreamSynchronize(st));  // the next chunk reuses every buffer
+}
+
 }  // namespace
 
 int b200_check_query(const b200_rank_engine* E, const b200_rank_query* q, int32_t* k_out) {
@@ -1583,6 +1666,105 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
     } catch (const CudaError& ce) {
         return fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_topk: %s failed at line %d: %s", ce.what,
                     ce.line, cudaGetErrorString(ce.e));
+    }
+    if (stats) *stats = c.S;
+    return B200_OK;
+}
+
+int b200_rank_topk_candidates(b200_rank_engine* E, const b200_rank_query* q, const int64_t* cand_indptr, const int32_t* cand_indices,
+                              b200_rank_stats* stats) {
+    if (!E || !q) return fail(B200_E_INVALID, "b200_rank_topk_candidates: NULL argument");
+    std::lock_guard<std::mutex> lock(E->mu);
+    E->snap.valid = 0;
+    Call c{};
+    c.E = E;
+    c.q = q;
+    memset(&c.S, 0, sizeof(c.S));
+    c.n_rows = q->n_rows;
+    c.n_pos = E->n_obj;
+    c.d = E->d;
+    c.hooks = read_hooks();
+    CandShape shape;
+    shape.n_rows = q->n_rows;
+    shape.n_objects = E->n_obj;
+    shape.k = q->k;
+    shape.d = E->d;
+    shape.flags = q->flags;
+    shape.whitelist = q->whitelist != nullptr;
+    shape.sparse = q->sub_indptr || q->sub_indices || q->sub_data;
+    shape.rows = q->object_rows != nullptr;
+    shape.res_device = !q->subjects && E->sub_res_on_device;
+    shape.id_offset = E->id_offset != 0;
+    // the path's own refusals first (a query this path never takes is refused as such), then b200_rank_topk's checks
+    const CandPlan P = plan_candidates(shape, cand_indptr, c.hooks);
+    if (P.error != B200_OK) return fail(P.error, "%s", P.message.c_str());
+    if (const int rc = validate_query(E, q)) return rc;
+    c.S.k_out = c.k_out = P.k_out;
+    c.S.path = (int)Path::CANDIDATES;
+    if (c.n_rows == 0 || c.k_out <= 0) {
+        if (stats) *stats = c.S;
+        return B200_OK;
+    }
+    std::string why;
+    if (check_candidate_ids(cand_indptr, cand_indices, c.n_rows, E->n_obj, why) != B200_OK) return fail(B200_E_INVALID, "%s", why.c_str());
+    const int64_t f_nnz = q->csr_indptr ? q->csr_indptr[c.n_rows] - q->csr_indptr[0] : 0;
+    if (q->csr_indptr) {
+        if (q->csr_indptr[0] < 0) return fail(B200_E_INVALID, "b200_rank_topk_candidates: csr_indptr[0] < 0");
+        for (int64_t r = 0; r < c.n_rows; ++r)
+            if (q->csr_indptr[r + 1] < q->csr_indptr[r])
+                return fail(B200_E_INVALID, "b200_rank_topk_candidates: csr_indptr is not monotone at row %lld", (long long)r);
+    }
+    if (f_nnz > 0 && !q->csr_indices) return fail(B200_E_INVALID, "b200_rank_topk_candidates: csr_indices is NULL");
+    const int64_t n_sub = q->subjects ? q->n_subjects_total : E->n_sub_res;
+    if (q->subject_ids)
+        for (int64_t r = 0; r < c.n_rows; ++r)
+            if (q->subject_ids[r] < 0 || q->subject_ids[r] >= n_sub)
+                return fail(B200_E_INVALID, "b200_rank_topk_candidates: subject_ids[%lld] = %lld is out of range (%lld subjects)", (long long)r,
+                            (long long)q->subject_ids[r], (long long)n_sub);
+    try {
+        CK(cudaSetDevice(E->device));
+        c.st = E->st;
+        CK(cudaEventRecord(E->ev_begin, c.st));
+        int64_t max_f = 0;
+        if (f_nnz > 0)
+            for (int64_t ci = 0; ci < P.n_chunks(); ++ci)
+                max_f = std::max(max_f, q->csr_indptr[P.bounds[ci + 1]] - q->csr_indptr[P.bounds[ci]]);
+        const int64_t rows = P.max_chunk_rows, cands = P.max_chunk_cands;
+        E->sp_indptr.ensure(sizeof(int64_t) * (rows + 1));
+        E->sp_indices.ensure(std::max<size_t>(sizeof(int32_t) * cands, 16));
+        E->sp_scores.ensure(std::max<size_t>(sizeof(float) * cands, 16));
+        if (c.k_out > LK_SMEM_PAIRS) E->lk_scratch.ensure(std::max<size_t>((size_t)16 * cands, 16));
+        if (f_nnz > 0) {
+            E->indptr.ensure(sizeof(int64_t) * (rows + 1));
+            E->indices.ensure(std::max<size_t>(sizeof(int32_t) * max_f, 16));
+        }
+        if (q->subject_ids) {
+            E->rowmap.ensure(sizeof(int64_t) * rows);
+            if (q->subjects) {  // an explicit matrix indexed by subject_ids: staged whole, once
+                E->sub32.ensure(std::max<size_t>(sizeof(float) * n_sub * c.d, 16));
+                CK(cudaMemcpyAsync(E->sub32.p, q->subjects, sizeof(float) * n_sub * c.d, cudaMemcpyHostToDevice, c.st));
+                c.S.h2d_bytes += (int64_t)(sizeof(float) * n_sub * c.d);
+                c.sub32 = E->sub32.as<float>();
+            } else {
+                c.sub32 = E->sub32_res_ptr;
+            }
+        } else {
+            E->sub32.ensure(std::max<size_t>(sizeof(float) * rows * c.d, 16));
+        }
+        E->out_ids.ensure(sizeof(int32_t) * rows * c.k_out);
+        E->out_scores.ensure(sizeof(float) * rows * c.k_out);
+        E->out_counts.ensure(sizeof(int32_t) * rows);
+        std::vector<int64_t> tmp;
+        for (int64_t ci = 0; ci < P.n_chunks(); ++ci) run_candidates(c, cand_indptr, cand_indices, P.bounds[ci], P.bounds[ci + 1], tmp);
+        c.S.n_chunks = (int32_t)P.n_chunks();
+        CK(cudaEventRecord(E->ev_end, c.st));
+        CK(cudaStreamSynchronize(c.st));
+        CK(cudaEventElapsedTime(&c.S.ms_total, E->ev_begin, E->ev_end));
+        c.collect_times();
+        c.S.n_tc_launches = 0;  // (collect_times counts the scoring launches there)
+    } catch (const CudaError& ce) {
+        return fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_topk_candidates: %s failed at line %d: %s",
+                    ce.what, ce.line, cudaGetErrorString(ce.e));
     }
     if (stats) *stats = c.S;
     return B200_OK;

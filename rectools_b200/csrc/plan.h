@@ -9,6 +9,7 @@
 #include <cstdlib>
 #include <optional>
 #include <string>
+#include <vector>
 
 #include "../../include/b200_rank.h"
 #include "sizes.h"
@@ -108,7 +109,7 @@ struct CallShape {
     bool id_offset = false;      // the engine has a non-zero id offset
 };
 
-enum class Path { EXACT = 0, TC = 1, SPARSE = 2, DENSE_LARGE_K = 3, ROWS = 4 };  // = b200_rank_stats::path
+enum class Path { EXACT = 0, TC = 1, SPARSE = 2, DENSE_LARGE_K = 3, ROWS = 4, CANDIDATES = 5 };  // = b200_rank_stats::path
 
 // How the tensor-core path ranks the rows of the main pass.
 enum class TcMode {
@@ -267,6 +268,117 @@ inline CallPlan plan_call(const CallShape& s, const Hooks& h) {
     }
     p.n_chunks = (s.n_rows + p.chunk - 1) / p.chunk;
     return p;
+}
+
+// ---- path 5: candidate sets (b200_rank_topk_candidates).  Row r is scored against its own ascending object ids
+// cand_indices[cand_indptr[r] .. cand_indptr[r+1]): cand_score_kernel writes one fp32 score per candidate into a ragged
+// buffer, cand_select_kernel selects from it.  A row chunk holds, per row, its 4 B scores, 16 B of sort scratch per
+// candidate when k_out > LK_SMEM_PAIRS (a row sorts at most |C_r| survivors; the scratch is addressed by candidate) and its
+// 8 B x k_out of device outputs -- within SELECT_CHUNK_BYTES, the 1 GiB rule of paths 2-4.
+struct CandShape {
+    int64_t n_rows = 0;
+    int64_t n_objects = 0;
+    int64_t k = 0;           // requested k
+    int d = 0;
+    int32_t flags = 0;       // B200_Q_*
+    bool whitelist = false;  // query.whitelist given
+    bool sparse = false;     // query.sub_* given
+    bool rows = false;       // query.object_rows given
+    bool res_device = false; // the batch reads resident subjects that live in device memory
+    bool id_offset = false;  // the engine has a non-zero id offset
+};
+
+// Largest subject row cand_score_kernel stages in shared memory (fp32 elements).
+constexpr int64_t CAND_MAX_D = 48 * 1024;
+
+inline int64_t cand_row_bytes(int64_t len, int64_t k_out) {
+    return 4 * len + (k_out > LK_SMEM_PAIRS ? 16 * len : 0) + 8 * k_out;
+}
+
+struct CandPlan {
+    int k_out = 0;
+    std::vector<int64_t> bounds;  // chunk c = rows [bounds[c], bounds[c + 1])
+    int64_t max_chunk_cands = 0;  // candidates of the largest chunk (score buffer, sort scratch)
+    int64_t max_chunk_rows = 0;
+    int error = B200_OK;
+    std::string message;
+    int64_t n_chunks() const { return bounds.empty() ? 0 : (int64_t)bounds.size() - 1; }
+};
+
+// The refusals, the candidate-row-pointer check and the row chunks of one call.  `indptr` (host, [n_rows + 1]) is read
+// only after the refusals.  Chunks take whole rows, in order, while their bytes stay within `budget` and their rows within
+// B200_CHUNK_ROWS when it is set; a row that alone exceeds the budget is refused with B200_E_NOMEM.
+inline CandPlan plan_candidates(const CandShape& s, const int64_t* indptr, const Hooks& h, int64_t budget = SELECT_CHUNK_BYTES) {
+    CandPlan p;
+    p.k_out = (int)std::min<int64_t>(s.k, s.n_objects);
+    auto refuse = [&](int code, const std::string& why) {
+        p.error = code;
+        p.message = "b200_rank_topk_candidates: " + why;
+        return p;
+    };
+    if (s.flags & (B200_Q_INPUTS_ON_DEVICE | B200_Q_OUTPUTS_ON_DEVICE))
+        return refuse(B200_E_UNSUPPORTED, "candidate sets take host inputs and outputs only");
+    if (s.res_device) return refuse(B200_E_UNSUPPORTED, "resident subjects in device memory are not read here");
+    if (s.sparse) return refuse(B200_E_UNSUPPORTED, "sparse subjects (sub_*) are not ranked against candidate sets");
+    if (s.rows) return refuse(B200_E_UNSUPPORTED, "stored rows (object_rows) are not ranked against candidate sets");
+    if (s.whitelist) return refuse(B200_E_UNSUPPORTED, "a global whitelist is not taken: intersect it into the candidate lists");
+    if (s.flags & B200_Q_SHARED_THRESHOLDS) return refuse(B200_E_UNSUPPORTED, "B200_Q_SHARED_THRESHOLDS has no thresholds to share here");
+    if (s.flags & B200_Q_FORCE_TC) return refuse(B200_E_UNSUPPORTED, "no tensor-core pass scores candidate sets (B200_Q_FORCE_TC)");
+    if (s.id_offset) return refuse(B200_E_UNSUPPORTED, "engines with an id offset hold one shard of the catalogue");
+    if (s.d > CAND_MAX_D) return refuse(B200_E_UNSUPPORTED, "d = " + std::to_string(s.d) + " exceeds the staged subject row's limit");
+    if (s.n_rows == 0 || p.k_out <= 0) return p;  // nothing to rank
+    if (!indptr) return refuse(B200_E_INVALID, "cand_indptr is NULL");
+    if (indptr[0] < 0) return refuse(B200_E_INVALID, "cand_indptr[0] < 0");
+    for (int64_t r = 0; r < s.n_rows; ++r)
+        if (indptr[r + 1] < indptr[r])
+            return refuse(B200_E_INVALID, "cand_indptr is not monotone at row " + std::to_string(r));
+    const int64_t max_rows = h.chunk_rows > 0 ? h.chunk_rows : s.n_rows;
+    p.bounds.push_back(0);
+    int64_t bytes = 0, cands = 0, rows = 0;
+    for (int64_t r = 0; r < s.n_rows; ++r) {
+        const int64_t len = indptr[r + 1] - indptr[r], b = cand_row_bytes(len, p.k_out);
+        if (b > budget)
+            return refuse(B200_E_NOMEM, "row " + std::to_string(r) + " (" + std::to_string(len) + " candidates, k_out = " +
+                                            std::to_string(p.k_out) + ") needs " + std::to_string(b) + " bytes, more than a chunk's " +
+                                            std::to_string(budget));
+        if (rows > 0 && (bytes + b > budget || rows == max_rows)) {
+            p.bounds.push_back(r);
+            p.max_chunk_cands = std::max(p.max_chunk_cands, cands);
+            p.max_chunk_rows = std::max(p.max_chunk_rows, rows);
+            bytes = cands = rows = 0;
+        }
+        bytes += b;
+        cands += len;
+        ++rows;
+    }
+    p.bounds.push_back(s.n_rows);
+    p.max_chunk_cands = std::max(p.max_chunk_cands, cands);
+    p.max_chunk_rows = std::max(p.max_chunk_rows, rows);
+    return p;
+}
+
+// The candidate ids of rows [0, n_rows): in [0, n_objects) and strictly ascending within a row.  B200_OK, or
+// B200_E_INVALID with the first offending row in `message`.
+inline int check_candidate_ids(const int64_t* indptr, const int32_t* indices, int64_t n_rows, int64_t n_objects, std::string& message) {
+    if (indptr[n_rows] > indptr[0] && !indices) {
+        message = "b200_rank_topk_candidates: cand_indices is NULL";
+        return B200_E_INVALID;
+    }
+    for (int64_t r = 0; r < n_rows; ++r) {
+        for (int64_t e = indptr[r]; e < indptr[r + 1]; ++e) {
+            const int32_t id = indices[e];
+            if (id < 0 || id >= n_objects) {
+                message = "b200_rank_topk_candidates: row " + std::to_string(r) + ": candidate " + std::to_string(id) +
+                          " is not an object of this engine (n_objects = " + std::to_string(n_objects) + ")";
+                return B200_E_INVALID;
+            }
+            if (e > indptr[r] && id <= indices[e - 1]) {
+                message = "b200_rank_topk_candidates: row " + std::to_string(r) + ": candidate ids are not strictly ascending";
+                return B200_E_INVALID;
+            }
+        }
+    }
+    return B200_OK;
 }
 
 }  // namespace b200

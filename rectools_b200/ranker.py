@@ -304,6 +304,71 @@ class Engine:
         `sparse_subjects`: the batch rows as a CSR matrix [n_rows, d] (EASE), instead of `subjects` / `subject_ids`.
         `object_rows`: batch row r is the engine's own stored object row object_rows[r], used as the score row (EASE
         item-to-item; needs d == n_objects), instead of any subjects."""
+        q, keep, n_rows, n_pos = self._host_query(k, subjects, subject_ids, indptr, indices, whitelist, flags, sparse_subjects, object_rows)
+        k_out = max(0, min(int(k), n_pos))
+        ids, scores, counts = self._host_outputs(q, n_rows, k_out, out)
+        self.topk_raw(q)
+        del keep
+        return ids, scores, counts
+
+    def topk_candidates(
+        self,
+        k: int,
+        cand_indptr: np.ndarray,
+        cand_indices: np.ndarray,
+        subjects: tp.Optional[np.ndarray] = None,
+        subject_ids: tp.Optional[np.ndarray] = None,
+        indptr: tp.Optional[np.ndarray] = None,
+        indices: tp.Optional[np.ndarray] = None,
+        flags: int = 0,
+        out: tp.Optional[tp.Tuple[np.ndarray, np.ndarray, np.ndarray]] = None,
+        whitelist: tp.Optional[np.ndarray] = None,
+        sparse_subjects: tp.Optional[sparse.csr_matrix] = None,
+        object_rows: tp.Optional[np.ndarray] = None,
+    ) -> tp.Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """Host-buffer call of `b200_rank_topk_candidates` (path 5): row r is ranked against its own object ids
+        `cand_indices[cand_indptr[r]:cand_indptr[r+1]]` (strictly ascending within a row), minus its filter row.  Returns padded
+        `(ids [n,k_out] int32, scores [n,k_out] fp32, counts [n] int32)` with k_out = min(k, n_objects).  `whitelist`,
+        `sparse_subjects` and `object_rows` are passed through for the engine to refuse."""
+        q, keep, n_rows, _ = self._host_query(k, subjects, subject_ids, indptr, indices, whitelist, flags, sparse_subjects, object_rows)
+        cand_indptr = np.ascontiguousarray(cand_indptr, dtype=np.int64).reshape(-1)
+        cand_indices = np.ascontiguousarray(cand_indices, dtype=np.int32).reshape(-1)
+        if len(cand_indptr) != n_rows + 1:
+            raise ValueError("`cand_indptr` must have `n_rows + 1` entries")
+        k_out = max(0, min(int(k), self.n_objects))
+        ids, scores, counts = self._host_outputs(q, n_rows, k_out, out)
+        st = _lib.Stats()
+        _lib.check(self._lib.b200_rank_topk_candidates(self._h, C.byref(q), cand_indptr.ctypes.data, cand_indices.ctypes.data, C.byref(st)))
+        self.last_stats = st.as_dict()
+        del keep
+        return ids, scores, counts
+
+    @staticmethod
+    def _host_outputs(
+        q: _lib.Query, n_rows: int, k_out: int, out: tp.Optional[tp.Tuple[np.ndarray, np.ndarray, np.ndarray]]
+    ) -> tp.Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        if out is None:
+            ids = np.empty((n_rows, k_out), dtype=np.int32)
+            scores = np.empty((n_rows, k_out), dtype=np.float32)
+            counts = np.zeros(n_rows, dtype=np.int32)
+        else:
+            ids, scores, counts = out
+        q.out_ids, q.out_scores, q.out_counts = ids.ctypes.data, scores.ctypes.data, counts.ctypes.data
+        return ids, scores, counts
+
+    def _host_query(
+        self,
+        k: int,
+        subjects: tp.Optional[np.ndarray],
+        subject_ids: tp.Optional[np.ndarray],
+        indptr: tp.Optional[np.ndarray],
+        indices: tp.Optional[np.ndarray],
+        whitelist: tp.Optional[np.ndarray],
+        flags: int,
+        sparse_subjects: tp.Optional[sparse.csr_matrix],
+        object_rows: tp.Optional[np.ndarray],
+    ) -> tp.Tuple[_lib.Query, tp.List[np.ndarray], int, int]:
+        """The query of a host-buffer call without its outputs: `(query, arrays it points into, n_rows, n_pos)`."""
         q = _lib.Query()
         keep = []
         if object_rows is not None:
@@ -360,17 +425,7 @@ class Engine:
             keep.append(whitelist)
         q.k = int(k)
         q.flags = int(flags)
-        k_out = max(0, min(int(k), n_pos))
-        if out is None:
-            ids = np.empty((n_rows, k_out), dtype=np.int32)
-            scores = np.empty((n_rows, k_out), dtype=np.float32)
-            counts = np.zeros(n_rows, dtype=np.int32)
-        else:
-            ids, scores, counts = out
-        q.out_ids, q.out_scores, q.out_counts = ids.ctypes.data, scores.ctypes.data, counts.ctypes.data
-        self.topk_raw(q)
-        del keep
-        return ids, scores, counts
+        return q, keep, n_rows, n_pos
 
 
 class EngineGroup(Engine):
@@ -458,6 +513,11 @@ class EngineGroup(Engine):
     def candidate_snapshot(self) -> tp.Optional[tp.Dict[str, tp.Any]]:
         raise NotImplementedError("snapshots are taken by single engines")
 
+    def topk_candidates(self, *args: tp.Any, **kwargs: tp.Any) -> tp.Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        raise NotImplementedError(
+            "candidate sets are ranked by single engines: an engine group has no candidate-set export yet (use one device)"
+        )
+
 
 Devices = tp.Union[int, str, tp.Sequence[int]]
 
@@ -542,6 +602,31 @@ def rank_object_rows_padded(
         return target_ids, z.astype(np.int32), z.astype(np.float32), np.zeros(len(target_ids), np.int32)
     ids, scores, counts = engine.topk(k, object_rows=target_ids, indptr=indptr, indices=indices, whitelist=whitelist)
     return target_ids, ids, scores, counts
+
+
+def normalize_candidates(
+    candidates_csr: tp.Any, n_rows: int, n_objects: int, sorted_object_whitelist: tp.Optional[np.ndarray] = None
+) -> tp.Tuple[np.ndarray, np.ndarray]:
+    """Per-row allow-lists as the engine takes them: `(indptr int64 [n_rows + 1], indices int32)`, row r = the sorted,
+    de-duplicated column ids of the STRUCTURE of `candidates_csr` row r (stored values, zeros included, are ignored, as for
+    `filter_pairs_csr`), intersected with `sorted_object_whitelist` when it is given.  Works on copies: the caller's matrix
+    is never changed."""
+    if candidates_csr.shape[0] != n_rows:
+        raise ValueError("Number of rows in `candidates_csr` must be equal to `len(subject_ids)`")
+    csr = candidates_csr if sparse.isspmatrix_csr(candidates_csr) else sparse.csr_matrix(candidates_csr)
+    indptr = np.asarray(csr.indptr, dtype=np.int64)
+    indices = np.asarray(csr.indices, dtype=np.int64)[indptr[0] : indptr[-1]]
+    indptr = indptr - indptr[0]
+    if len(indices) and (indices.min() < 0 or indices.max() >= n_objects):
+        raise ValueError(f"Candidate object ids in `candidates_csr` must be in [0, {n_objects}) (the objects of the ranker)")
+    rows = np.repeat(np.arange(n_rows, dtype=np.int64), np.diff(indptr))
+    key = np.unique(rows * n_objects + indices)  # sorted within a row, duplicates once (a new array)
+    if sorted_object_whitelist is not None:
+        key = key[np.isin(key % max(n_objects, 1), sorted_object_whitelist)]
+    rows, cols = np.divmod(key, max(n_objects, 1))
+    out_indptr = np.zeros(n_rows + 1, dtype=np.int64)
+    np.cumsum(np.bincount(rows, minlength=n_rows), out=out_indptr[1:])
+    return out_indptr, cols.astype(np.int32)
 
 
 def flatten_padded(
@@ -777,6 +862,84 @@ class B200Ranker:
         target_ids, ids, scores, counts = self.rank_object_rows_padded(target_ids, k, filter_pairs_csr, sorted_object_whitelist)
         return flatten_padded(target_ids, ids, scores, counts)
 
+    def rank_candidates_padded(
+        self,
+        subject_ids: InternalIds,
+        candidates_csr: tp.Any,
+        k: tp.Optional[int] = None,
+        filter_pairs_csr: tp.Optional[sparse.csr_matrix] = None,
+        sorted_object_whitelist: tp.Optional[np.ndarray] = None,
+        flags: int = 0,
+    ) -> tp.Tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+        """`rank_candidates` without the ragged flattening: `(subject_ids, ids [n,k], scores [n,k], counts [n])`."""
+        subject_ids = np.asarray(subject_ids, dtype=np.int64).reshape(-1)
+        if filter_pairs_csr is not None and filter_pairs_csr.shape[0] != len(subject_ids):
+            raise ValueError("Number of rows in `filter_pairs_csr` must be equal to `len(sublect_ids)`")
+        if len(subject_ids) and (subject_ids.min() < 0 or subject_ids.max() >= self.n_subjects):
+            raise IndexError("subject id out of range")
+        if self._subjects_csr is not None:
+            raise NotImplementedError("sparse (CSR) subjects are not ranked against candidate sets")
+        if isinstance(self.engine, EngineGroup):
+            raise NotImplementedError(
+                "candidate sets are ranked by single engines: an engine group has no candidate-set export yet (use one device)"
+            )
+        whitelist = None
+        if sorted_object_whitelist is not None:
+            whitelist = np.asarray(sorted_object_whitelist, dtype=np.int64).reshape(-1)
+            check_whitelist(whitelist, self.n_objects)
+        cand_indptr, cand_indices = normalize_candidates(candidates_csr, len(subject_ids), self.n_objects, whitelist)
+        if k is None:
+            k = int(np.diff(cand_indptr).max()) if len(subject_ids) else 0  # the longest list
+            if k == 0:
+                z = np.empty((len(subject_ids), 0))
+                return subject_ids, z.astype(np.int32), z.astype(np.float32), np.zeros(len(subject_ids), np.int32)
+        if k <= 0:
+            raise ValueError("`k` must be positive")
+        indptr = indices = None
+        if filter_pairs_csr is not None:
+            csr = filter_pairs_csr if sparse.isspmatrix_csr(filter_pairs_csr) else sparse.csr_matrix(filter_pairs_csr)
+            if not csr.has_sorted_indices:
+                csr = csr.sorted_indices()
+            indptr, indices = csr.indptr, csr.indices
+        if self.n_objects == 0 or len(subject_ids) == 0:
+            z = np.empty((len(subject_ids), 0))
+            return subject_ids, z.astype(np.int32), z.astype(np.float32), np.zeros(len(subject_ids), np.int32)
+        if getattr(self, "_subjects", None) is not None and self.engine.subjects_owner is not self:
+            self.engine.set_subjects(self._subjects, key=self._subjects_key, owner=self)
+        ids, scores, counts = self.engine.topk_candidates(
+            k, cand_indptr, cand_indices, subject_ids=subject_ids, indptr=indptr, indices=indices, flags=flags
+        )
+        self.last_stats = self.engine.last_stats
+        return (subject_ids,) + strip_sentinel_tail(ids, scores, counts)
+
+    def rank_candidates(
+        self,
+        subject_ids: InternalIds,
+        candidates_csr: tp.Any,
+        k: tp.Optional[int] = None,
+        filter_pairs_csr: tp.Optional[sparse.csr_matrix] = None,
+        sorted_object_whitelist: tp.Optional[np.ndarray] = None,
+    ) -> tp.Tuple[InternalIds, InternalIds, Scores]:
+        """Rank subject r against its own allow-list only: the structure of `candidates_csr` row r (column ids are object ids;
+        unsorted rows and repeated ids are fine), minus its `filter_pairs_csr` row, intersected with
+        `sorted_object_whitelist`.  `k = None`: the longest list.  Returns what `rank` returns -- flat `(subject ids repeated,
+        object ids, scores)`, grouped by subject in input order, best first, with the same scores for the same pairs."""
+        subject_ids, ids, scores, counts = self.rank_candidates_padded(
+            subject_ids, candidates_csr, k, filter_pairs_csr, sorted_object_whitelist
+        )
+        return self._final_scores(*flatten_padded(subject_ids, ids, scores, counts))
+
+    def _final_scores(
+        self, all_subjects: np.ndarray, all_ids: np.ndarray, all_scores: np.ndarray
+    ) -> tp.Tuple[InternalIds, InternalIds, Scores]:
+        """COSINE / EUCLIDEAN post-scaling of the flat triplet (rank_implicit.py:132-140)."""
+        if self.distance == Distance.COSINE:
+            all_scores = all_scores / self.subjects_norms[all_subjects]  # rank_implicit.py:132-134
+        elif self.distance == Distance.EUCLIDEAN:
+            d2 = self.subjects_dots[all_subjects] - all_scores  # rank_implicit.py:136-140
+            all_scores = np.sqrt(np.maximum(d2, 0)).astype(np.float32)
+        return all_subjects, all_ids, all_scores
+
     def rank(
         self,
         subject_ids: InternalIds,
@@ -787,10 +950,4 @@ class B200Ranker:
         """Same contract as `ImplicitRanker.rank` (rank_implicit.py:187-280): flat `(subject ids repeated, object ids,
         scores)`, grouped by subject in input order, best first, filtered objects never returned."""
         subject_ids, ids, scores, counts = self.rank_padded(subject_ids, k, filter_pairs_csr, sorted_object_whitelist)
-        all_subjects, all_ids, all_scores = flatten_padded(subject_ids, ids, scores, counts)
-        if self.distance == Distance.COSINE:
-            all_scores = all_scores / self.subjects_norms[all_subjects]  # rank_implicit.py:132-134
-        elif self.distance == Distance.EUCLIDEAN:
-            d2 = self.subjects_dots[all_subjects] - all_scores  # rank_implicit.py:136-140
-            all_scores = np.sqrt(np.maximum(d2, 0)).astype(np.float32)
-        return all_subjects, all_ids, all_scores
+        return self._final_scores(*flatten_padded(subject_ids, ids, scores, counts))
