@@ -222,7 +222,8 @@ int b200_rank_get_info(b200_rank_engine* engine, b200_rank_info* info);
  * Refused, with every output untouched:
  *   B200_E_INVALID      cand_indptr NULL or not monotone, candidate ids out of range or not strictly ascending in a row,
  *                       and every argument check of b200_rank_topk;
- *   B200_E_UNSUPPORTED  B200_Q_INPUTS_ON_DEVICE, B200_Q_OUTPUTS_ON_DEVICE, resident subjects set from a device pointer,
+ *   B200_E_UNSUPPORTED  B200_Q_INPUTS_ON_DEVICE, B200_Q_OUTPUTS_ON_DEVICE, resident subjects set from a device pointer
+ *                       (device lists and subjects: b200_rank_topk_candidates_device below),
  *                       sub_* and object_rows, a global whitelist (intersect it into the lists), B200_Q_SHARED_THRESHOLDS,
  *                       B200_Q_FORCE_TC, a non-zero id offset, d > 49152;
  *   B200_E_NOMEM        a row whose scores (4 B per candidate), sort scratch (16 B per candidate when k_out > 12288) and
@@ -233,6 +234,33 @@ int b200_rank_topk_candidates(b200_rank_engine* engine, const b200_rank_query* q
                               const int64_t* cand_indptr,  /* [n_rows + 1] */
                               const int32_t* cand_indices, /* object ids, strictly ascending within a row */
                               b200_rank_stats* stats /* nullable */);
+
+/* Candidate sets from device memory (stats.path = 5), for lists a GPU stage produced.  Same arguments; every input
+ * pointer -- cand_indptr, cand_indices, subjects, subject_ids, csr_* -- is device memory on the engine's device and
+ * B200_Q_INPUTS_ON_DEVICE is required (without it: B200_E_INVALID).  cand_indptr is [n_rows + 1] int64 offsets into
+ * cand_indices with any base >= 0, monotone; cand_indices are int32 ids in ANY order, repeats allowed; an entry outside
+ * [0, n_objects), negatives included, is no candidate and is never read as an object (a padded [n_rows, m] id matrix
+ * with -1 holes is passed with cand_indptr[r] = m * r).  Row r's set is the distinct valid ids of its slice, minus its
+ * filter row (device CSR, as for b200_rank_topk).  The result is, bit for bit, that of b200_rank_topk_candidates on the
+ * lists normalised on the host (sorted, valid, unique).  Subjects: a `subjects` matrix in batch order (fp32 / fp16 / bf16
+ * by subject_dtype), an fp32 `subjects` matrix with subject_ids, or subject_ids over resident subjects (set from the host
+ * or from a device pointer); device subject_ids and filter ids are the caller's contract, as in b200_rank_topk.  Outputs:
+ * device buffers with B200_Q_OUTPUTS_ON_DEVICE, written in place, else host buffers.  The call is ordered after the work
+ * queued on query.stream (NULL: the legacy default stream), which waits for device outputs.  cand_indptr is copied to
+ * the host once (n_rows + 1 words) to plan the row chunks.
+ * Refused, with every output untouched:
+ *   B200_E_INVALID      no B200_Q_INPUTS_ON_DEVICE, cand_indptr NULL, cand_indptr[0] < 0 or not monotone, cand_indices
+ *                       NULL with entries, and every argument check of b200_rank_topk;
+ *   B200_E_UNSUPPORTED  sub_* and object_rows, a global whitelist (mask it into the lists), B200_Q_SHARED_THRESHOLDS,
+ *                       B200_Q_FORCE_TC, a non-zero id offset, d > 49152;
+ *   B200_E_NOMEM        a row whose raw entries alone need more than a row chunk's 1 GiB: 8 B each (prepared ids and
+ *                       scores), 16 B more above 12288 entries (the preparation's sort scratch), 16 B more when
+ *                       k_out > 12288 (the selection's), plus 8 B x k_out of host outputs.
+ * stats: ms_main = preparation + scoring, ms_select = selection. */
+int b200_rank_topk_candidates_device(b200_rank_engine* engine, const b200_rank_query* query,
+                                     const int64_t* cand_indptr,  /* device, [n_rows + 1] */
+                                     const int32_t* cand_indices, /* device, object ids in any order */
+                                     b200_rank_stats* stats /* nullable */);
 
 /* Merge `n_lists` per-shard results (device pointers, each [n_rows, k] / [n_rows], list l at base + l * stride) into
  * the global top-k ordered by (score desc, id asc).  Runs on `stream` of `device`. */

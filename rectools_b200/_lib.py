@@ -26,6 +26,7 @@ EXPORTS = (
     "b200_rank_set_id_offset",
     "b200_rank_topk",
     "b200_rank_topk_candidates",
+    "b200_rank_topk_candidates_device",
     "b200_rank_get_info",
     "b200_rank_merge",
     "b200_rank_merge_certified",
@@ -178,6 +179,8 @@ def load() -> C.CDLL:
     lib.b200_rank_topk.argtypes = [vp, C.POINTER(Query), C.POINTER(Stats)]
     lib.b200_rank_topk_candidates.restype = C.c_int
     lib.b200_rank_topk_candidates.argtypes = [vp, C.POINTER(Query), vp, vp, C.POINTER(Stats)]
+    lib.b200_rank_topk_candidates_device.restype = C.c_int
+    lib.b200_rank_topk_candidates_device.argtypes = [vp, C.POINTER(Query), vp, vp, C.POINTER(Stats)]
     lib.b200_rank_get_info.restype = C.c_int
     lib.b200_rank_get_info.argtypes = [vp, C.POINTER(Info)]
     lib.b200_rank_merge.restype = C.c_int

@@ -7,6 +7,7 @@
 // exhaustive fp64 kernel) and returns padded [n_rows, k] arrays plus per-row counts.
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <cmath>
@@ -28,6 +29,7 @@
 #include "large_k_select.cuh"
 #include "row_select.cuh"
 #include "cand_select.cuh"
+#include "cand_prep.cuh"
 #include "fused_topk.cuh"
 
 namespace {
@@ -167,6 +169,8 @@ struct b200_rank_engine {
     DevBuf part_scores, part_ids;
     DevBuf fb_rows, scratch, excl, carousel, patch;
     DevBuf lk_scratch;            // sort scratch of the radix selection (k_out > LK_SMEM_PAIRS)
+    DevBuf cand_sort, cand_soff;  // device candidate lists: sort scratch of rows above LK_SMEM_PAIRS and their offsets in it,
+    DevBuf scan_tmp;              // and the row scan's storage
     int32_t* h_pinned = nullptr;  // small pinned scratch (counters)
     std::vector<char> h_patch;    // host copy of re-ranked rows (host-output calls)
 
@@ -181,7 +185,7 @@ struct b200_rank_engine {
         return {&obj_own, &obj16, &obj_norms, &objT, &sub32_res, &peer_pub, &sub32, &sub16, &row_exp, &rowmap, &indptr, &indices, &wl,
                 &obj16_wl, &sp_indptr, &sp_indices, &sp_data, &sp_scores, &out_ids, &out_scores, &out_counts, &out_bounds, &cand_scores,
                 &cand_ids, &cand_counts, &cand_thr, &part_scores, &part_ids, &fb_rows, &scratch, &excl, &carousel, &patch, &lk_scratch,
-                &snap_scores, &snap_ids, &snap_counts, &snap_thr, &snap_row_exp, &snap_rows, &snap_fb};
+                &cand_sort, &cand_soff, &scan_tmp, &snap_scores, &snap_ids, &snap_counts, &snap_thr, &snap_row_exp, &snap_rows, &snap_fb};
     }
     std::vector<cudaEvent_t*> call_events() { return {&ev_begin, &ev_staged, &ev_ranked, &ev_end, &ev_from_user, &ev_to_user}; }
     size_t hbm_bytes() {
@@ -413,6 +417,7 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
         // on the device, and smaller launches stay within it
         CK(cudaFuncSetAttribute(large_k_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lk_smem_bytes(LK_SMEM_PAIRS)));
         CK(cudaFuncSetAttribute(cand_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lk_smem_bytes(LK_SMEM_PAIRS)));
+        CK(cudaFuncSetAttribute(cand_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lk_smem_bytes(LK_SMEM_PAIRS)));
     } catch (const CudaError& ce) {
         int rc = fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_create: %s failed at line %d: %s",
                       ce.what, ce.line, cudaGetErrorString(ce.e));
@@ -1402,6 +1407,107 @@ void run_candidates(Call& c, const int64_t* cand_indptr, const int32_t* cand_ind
     CK(cudaStreamSynchronize(st));  // the next chunk reuses every buffer
 }
 
+// Path 5 from device memory: rows [r0, r1) of a b200_rank_topk_candidates_device call, prepared (cand_prep.cuh), scored,
+// selected and -- for host outputs -- copied back, on the engine stream.  `h_indptr` is the host copy of the device
+// cand_indptr.
+// Buffers: sp_indptr / sp_indices hold the prepared rows, sp_scores first the prepared ids at their raw offsets and then
+// the scores, cand_sort / lk_scratch the sorts' global scratch, sub32 widened 16-bit subject rows, out_* host outputs.
+// `sort_off` (device, [n_rows] of the call, or nullptr when no row is longer than LK_SMEM_PAIRS): each long row's entry
+// offset into cand_sort, a prefix over the chunk's long rows only.
+void run_candidates_device(Call& c, const int64_t* cand_indptr, const int32_t* cand_indices, const int64_t* h_indptr,
+                           const int64_t* sort_off, int64_t r0, int64_t r1) {
+    b200_rank_engine* E = c.E;
+    const b200_rank_query* q = c.q;
+    cudaStream_t st = c.st;
+    const int64_t nr = r1 - r0, k_out = c.k_out, d = c.d;
+    int64_t max_len = 0;
+    for (int64_t r = r0; r < r1; ++r) max_len = std::max(max_len, h_indptr[r + 1] - h_indptr[r]);
+
+    CandParams cp{};
+    cp.sp.objects = E->obj_ptr;
+    cp.sp.d = c.d;
+    cp.sp.obj_norms = c.norms();
+    cp.c_indptr = E->sp_indptr.as<int64_t>();
+    cp.c_indices = E->sp_indices.as<int32_t>();
+    cp.scores = E->sp_scores.as<float>();
+    if (q->csr_indptr) {  // the caller's device CSR: absolute offsets into csr_indices
+        cp.f_indptr = q->csr_indptr + r0;
+        cp.f_indices = q->csr_indices;
+    }
+    if (q->subject_ids) {
+        cp.row_map = q->subject_ids + r0;
+        cp.subjects = q->subjects ? q->subjects : E->sub32_res_ptr;
+    } else if (q->subject_dtype != B200_DT_F32) {
+        widen16_kernel<<<grid_for(nr * d, 256), 256, 0, st>>>(reinterpret_cast<const char*>(q->subjects) + 2 * r0 * d,
+                                                              q->subject_dtype == B200_DT_BF16 ? 1 : 0, nr * d, E->sub32.as<float>());
+        CK(cudaGetLastError());
+        c.S.n_launches++;
+        cp.subjects = E->sub32.as<float>();
+    } else {
+        cp.subjects = q->subjects + r0 * d;
+    }
+    cp.n_rows = nr;
+    cp.k_out = (int32_t)k_out;
+    cp.smem_pairs = (int32_t)std::min<int64_t>(k_out, LK_SMEM_PAIRS);
+    cp.scratch = k_out > LK_SMEM_PAIRS ? E->lk_scratch.as<uint32_t>() : nullptr;
+    if (c.out_dev) {
+        cp.out_ids = q->out_ids + r0 * k_out;
+        cp.out_scores = q->out_scores + r0 * k_out;
+        cp.out_counts = q->out_counts + r0;
+    } else {
+        cp.out_ids = E->out_ids.as<int32_t>();
+        cp.out_scores = E->out_scores.as<float>();
+        cp.out_counts = E->out_counts.as<int32_t>();
+    }
+
+    c.time_begin(0);
+    if (max_len > 0) {
+        CandPrepParams pp{};
+        pp.raw_indptr = cand_indptr + r0;
+        pp.raw_indices = cand_indices;
+        pp.raw_base = h_indptr[r0];
+        pp.n_rows = nr;
+        pp.n_objects = E->n_obj;
+        pp.smem_pairs = (int32_t)std::min<int64_t>(max_len, LK_SMEM_PAIRS);
+        if (max_len > LK_SMEM_PAIRS) {
+            pp.scratch = E->cand_sort.as<uint32_t>();
+            pp.sort_off = sort_off + r0;
+        }
+        pp.ids = reinterpret_cast<int32_t*>(E->sp_scores.p);
+        pp.kept = E->sp_indptr.as<int64_t>();
+        cand_prep_kernel<<<(unsigned)nr, LK_THREADS, lk_smem_bytes(pp.smem_pairs), st>>>(pp);
+        CK(cudaGetLastError());
+        size_t tmp_bytes = E->scan_tmp.cap;
+        CK(cub::DeviceScan::ExclusiveSum(E->scan_tmp.p, tmp_bytes, pp.kept, pp.kept, nr + 1, st));  // in place
+        const unsigned segs = (unsigned)std::min<int64_t>(65535, (max_len + CS_SEG - 1) / CS_SEG);
+        cand_compact_kernel<<<dim3((unsigned)nr, segs), 256, 0, st>>>(pp.raw_indptr, pp.raw_base, pp.ids, pp.kept, E->sp_indices.as<int32_t>(),
+                                                                      CS_SEG);
+        CK(cudaGetLastError());
+        const size_t smem = sizeof(float) * (size_t)c.d;
+        with_obj_type(E, [&](auto t) {
+            using TO = typename decltype(t)::type;
+            if (smem > 48 * 1024) CK(cudaFuncSetAttribute(cand_score_kernel<TO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            cand_score_kernel<TO><<<dim3((unsigned)nr, segs), CS_THREADS, smem, st>>>(cp);
+        });
+        CK(cudaGetLastError());
+        c.S.n_launches += 4;  // preparation, scan, compaction, scores
+    } else {  // every row empty: the selection pads them
+        CK(cudaMemsetAsync(E->sp_indptr.p, 0, sizeof(int64_t) * (nr + 1), st));
+    }
+    c.time_end();
+    c.time_begin(1);
+    cand_select_kernel<<<(unsigned)nr, LK_THREADS, lk_smem_bytes((int)k_out), st>>>(cp);
+    CK(cudaGetLastError());
+    c.time_end();
+    c.S.n_launches++;
+    if (!c.out_dev) {
+        CK(cudaMemcpyAsync(q->out_ids + r0 * k_out, cp.out_ids, sizeof(int32_t) * nr * k_out, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(q->out_scores + r0 * k_out, cp.out_scores, sizeof(float) * nr * k_out, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(q->out_counts + r0, cp.out_counts, sizeof(int32_t) * nr, cudaMemcpyDeviceToHost, st));
+        c.S.d2h_bytes += nr * k_out * 8 + nr * 4;
+    }
+}
+
 }  // namespace
 
 int b200_check_query(const b200_rank_engine* E, const b200_rank_query* q, int32_t* k_out) {
@@ -1764,6 +1870,119 @@ int b200_rank_topk_candidates(b200_rank_engine* E, const b200_rank_query* q, con
         c.S.n_tc_launches = 0;  // (collect_times counts the scoring launches there)
     } catch (const CudaError& ce) {
         return fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_topk_candidates: %s failed at line %d: %s",
+                    ce.what, ce.line, cudaGetErrorString(ce.e));
+    }
+    if (stats) *stats = c.S;
+    return B200_OK;
+}
+
+int b200_rank_topk_candidates_device(b200_rank_engine* E, const b200_rank_query* q, const int64_t* cand_indptr,
+                                     const int32_t* cand_indices, b200_rank_stats* stats) {
+    if (!E || !q) return fail(B200_E_INVALID, "b200_rank_topk_candidates_device: NULL argument");
+    CandShape shape;
+    shape.n_rows = q->n_rows;
+    shape.n_objects = E->n_obj;
+    shape.k = q->k;
+    shape.d = E->d;
+    shape.flags = q->flags;
+    shape.whitelist = q->whitelist != nullptr;
+    shape.sparse = q->sub_indptr || q->sub_indices || q->sub_data;
+    shape.rows = q->object_rows != nullptr;
+    shape.id_offset = E->id_offset != 0;
+    // the path's own refusals first, then b200_rank_topk's checks, then the arrays (one host copy of cand_indptr)
+    const CandPlan pre = refuse_candidates_device(shape);
+    if (pre.error != B200_OK) return fail(pre.error, "%s", pre.message.c_str());
+    if (const int rc = validate_query(E, q)) return rc;
+    std::lock_guard<std::mutex> lock(E->mu);
+    E->snap.valid = 0;
+    Call c{};
+    c.E = E;
+    c.q = q;
+    memset(&c.S, 0, sizeof(c.S));
+    c.n_rows = q->n_rows;
+    c.n_pos = E->n_obj;
+    c.d = E->d;
+    c.in_dev = true;
+    c.out_dev = q->flags & B200_Q_OUTPUTS_ON_DEVICE;
+    c.hooks = read_hooks();
+    c.S.k_out = c.k_out = pre.k_out;
+    c.S.path = (int)Path::CANDIDATES;
+    if (c.n_rows == 0 || c.k_out <= 0) {
+        if (stats) *stats = c.S;
+        return B200_OK;
+    }
+    if (!cand_indptr) return fail(B200_E_INVALID, "b200_rank_topk_candidates_device: cand_indptr is NULL");
+    if (q->csr_indptr && !q->csr_indices) return fail(B200_E_INVALID, "b200_rank_topk_candidates_device: csr_indices is NULL");
+    try {
+        CK(cudaSetDevice(E->device));
+        cudaStream_t st = c.st = E->st;
+        // every input is the caller's device memory (NULL stream: the legacy default stream), as in b200_rank_topk
+        cudaStream_t user = q->stream ? reinterpret_cast<cudaStream_t>(q->stream) : cudaStreamLegacy;
+        CK(cudaEventRecord(E->ev_from_user, user));
+        CK(cudaStreamWaitEvent(st, E->ev_from_user, 0));
+        CK(cudaEventRecord(E->ev_begin, st));
+        std::vector<int64_t> h_indptr(c.n_rows + 1);
+        CK(cudaMemcpyAsync(h_indptr.data(), cand_indptr, sizeof(int64_t) * (c.n_rows + 1), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        c.S.d2h_bytes += (int64_t)sizeof(int64_t) * (c.n_rows + 1);
+        const CandPlan P = plan_candidates_device(shape, h_indptr.data(), c.hooks);
+        if (P.error != B200_OK) return fail(P.error, "%s", P.message.c_str());
+        if (h_indptr[c.n_rows] > h_indptr[0] && !cand_indices)
+            return fail(B200_E_INVALID, "b200_rank_topk_candidates_device: cand_indices is NULL");
+
+        const int64_t rows = P.max_chunk_rows, cands = P.max_chunk_cands;
+        int64_t max_len = 0;
+        for (int64_t r = 0; r < c.n_rows; ++r) max_len = std::max(max_len, h_indptr[r + 1] - h_indptr[r]);
+        E->sp_indptr.ensure(sizeof(int64_t) * (rows + 1));
+        E->sp_indices.ensure(std::max<size_t>(sizeof(int32_t) * cands, 16));
+        E->sp_scores.ensure(std::max<size_t>(sizeof(float) * cands, 16));
+        // rows longer than LK_SMEM_PAIRS sort in cand_sort, at a prefix over the chunk's long rows: 16 B per entry of
+        // those rows, which is what the plan charges them
+        std::vector<int64_t> h_soff;
+        const int64_t* sort_off = nullptr;
+        if (max_len > LK_SMEM_PAIRS) {
+            h_soff.assign(c.n_rows, 0);
+            int64_t max_sort = 0;
+            for (int64_t ci = 0; ci < P.n_chunks(); ++ci) {
+                int64_t sum = 0;
+                for (int64_t r = P.bounds[ci]; r < P.bounds[ci + 1]; ++r) {
+                    const int64_t len = h_indptr[r + 1] - h_indptr[r];
+                    if (len > LK_SMEM_PAIRS) {
+                        h_soff[r] = sum;
+                        sum += len;
+                    }
+                }
+                max_sort = std::max(max_sort, sum);
+            }
+            E->cand_sort.ensure((size_t)16 * max_sort);
+            E->cand_soff.ensure(sizeof(int64_t) * c.n_rows);
+            CK(cudaMemcpyAsync(E->cand_soff.p, h_soff.data(), sizeof(int64_t) * c.n_rows, cudaMemcpyHostToDevice, st));
+            c.S.h2d_bytes += (int64_t)sizeof(int64_t) * c.n_rows;
+            sort_off = E->cand_soff.as<int64_t>();
+        }
+        if (c.k_out > LK_SMEM_PAIRS) E->lk_scratch.ensure(std::max<size_t>((size_t)16 * cands, 16));
+        size_t tmp_bytes = 0;
+        CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, E->sp_indptr.as<int64_t>(), E->sp_indptr.as<int64_t>(), rows + 1, st));
+        E->scan_tmp.ensure(std::max<size_t>(tmp_bytes, 16));
+        if (q->subjects && !q->subject_ids && q->subject_dtype != B200_DT_F32) E->sub32.ensure(sizeof(float) * rows * c.d);
+        if (!c.out_dev) {
+            E->out_ids.ensure(sizeof(int32_t) * rows * c.k_out);
+            E->out_scores.ensure(sizeof(float) * rows * c.k_out);
+            E->out_counts.ensure(sizeof(int32_t) * rows);
+        }
+        for (int64_t ci = 0; ci < P.n_chunks(); ++ci) run_candidates_device(c, cand_indptr, cand_indices, h_indptr.data(), sort_off, P.bounds[ci], P.bounds[ci + 1]);
+        c.S.n_chunks = (int32_t)P.n_chunks();
+        CK(cudaEventRecord(E->ev_end, st));
+        if (c.out_dev) {
+            CK(cudaEventRecord(E->ev_to_user, st));
+            CK(cudaStreamWaitEvent(user, E->ev_to_user, 0));
+        }
+        CK(cudaStreamSynchronize(st));
+        CK(cudaEventElapsedTime(&c.S.ms_total, E->ev_begin, E->ev_end));
+        c.collect_times();
+        c.S.n_tc_launches = 0;  // (collect_times counts the preparation + scoring spans there)
+    } catch (const CudaError& ce) {
+        return fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_topk_candidates_device: %s failed at line %d: %s",
                     ce.what, ce.line, cudaGetErrorString(ce.e));
     }
     if (stats) *stats = c.S;

@@ -305,6 +305,48 @@ struct CandPlan {
     int64_t n_chunks() const { return bounds.empty() ? 0 : (int64_t)bounds.size() - 1; }
 };
 
+// The candidate-row-pointer checks and the row chunks of a call that passed its refusals (`p` holds its k_out).  Chunks
+// take whole rows, in order, while the bytes `row_bytes(len)` of their rows stay within `budget` and their rows within
+// B200_CHUNK_ROWS when it is set; a row that alone exceeds the budget is refused with B200_E_NOMEM.  `who` prefixes the
+// messages.
+template <typename RowBytes>
+inline CandPlan cand_chunks(CandPlan p, int64_t n_rows, const int64_t* indptr, const Hooks& h, int64_t budget, const std::string& who,
+                            RowBytes row_bytes) {
+    auto refuse = [&](int code, const std::string& why) {
+        p.error = code;
+        p.message = who + why;
+        return p;
+    };
+    if (!indptr) return refuse(B200_E_INVALID, "cand_indptr is NULL");
+    if (indptr[0] < 0) return refuse(B200_E_INVALID, "cand_indptr[0] < 0");
+    for (int64_t r = 0; r < n_rows; ++r)
+        if (indptr[r + 1] < indptr[r])
+            return refuse(B200_E_INVALID, "cand_indptr is not monotone at row " + std::to_string(r));
+    const int64_t max_rows = h.chunk_rows > 0 ? h.chunk_rows : n_rows;
+    p.bounds.push_back(0);
+    int64_t bytes = 0, cands = 0, rows = 0;
+    for (int64_t r = 0; r < n_rows; ++r) {
+        const int64_t len = indptr[r + 1] - indptr[r], b = row_bytes(len);
+        if (b > budget)
+            return refuse(B200_E_NOMEM, "row " + std::to_string(r) + " (" + std::to_string(len) + " candidates, k_out = " +
+                                            std::to_string(p.k_out) + ") needs " + std::to_string(b) + " bytes, more than a chunk's " +
+                                            std::to_string(budget));
+        if (rows > 0 && (bytes + b > budget || rows == max_rows)) {
+            p.bounds.push_back(r);
+            p.max_chunk_cands = std::max(p.max_chunk_cands, cands);
+            p.max_chunk_rows = std::max(p.max_chunk_rows, rows);
+            bytes = cands = rows = 0;
+        }
+        bytes += b;
+        cands += len;
+        ++rows;
+    }
+    p.bounds.push_back(n_rows);
+    p.max_chunk_cands = std::max(p.max_chunk_cands, cands);
+    p.max_chunk_rows = std::max(p.max_chunk_rows, rows);
+    return p;
+}
+
 // The refusals, the candidate-row-pointer check and the row chunks of one call.  `indptr` (host, [n_rows + 1]) is read
 // only after the refusals.  Chunks take whole rows, in order, while their bytes stay within `budget` and their rows within
 // B200_CHUNK_ROWS when it is set; a row that alone exceeds the budget is refused with B200_E_NOMEM.
@@ -327,34 +369,48 @@ inline CandPlan plan_candidates(const CandShape& s, const int64_t* indptr, const
     if (s.id_offset) return refuse(B200_E_UNSUPPORTED, "engines with an id offset hold one shard of the catalogue");
     if (s.d > CAND_MAX_D) return refuse(B200_E_UNSUPPORTED, "d = " + std::to_string(s.d) + " exceeds the staged subject row's limit");
     if (s.n_rows == 0 || p.k_out <= 0) return p;  // nothing to rank
-    if (!indptr) return refuse(B200_E_INVALID, "cand_indptr is NULL");
-    if (indptr[0] < 0) return refuse(B200_E_INVALID, "cand_indptr[0] < 0");
-    for (int64_t r = 0; r < s.n_rows; ++r)
-        if (indptr[r + 1] < indptr[r])
-            return refuse(B200_E_INVALID, "cand_indptr is not monotone at row " + std::to_string(r));
-    const int64_t max_rows = h.chunk_rows > 0 ? h.chunk_rows : s.n_rows;
-    p.bounds.push_back(0);
-    int64_t bytes = 0, cands = 0, rows = 0;
-    for (int64_t r = 0; r < s.n_rows; ++r) {
-        const int64_t len = indptr[r + 1] - indptr[r], b = cand_row_bytes(len, p.k_out);
-        if (b > budget)
-            return refuse(B200_E_NOMEM, "row " + std::to_string(r) + " (" + std::to_string(len) + " candidates, k_out = " +
-                                            std::to_string(p.k_out) + ") needs " + std::to_string(b) + " bytes, more than a chunk's " +
-                                            std::to_string(budget));
-        if (rows > 0 && (bytes + b > budget || rows == max_rows)) {
-            p.bounds.push_back(r);
-            p.max_chunk_cands = std::max(p.max_chunk_cands, cands);
-            p.max_chunk_rows = std::max(p.max_chunk_rows, rows);
-            bytes = cands = rows = 0;
-        }
-        bytes += b;
-        cands += len;
-        ++rows;
-    }
-    p.bounds.push_back(s.n_rows);
-    p.max_chunk_cands = std::max(p.max_chunk_cands, cands);
-    p.max_chunk_rows = std::max(p.max_chunk_rows, rows);
+    return cand_chunks(p, s.n_rows, indptr, h, budget, "b200_rank_topk_candidates: ",
+                       [&](int64_t len) { return cand_row_bytes(len, p.k_out); });
+}
+
+// ---- path 5 from device memory (b200_rank_topk_candidates_device).  The raw lists are any int32 ids in any order: a
+// preparation pass sorts each row, drops ids outside [0, n_objects) and repeats, and the kernels above rank what is left.
+// Chunks are planned on the raw lengths, which bound the prepared ones from above.  Per raw entry: 4 B of prepared ids and
+// 4 B of scores, 16 B of preparation scratch when the row is longer than LK_SMEM_PAIRS (it sorts in global memory), 16 B
+// of selection scratch when k_out > LK_SMEM_PAIRS; plus 8 B x k_out per row of staged outputs when they go to the host.
+inline int64_t cand_device_row_bytes(int64_t len, int64_t k_out, bool host_out) {
+    return 8 * len + (len > LK_SMEM_PAIRS ? 16 * len : 0) + (k_out > LK_SMEM_PAIRS ? 16 * len : 0) + (host_out ? 8 * k_out : 0);
+}
+
+// The refusals of a device call that need no array (B200_OK: none); s.res_device is no refusal here.
+inline CandPlan refuse_candidates_device(const CandShape& s) {
+    CandPlan p;
+    p.k_out = (int)std::min<int64_t>(s.k, s.n_objects);
+    auto refuse = [&](int code, const std::string& why) {
+        p.error = code;
+        p.message = "b200_rank_topk_candidates_device: " + why;
+        return p;
+    };
+    if (!(s.flags & B200_Q_INPUTS_ON_DEVICE))
+        return refuse(B200_E_INVALID, "needs B200_Q_INPUTS_ON_DEVICE: host candidate lists go to b200_rank_topk_candidates");
+    if (s.sparse) return refuse(B200_E_UNSUPPORTED, "sparse subjects (sub_*) are not ranked against candidate sets");
+    if (s.rows) return refuse(B200_E_UNSUPPORTED, "stored rows (object_rows) are not ranked against candidate sets");
+    if (s.whitelist) return refuse(B200_E_UNSUPPORTED, "a global whitelist is not taken: mask it into the candidate lists");
+    if (s.flags & B200_Q_SHARED_THRESHOLDS) return refuse(B200_E_UNSUPPORTED, "B200_Q_SHARED_THRESHOLDS has no thresholds to share here");
+    if (s.flags & B200_Q_FORCE_TC) return refuse(B200_E_UNSUPPORTED, "no tensor-core pass scores candidate sets (B200_Q_FORCE_TC)");
+    if (s.id_offset) return refuse(B200_E_UNSUPPORTED, "engines with an id offset hold one shard of the catalogue");
+    if (s.d > CAND_MAX_D) return refuse(B200_E_UNSUPPORTED, "d = " + std::to_string(s.d) + " exceeds the staged subject row's limit");
     return p;
+}
+
+// The refusals, the row-pointer checks and the row chunks of one device call.  `indptr` is the host copy of the device
+// cand_indptr ([n_rows + 1], any base), read only after the refusals.
+inline CandPlan plan_candidates_device(const CandShape& s, const int64_t* indptr, const Hooks& h, int64_t budget = SELECT_CHUNK_BYTES) {
+    const CandPlan p = refuse_candidates_device(s);
+    if (p.error != B200_OK || s.n_rows == 0 || p.k_out <= 0) return p;  // refused, or nothing to rank
+    const bool host_out = !(s.flags & B200_Q_OUTPUTS_ON_DEVICE);
+    return cand_chunks(p, s.n_rows, indptr, h, budget, "b200_rank_topk_candidates_device: ",
+                       [&](int64_t len) { return cand_device_row_bytes(len, p.k_out, host_out); });
 }
 
 // The candidate ids of rows [0, n_rows): in [0, n_objects) and strictly ascending within a row.  B200_OK, or

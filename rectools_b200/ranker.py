@@ -196,6 +196,7 @@ class Engine:
 
     def _set_subjects(self, ptr: int, n_subjects: int, on_device: int) -> None:
         _lib.check(self._lib.b200_rank_set_subjects(self._h, ptr, n_subjects, on_device))
+        self.n_resident_subjects = int(n_subjects)
 
     def peer_export(self, max_rows: int) -> bytes:
         """Allocate this engine's published-threshold array (threshold sharing between the ranks of an item-sharded
@@ -342,6 +343,109 @@ class Engine:
         self.last_stats = st.as_dict()
         del keep
         return ids, scores, counts
+
+    def topk_candidates_device(
+        self,
+        k: int,
+        cand_indptr: tp.Any,
+        cand_indices: tp.Any,
+        subjects: tp.Any = None,
+        subject_ids: tp.Any = None,
+        indptr: tp.Any = None,
+        indices: tp.Any = None,
+        out: tp.Optional[tp.Tuple[tp.Any, tp.Any, tp.Any]] = None,
+        stream: tp.Any = None,
+    ) -> tp.Tuple[tp.Any, tp.Any, tp.Any]:
+        """Device-memory call of `b200_rank_topk_candidates_device` (path 5): row r is ranked against the distinct ids of
+        `cand_indices[cand_indptr[r]:cand_indptr[r+1]]` that are objects of the engine (any order, repeats and out-of-range
+        ids such as -1 holes allowed), minus its filter row.  Every input is a CUDA tensor on the engine's device:
+        `cand_indptr` int64 [n + 1] (any base), `cand_indices` int32, `subjects` fp32 / fp16 / bf16 in batch order or fp32
+        with `subject_ids` (int64), else `subject_ids` over the resident subjects, and the filter CSR `indptr` / `indices`.
+        Returns `(ids [n,k_out] int32, scores [n,k_out] fp32, counts [n] int32)`, k_out = min(k, n_objects): new CUDA
+        tensors, or `out` filled in place (CUDA tensors, or numpy arrays for host outputs).  The call is ordered after
+        `stream` (default: the current torch stream of the device), which waits for device outputs."""
+        import torch
+
+        dev = torch.device("cuda", self.device)
+
+        def device_tensor(name: str, t: tp.Any, dtypes: tp.Tuple[tp.Any, ...]) -> tp.Any:
+            if not _is_cuda_tensor(t) or t.device != dev:
+                raise TypeError(f"`{name}` must be a CUDA tensor on {dev}")
+            if t.dtype not in dtypes:
+                raise TypeError(f"`{name}` must be of dtype {' / '.join(str(d) for d in dtypes)}, not {t.dtype}")
+            return t.contiguous()
+
+        keep = []
+        cand_indptr = device_tensor("cand_indptr", cand_indptr, (torch.int64,)).reshape(-1)
+        cand_indices = device_tensor("cand_indices", cand_indices, (torch.int32,)).reshape(-1)
+        n_rows = len(cand_indptr) - 1
+        if n_rows < 0:
+            raise ValueError("`cand_indptr` must have `n_rows + 1` entries")
+        keep += [cand_indptr, cand_indices]
+        q = _lib.Query()
+        q.flags = _lib.Q_INPUTS_ON_DEVICE
+        if subjects is not None:
+            subjects = device_tensor("subjects", subjects, (torch.float32, torch.float16, torch.bfloat16))
+            if subjects.ndim != 2 or subjects.shape[1] != self.d:
+                raise ValueError("subject and object factors must have the same number of columns")
+            q.subjects = subjects.data_ptr()
+            q.subject_dtype = {torch.float32: _lib.DT_F32, torch.float16: _lib.DT_F16, torch.bfloat16: _lib.DT_BF16}[subjects.dtype]
+            keep.append(subjects)
+        if subject_ids is not None:
+            subject_ids = device_tensor("subject_ids", subject_ids, (torch.int64,)).reshape(-1)
+            if len(subject_ids) != n_rows:
+                raise ValueError("`subject_ids` must have one entry per candidate row")
+            q.subject_ids = subject_ids.data_ptr()
+            q.n_subjects_total = 0 if subjects is None else subjects.shape[0]
+            keep.append(subject_ids)
+        elif subjects is None:
+            raise ValueError("either subjects or subject_ids is required")
+        elif subjects.shape[0] != n_rows:
+            raise ValueError("`subjects` must have one row per candidate row")
+        q.n_rows = n_rows
+        if indptr is not None:
+            indptr = device_tensor("indptr", indptr, (torch.int64,)).reshape(-1)
+            if len(indptr) != n_rows + 1:
+                raise ValueError("Number of rows in `filter_pairs_csr` must be equal to `len(sublect_ids)`")
+            indices = device_tensor("indices", indices if indices is not None else torch.empty(0, dtype=torch.int32, device=dev),
+                                    (torch.int32,)).reshape(-1)
+            q.csr_indptr, q.csr_indices = indptr.data_ptr(), indices.data_ptr()
+            keep += [indptr, indices]
+        q.k = int(k)
+        k_out = max(0, min(int(k), self.n_objects))
+        if out is None:
+            out = (
+                torch.empty((n_rows, k_out), dtype=torch.int32, device=dev),
+                torch.empty((n_rows, k_out), dtype=torch.float32, device=dev),
+                torch.zeros(n_rows, dtype=torch.int32, device=dev),
+            )
+        if check_candidate_outputs(out, n_rows, k_out, dev):
+            q.flags |= _lib.Q_OUTPUTS_ON_DEVICE
+            q.out_ids, q.out_scores, q.out_counts = (a.data_ptr() for a in out)
+        else:
+            self._host_outputs(q, n_rows, k_out, out)
+        # what the engine takes on trust from device arrays, checked here in one device -> host read: the lists and the
+        # filter stay inside their index arrays, the subject ids inside their matrix
+        if n_rows > 0:
+            n_sub = subjects.shape[0] if subjects is not None else getattr(self, "n_resident_subjects", None)
+            bad = [cand_indptr[-1] > len(cand_indices)]
+            if subject_ids is not None and n_sub is not None:
+                bad.append(((subject_ids < 0) | (subject_ids >= n_sub)).any())
+            if indptr is not None:
+                bad.append((indptr[0] < 0) | (indptr[1:] < indptr[:-1]).any() | (indptr[-1] > len(indices)))
+            bad = torch.stack(bad).cpu().tolist()
+            if bad[0]:
+                raise ValueError("`cand_indptr[-1]` exceeds the length of `cand_indices`")
+            if subject_ids is not None and n_sub is not None and bad[1]:
+                raise IndexError("subject id out of range")
+            if indptr is not None and bad[-1]:
+                raise ValueError("the filter's `indptr` must be non-negative, monotone and within `indices`")
+        q.stream = stream if isinstance(stream, int) else (stream or torch.cuda.current_stream(dev)).cuda_stream
+        st = _lib.Stats()
+        _lib.check(self._lib.b200_rank_topk_candidates_device(self._h, C.byref(q), cand_indptr.data_ptr(), cand_indices.data_ptr(), C.byref(st)))
+        self.last_stats = st.as_dict()
+        del keep
+        return tuple(out)
 
     @staticmethod
     def _host_outputs(
@@ -518,6 +622,11 @@ class EngineGroup(Engine):
             "candidate sets are ranked by single engines: an engine group has no candidate-set export yet (use one device)"
         )
 
+    def topk_candidates_device(self, *args: tp.Any, **kwargs: tp.Any) -> tp.Tuple[tp.Any, tp.Any, tp.Any]:
+        raise NotImplementedError(
+            "candidate sets are ranked by single engines: an engine group has no candidate-set export yet (use one device)"
+        )
+
 
 Devices = tp.Union[int, str, tp.Sequence[int]]
 
@@ -602,6 +711,29 @@ def rank_object_rows_padded(
         return target_ids, z.astype(np.int32), z.astype(np.float32), np.zeros(len(target_ids), np.int32)
     ids, scores, counts = engine.topk(k, object_rows=target_ids, indptr=indptr, indices=indices, whitelist=whitelist)
     return target_ids, ids, scores, counts
+
+
+def check_candidate_outputs(out: tp.Sequence[tp.Any], n_rows: int, k_out: int, dev: tp.Any) -> bool:
+    """The `out` triplet of `Engine.topk_candidates_device`: `(ids int32 [n_rows, k_out], scores fp32 [n_rows, k_out],
+    counts int32 [n_rows])`, all numpy arrays (host outputs: False) or all contiguous CUDA tensors on `dev` (True).  A
+    wrong type, dtype or shape raises before the engine could write past the caller's buffers."""
+    if len(out) != 3:
+        raise ValueError("`out` must be (ids, scores, counts)")
+    shapes = ((n_rows, k_out), (n_rows, k_out), (n_rows,))
+    for name, a, shape, dtype in zip(("ids", "scores", "counts"), out, shapes, ("int32", "float32", "int32")):
+        if not (isinstance(a, np.ndarray) or hasattr(a, "data_ptr")):
+            raise TypeError(f"`out` {name}: a numpy array or a CUDA tensor, not {type(a).__name__}")
+        if str(a.dtype).replace("torch.", "") != dtype:
+            raise TypeError(f"`out` {name} must be {dtype}, not {a.dtype}")
+        if tuple(a.shape) != shape:
+            raise ValueError(f"`out` {name} must have shape {shape}, not {tuple(a.shape)}")
+    if all(isinstance(a, np.ndarray) for a in out):
+        if not all(a.flags.c_contiguous for a in out):
+            raise ValueError("`out` numpy arrays must be C-contiguous")
+        return False
+    if all(_is_cuda_tensor(a) and a.device == dev and a.is_contiguous() for a in out):
+        return True
+    raise TypeError(f"`out` must be three numpy arrays or three contiguous CUDA tensors on {dev}")
 
 
 def normalize_candidates(
@@ -928,6 +1060,98 @@ class B200Ranker:
             subject_ids, candidates_csr, k, filter_pairs_csr, sorted_object_whitelist
         )
         return self._final_scores(*flatten_padded(subject_ids, ids, scores, counts))
+
+    def rank_candidates_device(
+        self,
+        subject_ids: tp.Any,
+        candidates: tp.Any,
+        k: tp.Optional[int] = None,
+        filter_pairs_csr: tp.Any = None,
+        sorted_object_whitelist: tp.Optional[np.ndarray] = None,
+    ) -> tp.Tuple[tp.Any, tp.Any, tp.Any]:
+        """`rank_candidates` for candidates a GPU stage produced, with no host round trip: `candidates` is a CUDA int32 /
+        int64 tensor [len(subject_ids), m] on the engine's device, row r = subject r's candidate ids in any order, repeats
+        allowed, negative entries meaning "no candidate" (an entry >= n_objects raises ValueError).  `subject_ids`: numpy or
+        CUDA.  `filter_pairs_csr`: a scipy CSR matrix or a CUDA `torch.sparse_csr_tensor` (column ids sorted within each
+        row).  The whitelist is masked into the lists on the device.  `k = None`: m.
+        Returns CUDA tensors `(ids [n, k_out] int32, scores [n, k_out], counts [n] int32)`, padded as
+        `rank_candidates_padded` pads them and post-scaled as `rank_candidates` scales them: flattened (the first counts[r]
+        entries of each row), they are bit for bit what `rank_candidates` returns for the same lists."""
+        import torch
+
+        if self._subjects_csr is not None:
+            raise NotImplementedError("sparse (CSR) subjects are not ranked against candidate sets")
+        if isinstance(self.engine, EngineGroup):
+            raise NotImplementedError(
+                "candidate sets are ranked by single engines: an engine group has no candidate-set export yet (use one device)"
+            )
+        dev = torch.device("cuda", self.engine.device)
+        if not _is_cuda_tensor(candidates) or candidates.device != dev or candidates.ndim != 2:
+            raise TypeError(f"`candidates` must be a 2-dimensional CUDA tensor on {dev}")
+        if candidates.dtype not in (torch.int32, torch.int64):
+            raise TypeError(f"`candidates` must be int32 or int64, not {candidates.dtype}")
+        n, m = int(candidates.shape[0]), int(candidates.shape[1])
+        sids = subject_ids if _is_cuda_tensor(subject_ids) else torch.from_numpy(np.asarray(subject_ids, dtype=np.int64).reshape(-1))
+        sids = sids.to(device=dev, dtype=torch.int64).reshape(-1).contiguous()
+        if len(sids) != n:
+            raise ValueError("Number of rows in `candidates` must be equal to `len(subject_ids)`")
+        if n and bool(((sids < 0) | (sids >= self.n_subjects)).any()):
+            raise IndexError("subject id out of range")
+        if filter_pairs_csr is not None and filter_pairs_csr.shape[0] != n:
+            raise ValueError("Number of rows in `filter_pairs_csr` must be equal to `len(sublect_ids)`")
+        whitelist = None
+        if sorted_object_whitelist is not None:
+            whitelist = np.asarray(sorted_object_whitelist, dtype=np.int64).reshape(-1)
+            check_whitelist(whitelist, self.n_objects)
+        if k is None:
+            k = m
+        if k <= 0:
+            if m == 0:
+                z = torch.empty((n, 0), device=dev)
+                return z.to(torch.int32), z, torch.zeros(n, dtype=torch.int32, device=dev)
+            raise ValueError("`k` must be positive")
+        if n and bool((candidates >= self.n_objects).any()):
+            raise ValueError(f"Candidate object ids in `candidates` must be in [0, {self.n_objects}) (the objects of the ranker)")
+        cand = torch.where(candidates < 0, -1, candidates).to(torch.int32)  # (no int64 negative wraps to an id)
+        if whitelist is not None:
+            cand = torch.where(torch.isin(cand, torch.from_numpy(whitelist.astype(np.int32)).to(dev)), cand, -1)
+        cand_indptr = torch.arange(n + 1, dtype=torch.int64, device=dev) * m
+        indptr = indices = None
+        if filter_pairs_csr is not None:
+            if _is_cuda_tensor(filter_pairs_csr):
+                indptr = filter_pairs_csr.crow_indices().to(torch.int64)
+                indices = filter_pairs_csr.col_indices().to(torch.int32)
+            else:
+                csr = filter_pairs_csr if sparse.isspmatrix_csr(filter_pairs_csr) else sparse.csr_matrix(filter_pairs_csr)
+                if not csr.has_sorted_indices:
+                    csr = csr.sorted_indices()
+                indptr = torch.from_numpy(np.asarray(csr.indptr, dtype=np.int64)).to(dev)
+                indices = torch.from_numpy(np.asarray(csr.indices, dtype=np.int32)).to(dev)
+        if getattr(self, "_subjects", None) is not None and self.engine.subjects_owner is not self:
+            self.engine.set_subjects(self._subjects, key=self._subjects_key, owner=self)
+        ids, scores, counts = self.engine.topk_candidates_device(
+            k, cand_indptr, cand.reshape(-1), subject_ids=sids, indptr=indptr, indices=indices
+        )
+        self.last_stats = self.engine.last_stats
+        # the sentinel tail (strip_sentinel_tail): rows are best first, so the kept entries are those above it
+        pos = torch.arange(ids.shape[1], device=dev)[None, :]
+        kept = (pos < counts[:, None].long()) & (scores > float(_NEGINF_SCORE))
+        counts = kept.sum(dim=1, dtype=torch.int32)
+        ids = torch.where(kept, ids, -1)
+        scores = torch.where(kept, scores, -float(np.finfo(np.float32).max))
+        # the post-scaling of _final_scores, in the dtypes of its numpy arrays (uploaded once per ranker)
+        if self.distance in (Distance.COSINE, Distance.EUCLIDEAN):
+            post = getattr(self, "_post_device", None)
+            if post is None or post.device != dev:
+                host = self.subjects_norms if self.distance == Distance.COSINE else self.subjects_dots
+                post = self._post_device = torch.from_numpy(np.ascontiguousarray(host)).to(dev)
+            per_row = post[sids][:, None]
+            if self.distance == Distance.COSINE:
+                scaled = scores / per_row
+            else:
+                scaled = torch.sqrt(torch.clamp_min(per_row - scores, 0)).to(torch.float32)
+            scores = torch.where(kept, scaled, scores.to(scaled.dtype))
+        return ids, scores, counts
 
     def _final_scores(
         self, all_subjects: np.ndarray, all_ids: np.ndarray, all_scores: np.ndarray
