@@ -147,7 +147,8 @@ typedef struct b200_rank_stats {
                               * problem below the tiny-problem size, B200_Q_FORCE_EXACT, B200_WIDE=0, or an expected candidate count
                               * above half the catalogue): exhaustive scores materialised once + selection passes, 4 = stored
                               * rows (object_rows): one radix-select launch per row chunk over the rows in place, 5 = candidate
-                              * sets (b200_rank_topk_candidates): ms_main = scoring, ms_select = selection */
+                              * sets (b200_rank_topk_candidates): ms_main = scoring, ms_select = selection, 6 = scored pairs
+                              * (b200_rank_topk_pairs) */
     int32_t tc_dtype;        /* B200_TC_FP16 / B200_TC_BF16 when path == 1 */
     int32_t k_out;           /* columns of the output arrays */
     int32_t k_cand;          /* candidates kept per row and item split by the tensor-core pass */
@@ -261,6 +262,31 @@ int b200_rank_topk_candidates_device(b200_rank_engine* engine, const b200_rank_q
                                      const int64_t* cand_indptr,  /* device, [n_rows + 1] */
                                      const int32_t* cand_indices, /* device, object ids in any order */
                                      b200_rank_stats* stats /* nullable */);
+
+/* Scored pairs (stats.path = 6; no engine, no catalogue): the k best rows of each group, as `Reranker.recommend`
+ * (rectools/models/ranking/candidate_ranking.py:203-236) keeps the k best scored pairs of each user.
+ *   group_codes [n] int64: row i belongs to group group_codes[i] in [0, n_groups); -1 drops the row.
+ *   scores      [n] of score_type (B200_PAIRS_*): float64 is ordered as float64, float32 as float32 (widened exactly),
+ *               int64 / int32 exactly.  Floats: -0 equals +0, +-inf are ordinary values, NaN ranks below -inf (and is
+ *               returned when a group has fewer than k other rows).
+ *   Order within a group: score descending, ties by input position ascending.
+ *   out_offsets [n_groups + 1]: group g's rows are out_pos[out_offsets[g] .. out_offsets[g+1]), min(k, its row count)
+ *               input positions in order; out_pos holds min(n_valid, n_groups * k) entries at most.
+ * B200_Q_INPUTS_ON_DEVICE: group_codes / scores are device memory of `device`; B200_Q_OUTPUTS_ON_DEVICE: out_pos /
+ * out_offsets are.  The call is ordered after the work queued on `stream` (NULL: the legacy default stream), and that
+ * stream waits for device outputs.  Scratch is allocated per call and freed before it returns.
+ * Refused, with every output untouched:
+ *   B200_E_INVALID  n or n_groups < 0, k < 1, an unknown score type or flag, NULL arrays, a code outside [-1, n_groups)
+ *   B200_E_NOMEM    a failed scratch allocation.
+ * stats: ms_main = order keys and grouping, ms_select = the per-group selection; n_chunks = 1. */
+#define B200_PAIRS_F64 0
+#define B200_PAIRS_F32 1
+#define B200_PAIRS_I64 2
+#define B200_PAIRS_I32 3
+
+int b200_rank_topk_pairs(int32_t device, void* stream, int64_t n, const int64_t* group_codes, const void* scores,
+                         int32_t score_type, int64_t n_groups, int32_t k, int32_t flags, int64_t* out_pos,
+                         int64_t* out_offsets, b200_rank_stats* stats /* nullable */);
 
 /* Merge `n_lists` per-shard results (device pointers, each [n_rows, k] / [n_rows], list l at base + l * stride) into
  * the global top-k ordered by (score desc, id asc).  Runs on `stream` of `device`. */

@@ -17,6 +17,7 @@ TC_AUTO, TC_FP16, TC_BF16, TC_OFF = 0, 1, 2, 3
 F_OBJECTS_ON_DEVICE, F_OBJECTS_16BIT = 1, 2
 Q_INPUTS_ON_DEVICE, Q_OUTPUTS_ON_DEVICE, Q_FORCE_EXACT, Q_FORCE_TC, Q_SHARED_THRESHOLDS = 1, 2, 4, 8, 16
 DT_F32, DT_F16, DT_BF16 = 0, 1, 2
+PAIRS_F64, PAIRS_F32, PAIRS_I64, PAIRS_I32 = 0, 1, 2, 3
 
 EXPORTS = (
     "b200_rank_create",
@@ -30,6 +31,7 @@ EXPORTS = (
     "b200_rank_get_info",
     "b200_rank_merge",
     "b200_rank_merge_certified",
+    "b200_rank_topk_pairs",
     "b200_rank_peer_export",
     "b200_rank_peer_import",
     "b200_rank_get_snapshot",
@@ -187,6 +189,8 @@ def load() -> C.CDLL:
     lib.b200_rank_merge.argtypes = [i32, vp, i32, i64, i32, vp, vp, vp, vp, vp, vp]
     lib.b200_rank_merge_certified.restype = C.c_int
     lib.b200_rank_merge_certified.argtypes = [i32, vp, i32, i64, i32, vp, vp, vp, vp, i64, vp, vp, vp, vp, vp]
+    lib.b200_rank_topk_pairs.restype = C.c_int
+    lib.b200_rank_topk_pairs.argtypes = [i32, vp, i64, vp, vp, i32, i64, i32, i32, vp, vp, C.POINTER(Stats)]
     lib.b200_rank_peer_export.restype = C.c_int
     lib.b200_rank_peer_export.argtypes = [vp, i64, vp]
     lib.b200_rank_peer_import.restype = C.c_int

@@ -160,6 +160,7 @@ class B200TorchRanker(B200Ranker):
 _ORIGINALS: tp.Dict[str, tp.Any] = {}
 _FAST_KEY = "VectorModel.recommend"
 _EASE_I2I_KEY = "EASEModel._recommend_i2i"
+_RERANK_KEY = "Reranker.recommend"
 
 
 def ease_recommend_i2i(self, target_ids, dataset, k, sorted_item_ids_to_recommend):
@@ -179,7 +180,7 @@ def ease_recommend_i2i(self, target_ids, dataset, k, sorted_item_ids_to_recommen
     return flatten_padded(target_ids, ids, scores, counts)
 
 
-def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = True) -> None:
+def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = True, rerank: bool = False) -> None:
     """Route `VectorModel` (ALS / PureSVD / LightFM / BPR / DSSM) and `EASEModel` ranking (u2i and i2i) through the B200
     engine.
 
@@ -189,7 +190,11 @@ def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = T
 
     `fast_recommend`: also give `VectorModel` the vectorised `recommend()` of `rectools_b200.recommend` (cached viewed-items
     CSR, id maps by array indexing, no per-user Python loop); warm / cold targets and context models still go through
-    `ModelBase.recommend` (rectools/models/base.py:385-519)."""
+    `ModelBase.recommend` (rectools/models/base.py:385-519).
+
+    `rerank`: also rebind the classmethod `Reranker.recommend` (rectools/models/ranking/candidate_ranking.py:203-236), the
+    per-user top-k that ends `CandidateRankingModel.recommend`, to `rectools_b200.rerank.reranker_recommend` on the home
+    device (`device`, or its first entry)."""
     import importlib
 
     B200ImplicitRanker.default_device = parse_devices(device)
@@ -227,6 +232,18 @@ def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = T
         _ORIGINALS[_FAST_KEY] = (VectorModel.__dict__.get("recommend"), VectorModel.__dict__.get("recommend_to_items"))
         VectorModel.recommend = _recommend
         VectorModel.recommend_to_items = _recommend_to_items
+    if rerank and _RERANK_KEY not in _ORIGINALS:
+        from rectools.models.ranking.candidate_ranking import Reranker
+
+        from .rerank import reranker_recommend
+
+        def _rerank_recommend(cls, scored_pairs, k, add_rank_col=True):  # pylint: disable=unused-argument
+            home = B200ImplicitRanker.default_device
+            return reranker_recommend(scored_pairs, k, add_rank_col, device=home[0] if isinstance(home, tuple) else home)
+
+        _rerank_recommend.__doc__ = Reranker.recommend.__doc__
+        _ORIGINALS[_RERANK_KEY] = Reranker.__dict__["recommend"]
+        Reranker.recommend = classmethod(_rerank_recommend)
 
 
 def uninstall() -> None:
@@ -240,6 +257,10 @@ def uninstall() -> None:
                 delattr(VectorModel, name)
             else:
                 setattr(VectorModel, name, orig)
+    if _RERANK_KEY in _ORIGINALS:
+        from rectools.models.ranking.candidate_ranking import Reranker
+
+        Reranker.recommend = _ORIGINALS.pop(_RERANK_KEY)
     if _EASE_I2I_KEY in _ORIGINALS:
         from rectools.models.ease import EASEModel
 
