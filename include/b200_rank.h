@@ -148,7 +148,7 @@ typedef struct b200_rank_stats {
                               * above half the catalogue): exhaustive scores materialised once + selection passes, 4 = stored
                               * rows (object_rows): one radix-select launch per row chunk over the rows in place, 5 = candidate
                               * sets (b200_rank_topk_candidates): ms_main = scoring, ms_select = selection, 6 = scored pairs
-                              * (b200_rank_topk_pairs) */
+                              * (b200_rank_topk_pairs), 7 = a shared list minus viewed ids (b200_rank_topk_list) */
     int32_t tc_dtype;        /* B200_TC_FP16 / B200_TC_BF16 when path == 1 */
     int32_t k_out;           /* columns of the output arrays */
     int32_t k_cand;          /* candidates kept per row and item split by the tensor-core pass */
@@ -287,6 +287,30 @@ int b200_rank_topk_candidates_device(b200_rank_engine* engine, const b200_rank_q
 int b200_rank_topk_pairs(int32_t device, void* stream, int64_t n, const int64_t* group_codes, const void* scores,
                          int32_t score_type, int64_t n_groups, int32_t k, int32_t flags, int64_t* out_pos,
                          int64_t* out_offsets, b200_rank_stats* stats /* nullable */);
+
+/* A shared list minus viewed ids (stats.path = 7; no engine, no catalogue): for each row, the first k entries of one
+ * ordered list that the row has not viewed, as `PopularModel._recommend_u2i` (rectools/models/popular.py:229-277) takes
+ * them from the popularity list for each user.
+ *   list_ids   [n_list] int32 ids >= 0, in list order, shared by every row.
+ *   csr_*      row r's viewed ids are csr_indices[csr_indptr[r] .. csr_indptr[r+1]), ascending within the row, repeats
+ *              allowed, any int32 value (an id not in the list changes nothing).  csr_indptr NULL: nothing viewed.
+ *   Row r keeps the positions p < min(n_list, k + m_r), ascending, whose list_ids[p] it has not viewed (m_r = the row's
+ *   viewed count, the reference's window; with distinct list ids this is every unviewed position), and of them the first
+ *   min(k, their count).
+ *   out_pos    [n_rows, k_out] with k_out = min(k, n_list): list positions, unfilled slots -1; out_counts [n_rows]: the
+ *              kept count.  Positions, not ids, so the caller gathers its own ids and scores of the list in their types.
+ * Host buffers only.  Rows are ranked in chunks of whole rows within 1 GiB of device memory (8 B + 4 B per viewed id +
+ * 4 B x (k_out + 1) per row; B200_LIST_CHUNK_ROWS=n caps a chunk's rows), on a stream the call creates and destroys.
+ * n_rows = 0 or n_list = 0 writes the counts (0) without touching the device.
+ * Refused, with every output untouched:
+ *   B200_E_INVALID  n_list or n_rows < 0, n_list > 2^31 - 1, k < 1, NULL arrays that have entries (out_pos when
+ *                   k_out = 0 and csr_indices when no row has an entry may be NULL), a negative list id, csr_indptr[0] != 0,
+ *                   csr_indptr not monotone, viewed ids not ascending within a row;
+ *   B200_E_NOMEM    a row that alone needs more than a chunk's 1 GiB, or a failed device allocation.
+ * stats: ms_main = the selection kernels, ms_h2d / ms_d2h = the copies, summed over chunks; ms_total = their sum. */
+int b200_rank_topk_list(int32_t device, int64_t n_list, const int32_t* list_ids, int64_t n_rows, const int64_t* csr_indptr,
+                        const int32_t* csr_indices, int32_t k, int32_t* out_pos, int32_t* out_counts,
+                        b200_rank_stats* stats /* nullable */);
 
 /* Merge `n_lists` per-shard results (device pointers, each [n_rows, k] / [n_rows], list l at base + l * stride) into
  * the global top-k ordered by (score desc, id asc).  Runs on `stream` of `device`. */

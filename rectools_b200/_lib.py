@@ -32,6 +32,7 @@ EXPORTS = (
     "b200_rank_merge",
     "b200_rank_merge_certified",
     "b200_rank_topk_pairs",
+    "b200_rank_topk_list",
     "b200_rank_peer_export",
     "b200_rank_peer_import",
     "b200_rank_get_snapshot",
@@ -191,6 +192,8 @@ def load() -> C.CDLL:
     lib.b200_rank_merge_certified.argtypes = [i32, vp, i32, i64, i32, vp, vp, vp, vp, i64, vp, vp, vp, vp, vp]
     lib.b200_rank_topk_pairs.restype = C.c_int
     lib.b200_rank_topk_pairs.argtypes = [i32, vp, i64, vp, vp, i32, i64, i32, i32, vp, vp, C.POINTER(Stats)]
+    lib.b200_rank_topk_list.restype = C.c_int
+    lib.b200_rank_topk_list.argtypes = [i32, i64, vp, i64, vp, vp, i32, vp, vp, C.POINTER(Stats)]
     lib.b200_rank_peer_export.restype = C.c_int
     lib.b200_rank_peer_export.argtypes = [vp, i64, vp]
     lib.b200_rank_peer_import.restype = C.c_int

@@ -161,6 +161,7 @@ _ORIGINALS: tp.Dict[str, tp.Any] = {}
 _FAST_KEY = "VectorModel.recommend"
 _EASE_I2I_KEY = "EASEModel._recommend_i2i"
 _RERANK_KEY = "Reranker.recommend"
+_POPULAR_KEY = "PopularModel._recommend_u2i"
 
 
 def ease_recommend_i2i(self, target_ids, dataset, k, sorted_item_ids_to_recommend):
@@ -180,7 +181,8 @@ def ease_recommend_i2i(self, target_ids, dataset, k, sorted_item_ids_to_recommen
     return flatten_padded(target_ids, ids, scores, counts)
 
 
-def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = True, rerank: bool = False) -> None:
+def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = True, rerank: bool = False,
+            popular: bool = False) -> None:
     """Route `VectorModel` (ALS / PureSVD / LightFM / BPR / DSSM) and `EASEModel` ranking (u2i and i2i) through the B200
     engine.
 
@@ -194,7 +196,11 @@ def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = T
 
     `rerank`: also rebind the classmethod `Reranker.recommend` (rectools/models/ranking/candidate_ranking.py:203-236), the
     per-user top-k that ends `CandidateRankingModel.recommend`, to `rectools_b200.rerank.reranker_recommend` on the home
-    device (`device`, or its first entry)."""
+    device (`device`, or its first entry).
+
+    `popular`: also rebind `PopularModel._recommend_u2i` (rectools/models/popular.py:229-255), the per-user loop over the
+    popularity list, to `rectools_b200.popular.popular_recommend_u2i` on the home device.  `PopularInCategoryModel` ranks
+    through its per-category `PopularModel`s, so it is served as well."""
     import importlib
 
     B200ImplicitRanker.default_device = parse_devices(device)
@@ -244,6 +250,19 @@ def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = T
         _rerank_recommend.__doc__ = Reranker.recommend.__doc__
         _ORIGINALS[_RERANK_KEY] = Reranker.__dict__["recommend"]
         Reranker.recommend = classmethod(_rerank_recommend)
+    if popular and _POPULAR_KEY not in _ORIGINALS:
+        from rectools.models.popular import PopularModel
+
+        from .popular import popular_recommend_u2i
+
+        def _popular_recommend_u2i(self, user_ids, dataset, k, filter_viewed, sorted_item_ids_to_recommend):
+            home = B200ImplicitRanker.default_device
+            return popular_recommend_u2i(self, user_ids, dataset, k, filter_viewed, sorted_item_ids_to_recommend,
+                                         device=home[0] if isinstance(home, tuple) else home)
+
+        _popular_recommend_u2i.__doc__ = PopularModel._recommend_u2i.__doc__  # pylint: disable=protected-access
+        _ORIGINALS[_POPULAR_KEY] = PopularModel.__dict__["_recommend_u2i"]
+        PopularModel._recommend_u2i = _popular_recommend_u2i  # pylint: disable=protected-access
 
 
 def uninstall() -> None:
@@ -261,6 +280,10 @@ def uninstall() -> None:
         from rectools.models.ranking.candidate_ranking import Reranker
 
         Reranker.recommend = _ORIGINALS.pop(_RERANK_KEY)
+    if _POPULAR_KEY in _ORIGINALS:
+        from rectools.models.popular import PopularModel
+
+        PopularModel._recommend_u2i = _ORIGINALS.pop(_POPULAR_KEY)  # pylint: disable=protected-access
     if _EASE_I2I_KEY in _ORIGINALS:
         from rectools.models.ease import EASEModel
 
