@@ -8,7 +8,9 @@ Seams (SURVEY.md section 8b):
     ->  `install()` rebinds it to `ease_recommend_i2i`, which ranks those rows where the u2i engine already holds them.
   * transformer models take `similarity_module_type` (rectools/models/nn/transformers/base.py:219, :423); their
     `DistanceSimilarityModule._recommend_u2i` builds a `TorchRanker` (rectools/models/nn/transformers/similarity.py:127-132)
-    ->  `make_similarity_module()` returns a subclass that builds a `B200TorchRanker` instead.
+    ->  `make_similarity_module()` returns a subclass that builds a `B200TorchRanker` instead, and
+    `install(transformers=True)` rebinds the module-level `TorchRanker` of similarity.py and of lightning.py (item-to-item,
+    `TransformerLightningModule._recommend_i2i`, lightning.py:428-449) for the stock module.
 """
 from __future__ import annotations
 
@@ -22,7 +24,8 @@ import numpy as np
 from scipy import sparse
 
 from .ranker import (
-    B200Ranker, Devices, Distance, Engine, _as_distance, _dense_f32, flatten_padded, new_engine, parse_devices, rank_object_rows_padded,
+    B200Ranker, Devices, Distance, Engine, _as_distance, _dense_f32, _is_cuda_tensor, flatten_padded, new_engine, parse_devices,
+    rank_object_rows_padded,
 )
 
 _ENGINE_CACHE: "tp.Dict[tp.Tuple, Engine]" = {}
@@ -136,7 +139,10 @@ class B200TorchRanker(B200Ranker):
     device is its home device.
 
     `keep_16bit` (not in the reference): fp16 / bf16 `objects_factors` stay at 16 bits in the engine, read in place with
-    no fp32 master copy (the ranker keeps the tensor alive); False widens them into an fp32 copy.  Same results."""
+    no fp32 master copy (the ranker keeps the tensor alive); False widens them into an fp32 copy.  Same results.
+
+    One CUDA tensor passed as both factors (item-to-item, lightning.py:440-442) takes the identity route of `B200Ranker`:
+    no copy of the catalogue; each call gathers its target rows in their own dtype.  Same results as a copy."""
 
     def __init__(self, distance, device, subjects_factors, objects_factors, batch_size: int = 128, dtype=None,
                  devices: tp.Optional[Devices] = None, keep_16bit: bool = True) -> None:
@@ -157,11 +163,34 @@ class B200TorchRanker(B200Ranker):
         return super().rank(subject_ids, k, filter_pairs_csr, sorted_object_whitelist)
 
 
-_ORIGINALS: tp.Dict[str, tp.Any] = {}
+_ORIGINALS: tp.Dict[tp.Any, tp.Any] = {}  # (name, module) tuples: rebound module-level names
 _FAST_KEY = "VectorModel.recommend"
 _EASE_I2I_KEY = "EASEModel._recommend_i2i"
 _RERANK_KEY = "Reranker.recommend"
 _POPULAR_KEY = "PopularModel._recommend_u2i"
+# the transformer modules whose module-level `TorchRanker` ranks: u2i (`DistanceSimilarityModule._recommend_u2i`,
+# similarity.py:127-132) and i2i (`TransformerLightningModule._recommend_i2i`, lightning.py:440-442)
+_TRANSFORMER_MODULES = ("rectools.models.nn.transformers.similarity", "rectools.models.nn.transformers.lightning")
+
+
+def transformer_ranker(ranker_factory: tp.Callable[..., tp.Any] = B200TorchRanker) -> tp.Callable[..., tp.Any]:
+    """The `TorchRanker` stand-in `install(transformers=True)` binds: `ranker_factory` (a `TorchRanker`-signature class)
+    on the device of `objects_factors`, as `TorchRanker` ranks (rank_torch.py:135).  When `install(device=...)` named a group
+    that contains that device, the group ranks, with that device as home (`devices=`); host factors rank on the installed
+    device."""
+
+    def make(distance, device, subjects_factors, objects_factors, *args: tp.Any, **kwargs: tp.Any) -> tp.Any:
+        installed = B200ImplicitRanker.default_device
+        target = str(objects_factors.device if _is_cuda_tensor(objects_factors) else device)
+        if target.startswith("cuda"):
+            home = int(target.split(":")[1]) if ":" in target else 0
+            if isinstance(installed, tuple) and home in installed:
+                kwargs["devices"] = installed
+        elif installed != 0:
+            kwargs["devices"] = installed
+        return ranker_factory(distance, device, subjects_factors, objects_factors, *args, **kwargs)
+
+    return make
 
 
 def ease_recommend_i2i(self, target_ids, dataset, k, sorted_item_ids_to_recommend):
@@ -182,7 +211,8 @@ def ease_recommend_i2i(self, target_ids, dataset, k, sorted_item_ids_to_recommen
 
 
 def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = True, rerank: bool = False,
-            popular: bool = False) -> None:
+            popular: bool = False, transformers: bool = False,
+            ranker_factory: tp.Optional[tp.Callable[..., tp.Any]] = None) -> None:
     """Route `VectorModel` (ALS / PureSVD / LightFM / BPR / DSSM) and `EASEModel` ranking (u2i and i2i) through the B200
     engine.
 
@@ -200,9 +230,24 @@ def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = T
 
     `popular`: also rebind `PopularModel._recommend_u2i` (rectools/models/popular.py:229-255), the per-user loop over the
     popularity list, to `rectools_b200.popular.popular_recommend_u2i` on the home device.  `PopularInCategoryModel` ranks
-    through its per-category `PopularModel`s, so it is served as well."""
+    through its per-category `PopularModel`s, so it is served as well.
+
+    `transformers`: also rebind the module-level `TorchRanker` of rectools.models.nn.transformers.similarity (u2i of
+    `DistanceSimilarityModule`) and of rectools.models.nn.transformers.lightning (item-to-item of
+    `TransformerLightningModule`) to `transformer_ranker()`: SASRec / BERT4Rec / HSTU rank on the engine with their stock
+    similarity module, so their configs stay serialisable.  Item-to-item passes one tensor as both factors, which
+    `B200TorchRanker` ranks without a copy of the catalogue.  Needs `pytorch_lightning` (an ImportError names what is
+    missing, and nothing is rebound).  `ranker_factory`: another `TorchRanker`-signature class to bind (the CPU tests plug an
+    oracle-backed stand-in in; default `B200TorchRanker`)."""
     import importlib
 
+    transformer_modules = []
+    if transformers:
+        for modname in _TRANSFORMER_MODULES:
+            try:
+                transformer_modules.append(importlib.import_module(modname))
+            except ImportError as e:
+                raise ImportError(f"install(transformers=True) needs the package {e.name!r} to import {modname}: {e}", name=e.name) from e
     B200ImplicitRanker.default_device = parse_devices(device)
     B200ImplicitRanker.default_tc_mode = tc_mode
     for modname in ("rectools.models.vector", "rectools.models.ease"):
@@ -263,11 +308,18 @@ def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = T
         _popular_recommend_u2i.__doc__ = PopularModel._recommend_u2i.__doc__  # pylint: disable=protected-access
         _ORIGINALS[_POPULAR_KEY] = PopularModel.__dict__["_recommend_u2i"]
         PopularModel._recommend_u2i = _popular_recommend_u2i  # pylint: disable=protected-access
+    if transformer_modules:
+        bound = transformer_ranker(ranker_factory or B200TorchRanker)
+        for mod in transformer_modules:
+            _ORIGINALS.setdefault(("TorchRanker", mod.__name__), mod.TorchRanker)
+            mod.TorchRanker = bound
 
 
 def uninstall() -> None:
     import importlib
 
+    for key in [k for k in _ORIGINALS if isinstance(k, tuple)]:
+        setattr(importlib.import_module(key[1]), key[0], _ORIGINALS.pop(key))
     if _FAST_KEY in _ORIGINALS:
         from rectools.models.vector import VectorModel
 

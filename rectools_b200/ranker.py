@@ -60,6 +60,15 @@ def _norms_f32(x: np.ndarray) -> np.ndarray:
     return n
 
 
+def _device_norms(x: tp.Any) -> np.ndarray:
+    """`_norms_f32` of a CUDA tensor's rows (any float type, widened exactly to fp64), as a host fp32 array."""
+    import torch
+
+    norms = torch.linalg.vector_norm(x.double(), dim=1).float()
+    norms[norms == 0] = 1e-10
+    return norms.cpu().numpy()
+
+
 def check_whitelist(whitelist: np.ndarray, n_objects: int) -> None:
     """`sorted_object_whitelist` (rank.py:39): object ids in range, strictly ascending -- the kernels merge a row's viewed ids
     against the whitelist positions in ascending order, so an unsorted whitelist would let viewed objects through."""
@@ -813,6 +822,9 @@ class B200Ranker:
     keep_16bit : fp16 / bf16 CUDA tensors and numpy fp16 object factors stay at 16 bits in the engine, with no fp32
         master copy (same results; `object_storage_dtype`).  A CUDA tensor is then read in place for the ranker's life.
         False: the engine widens them into an fp32 copy.
+
+    One CUDA tensor passed as both factors (`subjects_factors is objects_factors`, item-to-item) ranks the catalogue's own
+    rows: no copy of it is made, each `rank()` gathers its rows in their own type (`_rank_identity_padded`).
     """
 
     def __init__(
@@ -884,22 +896,28 @@ class B200Ranker:
             objects = objects.to(torch.float32)
         objects = objects.contiguous()
         dev = objects.device
-        subjects = subjects_factors
-        if sparse.issparse(subjects):
-            raise ValueError("CSR subjects need host object factors")
-        if not hasattr(subjects, "detach"):
-            subjects = torch.from_numpy(_dense_f32(subjects))
-        subjects = subjects.detach().to(device=dev, dtype=torch.float32).contiguous()
-        if subjects.shape[1] != objects.shape[1]:
-            raise ValueError("subject and object factors must have the same number of columns")
-        self.n_subjects, self.n_objects = int(subjects.shape[0]), int(objects.shape[0])
+        # item-to-item passes one tensor as both factors (rectools/models/nn/transformers/lightning.py:440-442): the
+        # subjects are the engine's own objects, so no copy of the catalogue is made; each call gathers its target rows
+        # (`_rank_identity_padded`)
+        self._identity = objects if subjects_factors is objects_factors else None
         self.subjects_norms = self.subjects_dots = None
-        if self.distance == Distance.COSINE:
-            norms = torch.linalg.vector_norm(subjects.double(), dim=1).float()
-            norms[norms == 0] = 1e-10
-            self.subjects_norms = norms.cpu().numpy()
+        if self._identity is not None:
+            self.n_subjects = self.n_objects = int(objects.shape[0])
+            self._device_tensors = (objects,)  # the engine references this memory: keep it alive
+        else:
+            subjects = subjects_factors
+            if sparse.issparse(subjects):
+                raise ValueError("CSR subjects need host object factors")
+            if not hasattr(subjects, "detach"):
+                subjects = torch.from_numpy(_dense_f32(subjects))
+            subjects = subjects.detach().to(device=dev, dtype=torch.float32).contiguous()
+            if subjects.shape[1] != objects.shape[1]:
+                raise ValueError("subject and object factors must have the same number of columns")
+            self.n_subjects, self.n_objects = int(subjects.shape[0]), int(objects.shape[0])
+            if self.distance == Distance.COSINE:
+                self.subjects_norms = _device_norms(subjects)
+            self._device_tensors = (subjects, objects)  # the engine references this memory: keep it alive
         torch.cuda.current_stream(dev).synchronize()
-        self._device_tensors = (subjects, objects)  # the engine references this memory: keep it alive
         home = dev.index or 0
         devices = parse_devices(device)
         if not isinstance(devices, int):  # a group whose home device is the tensors' device
@@ -913,9 +931,69 @@ class B200Ranker:
             objects_device_ptr=objects.data_ptr(), shape=(self.n_objects, int(objects.shape[1])), objects_dtype=dtypes[objects.dtype],
             keep_16bit=object_storage_dtype(self.distance, objects.dtype, keep_16bit) != _lib.DT_F32,
         )
-        self.engine.set_subjects_device(subjects.data_ptr(), self.n_subjects)
+        if self._identity is None:
+            self.engine.set_subjects_device(self._device_tensors[0].data_ptr(), self.n_subjects)
         self._subjects = self._subjects_key = None
         self.last_stats = {}
+
+    def _make_subjects_resident(self) -> None:
+        """Leave the identity route: an fp32 copy of the catalogue becomes the resident subjects, as for two tensors (the
+        candidate-set calls rank resident subjects by id)."""
+        if getattr(self, "_identity", None) is None:
+            return
+        import torch
+
+        objects = self._identity
+        subjects = objects.to(torch.float32).contiguous()
+        if self.distance == Distance.COSINE:
+            self.subjects_norms = _device_norms(subjects)
+        torch.cuda.current_stream(objects.device).synchronize()
+        self._device_tensors = (subjects, objects)
+        self.engine.set_subjects_device(subjects.data_ptr(), self.n_subjects)
+        self._identity = None
+
+    def _rank_identity_padded(
+        self,
+        subject_ids: np.ndarray,
+        k: int,
+        indptr: tp.Optional[np.ndarray],
+        indices: tp.Optional[np.ndarray],
+        whitelist: tp.Optional[np.ndarray],
+        flags: int,
+    ) -> tp.Tuple[np.ndarray, np.ndarray, np.ndarray, tp.Optional[np.ndarray]]:
+        """The identity route of `rank_padded`: the target rows are gathered on the device in the catalogue's own type and
+        handed to the engine as a batch of device subjects (16-bit rows are widened exactly by the engine).  Returns
+        `(ids, scores, counts, norms)`; `norms` are the fp32 COSINE norms of these rows, computed as `_device_norms` computes
+        them for resident subjects (None for DOT)."""
+        import torch
+
+        objects = self._identity
+        dev = objects.device
+        rows = objects.index_select(0, torch.from_numpy(subject_ids).to(dev))
+        norms = _device_norms(rows) if self.distance == Distance.COSINE else None
+        keep = [rows]
+        q_kw = {}
+        if whitelist is not None:
+            wl = torch.from_numpy(np.ascontiguousarray(whitelist, dtype=np.int32)).to(dev)
+            q_kw.update(whitelist=wl.data_ptr(), n_whitelist=len(wl))
+            keep.append(wl)
+        if indptr is not None:
+            ip = torch.from_numpy(np.ascontiguousarray(indptr, dtype=np.int64)).to(dev)
+            ix = torch.from_numpy(np.ascontiguousarray(indices, dtype=np.int32)).to(dev)
+            q_kw.update(indptr=ip.data_ptr(), indices=ix.data_ptr() if len(ix) else 0)
+            keep += [ip, ix]
+        n_rows = len(subject_ids)
+        k_out = min(int(k), len(whitelist) if whitelist is not None else self.n_objects)
+        ids = np.empty((n_rows, k_out), dtype=np.int32)
+        scores = np.empty((n_rows, k_out), dtype=np.float32)
+        counts = np.zeros(n_rows, dtype=np.int32)
+        dtypes = {torch.float32: _lib.DT_F32, torch.float16: _lib.DT_F16, torch.bfloat16: _lib.DT_BF16}
+        self.engine.topk_ptrs(
+            n_rows, k, ids.ctypes.data, scores.ctypes.data, counts.ctypes.data, flags | _lib.Q_INPUTS_ON_DEVICE,
+            subjects=rows.data_ptr(), subject_dtype=dtypes[rows.dtype], stream=torch.cuda.current_stream(dev).cuda_stream, **q_kw,
+        )
+        del keep
+        return ids, scores, counts, norms
 
     # ------------------------------------------------------------------------------------------------------------
     def rank_padded(
@@ -927,6 +1005,18 @@ class B200Ranker:
         flags: int = 0,
     ) -> tp.Tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
         """`rank` without the ragged flattening: `(subject_ids, ids [n,k], scores [n,k], counts [n])`."""
+        return self._rank_padded(subject_ids, k, filter_pairs_csr, sorted_object_whitelist, flags)[:4]
+
+    def _rank_padded(
+        self,
+        subject_ids: InternalIds,
+        k: tp.Optional[int] = None,
+        filter_pairs_csr: tp.Optional[sparse.csr_matrix] = None,
+        sorted_object_whitelist: tp.Optional[np.ndarray] = None,
+        flags: int = 0,
+    ) -> tp.Tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray, tp.Optional[np.ndarray]]:
+        """`rank_padded` plus the COSINE norms of the rows when the identity route computed them for this call (else None:
+        `subjects_norms` holds them)."""
         subject_ids = np.asarray(subject_ids, dtype=np.int64).reshape(-1)
         if filter_pairs_csr is not None and filter_pairs_csr.shape[0] != len(subject_ids):
             raise ValueError("Number of rows in `filter_pairs_csr` must be equal to `len(sublect_ids)`")
@@ -950,14 +1040,18 @@ class B200Ranker:
             indptr, indices = csr.indptr, csr.indices
         if n_pos == 0 or len(subject_ids) == 0:
             z = np.empty((len(subject_ids), 0))
-            return subject_ids, z.astype(np.int32), z.astype(np.float32), np.zeros(len(subject_ids), np.int32)
+            return subject_ids, z.astype(np.int32), z.astype(np.float32), np.zeros(len(subject_ids), np.int32), None
         if self._subjects_csr is not None:
             rows = self._subjects_csr[subject_ids]  # CSR row gather: cheap, stays sparse (rank_implicit.py:236)
             ids, scores, counts = self.engine.topk(
                 k, sparse_subjects=rows, indptr=indptr, indices=indices, whitelist=whitelist, flags=flags & ~_lib.Q_FORCE_TC
             )
             self.last_stats = self.engine.last_stats
-            return (subject_ids,) + strip_sentinel_tail(ids, scores, counts)
+            return (subject_ids,) + strip_sentinel_tail(ids, scores, counts) + (None,)
+        if getattr(self, "_identity", None) is not None:
+            ids, scores, counts, norms = self._rank_identity_padded(subject_ids, k, indptr, indices, whitelist, flags)
+            self.last_stats = self.engine.last_stats
+            return (subject_ids,) + strip_sentinel_tail(ids, scores, counts) + (norms,)
         if getattr(self, "_subjects", None) is not None and self.engine.subjects_owner is not self:
             # another ranker sharing this (cached) engine made its own subject factors resident in the meantime
             self.engine.set_subjects(self._subjects, key=self._subjects_key, owner=self)
@@ -965,7 +1059,7 @@ class B200Ranker:
             k, subject_ids=subject_ids, indptr=indptr, indices=indices, whitelist=whitelist, flags=flags
         )
         self.last_stats = self.engine.last_stats
-        return (subject_ids,) + strip_sentinel_tail(ids, scores, counts)
+        return (subject_ids,) + strip_sentinel_tail(ids, scores, counts) + (None,)
 
     def rank_object_rows_padded(
         self,
@@ -1015,6 +1109,7 @@ class B200Ranker:
             raise NotImplementedError(
                 "candidate sets are ranked by single engines: an engine group has no candidate-set export yet (use one device)"
             )
+        self._make_subjects_resident()
         whitelist = None
         if sorted_object_whitelist is not None:
             whitelist = np.asarray(sorted_object_whitelist, dtype=np.int64).reshape(-1)
@@ -1085,6 +1180,7 @@ class B200Ranker:
             raise NotImplementedError(
                 "candidate sets are ranked by single engines: an engine group has no candidate-set export yet (use one device)"
             )
+        self._make_subjects_resident()
         dev = torch.device("cuda", self.engine.device)
         if not _is_cuda_tensor(candidates) or candidates.device != dev or candidates.ndim != 2:
             raise TypeError(f"`candidates` must be a 2-dimensional CUDA tensor on {dev}")
@@ -1173,5 +1269,9 @@ class B200Ranker:
     ) -> tp.Tuple[InternalIds, InternalIds, Scores]:
         """Same contract as `ImplicitRanker.rank` (rank_implicit.py:187-280): flat `(subject ids repeated, object ids,
         scores)`, grouped by subject in input order, best first, filtered objects never returned."""
-        subject_ids, ids, scores, counts = self.rank_padded(subject_ids, k, filter_pairs_csr, sorted_object_whitelist)
-        return self._final_scores(*flatten_padded(subject_ids, ids, scores, counts))
+        subject_ids, ids, scores, counts, norms = self._rank_padded(subject_ids, k, filter_pairs_csr, sorted_object_whitelist)
+        flat = flatten_padded(subject_ids, ids, scores, counts)
+        if getattr(self, "_identity", None) is None:
+            return self._final_scores(*flat)
+        # identity route: COSINE divides by the norms of this call's rows, in fp32 as `_final_scores` does (no rows: None)
+        return flat if norms is None else (flat[0], flat[1], flat[2] / np.repeat(norms, counts))
