@@ -148,7 +148,8 @@ typedef struct b200_rank_stats {
                               * above half the catalogue): exhaustive scores materialised once + selection passes, 4 = stored
                               * rows (object_rows): one radix-select launch per row chunk over the rows in place, 5 = candidate
                               * sets (b200_rank_topk_candidates): ms_main = scoring, ms_select = selection, 6 = scored pairs
-                              * (b200_rank_topk_pairs), 7 = a shared list minus viewed ids (b200_rank_topk_list) */
+                              * (b200_rank_topk_pairs), 7 = a shared list minus viewed ids (b200_rank_topk_list),
+                              * 8 = per-category lists minus viewed ids, mixed (b200_rank_topk_list_mix) */
     int32_t tc_dtype;        /* B200_TC_FP16 / B200_TC_BF16 when path == 1 */
     int32_t k_out;           /* columns of the output arrays */
     int32_t k_cand;          /* candidates kept per row and item split by the tensor-core pass */
@@ -311,6 +312,41 @@ int b200_rank_topk_pairs(int32_t device, void* stream, int64_t n, const int64_t*
 int b200_rank_topk_list(int32_t device, int64_t n_list, const int32_t* list_ids, int64_t n_rows, const int64_t* csr_indptr,
                         const int32_t* csr_indices, int32_t k, int32_t* out_pos, int32_t* out_counts,
                         b200_rank_stats* stats /* nullable */);
+
+/* Per-category lists minus viewed ids, mixed (stats.path = 8; no engine, no catalogue): for each row, the recommendations
+ * `PopularInCategoryModel._recommend_u2i` (rectools/models/popular_in_category.py:333-373) makes from its category models'
+ * popularity lists.
+ *   list_offsets [n_lists + 1], list_offsets[0] = 0, monotone: list c (its priority) is
+ *                list_ids[list_offsets[c] .. list_offsets[c + 1]), int32 ids >= 0 in list order; ids may repeat across
+ *                lists.  At most 2^31 - 1 ids in all.
+ *   quota        [n_lists] >= 0, summing to at most k: entries of list c with rank < quota[c] are main, the others fallback.
+ *   mixing       B200_MIX_ROTATE or B200_MIX_GROUP.
+ *   csr_*        the viewed ids of each row, as for b200_rank_topk_list; a NULL csr_indptr: nothing viewed.
+ *   For row r, list c contributes its first min(k, n_c) unviewed positions p < min(n_c, k + m_r) (path 7's window), of
+ *   rank 0, 1, ... in list order.  Main entries in (c, rank) order, then fallback entries in (c, rank) order, keep the first
+ *   entry of each id; all main survivors are kept, and if that leaves room, the fallback survivors first in (rank, c)
+ *   order up to k in all.  The kept entries come out in (c, rank) order for B200_MIX_GROUP, and in (r', c) order for
+ *   B200_MIX_ROTATE, r' = an entry's index among the kept entries of its list.
+ *   out_pos      [n_rows, k_out] with k_out = min(k, list_offsets[n_lists]): positions into list_ids, unfilled slots -1;
+ *   out_counts   [n_rows]: the kept count.
+ * Host buffers only.  Rows are ranked in chunks of whole rows within 1 GiB of device memory (path 7's per-row bytes, plus
+ * the row's scratch when that does not fit in shared memory; B200_LIST_CHUNK_ROWS=n caps a chunk's rows), one CTA per row
+ * in one kernel launch per chunk, on a stream the call creates and destroys.
+ * n_rows = 0, n_lists = 0 or only empty lists writes the counts (0) without touching the device.
+ * Refused, with every output untouched:
+ *   B200_E_INVALID  n_lists or n_rows < 0, k < 1, an unknown mixing, list_offsets[0] != 0 or not monotone, more than
+ *                   2^31 - 1 ids, a negative list id, a negative quota or quotas summing to more than k, NULL arrays that
+ *                   have entries (list_offsets and quota may be NULL when n_lists = 0), and the CSR refusals of
+ *                   b200_rank_topk_list;
+ *   B200_E_NOMEM    a row that alone needs more than a chunk's 1 GiB, or a failed device allocation.
+ * stats: ms_main = the mixing kernels, ms_h2d / ms_d2h = the copies, summed over chunks; ms_total = their sum. */
+#define B200_MIX_ROTATE 0
+#define B200_MIX_GROUP 1
+
+int b200_rank_topk_list_mix(int32_t device, int32_t n_lists, const int64_t* list_offsets, const int32_t* list_ids,
+                            const int32_t* quota, int32_t mixing, int64_t n_rows, const int64_t* csr_indptr,
+                            const int32_t* csr_indices, int32_t k, int32_t* out_pos, int32_t* out_counts,
+                            b200_rank_stats* stats /* nullable */);
 
 /* Merge `n_lists` per-shard results (device pointers, each [n_rows, k] / [n_rows], list l at base + l * stride) into
  * the global top-k ordered by (score desc, id asc).  Runs on `stream` of `device`. */

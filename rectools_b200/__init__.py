@@ -8,6 +8,8 @@ Public surface (host-side mirror of `rectools.models.rank`):
   * `EngineGroup`                         -- one engine per GPU of the host (`device=[...]` / "all"), rows split between them
   * `rank_pairs()`, `reranker_recommend()` -- per-group top-k of scored pairs (`Reranker.recommend`, install(rerank=True))
   * `rank_list()`                         -- a shared ordered list minus each row's viewed ids (`PopularModel`, install(popular=True))
+  * `rank_list_mix()`                     -- per-category lists minus viewed ids, mixed (`PopularInCategoryModel`,
+                                             install(popular_in_category=True))
   * `ShardedB200Ranker`                   -- item-sharded multi-GPU ranking (one process per GPU, NCCL all-gather + merge)
 The CUDA library is `rectools_b200/libb200rank.so` (C ABI: include/b200_rank.h); build it with
 `python -m rectools_b200.build`.  There is no CPU fallback.
@@ -16,7 +18,7 @@ from .ranker import B200Ranker, Distance, Engine, EngineGroup, flatten_padded  #
 from .integration import B200ImplicitRanker, B200TorchRanker, install, uninstall  # noqa: F401
 from .recommend import recommend, recommend_to_items  # noqa: F401
 from .rerank import rank_pairs, reranker_recommend  # noqa: F401
-from .popular import rank_list  # noqa: F401
+from .popular import rank_list, rank_list_mix  # noqa: F401
 
 __all__ = [
     "B200Ranker",
@@ -28,6 +30,7 @@ __all__ = [
     "flatten_padded",
     "install",
     "rank_list",
+    "rank_list_mix",
     "rank_pairs",
     "recommend",
     "recommend_to_items",

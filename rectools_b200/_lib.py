@@ -18,6 +18,7 @@ F_OBJECTS_ON_DEVICE, F_OBJECTS_16BIT = 1, 2
 Q_INPUTS_ON_DEVICE, Q_OUTPUTS_ON_DEVICE, Q_FORCE_EXACT, Q_FORCE_TC, Q_SHARED_THRESHOLDS = 1, 2, 4, 8, 16
 DT_F32, DT_F16, DT_BF16 = 0, 1, 2
 PAIRS_F64, PAIRS_F32, PAIRS_I64, PAIRS_I32 = 0, 1, 2, 3
+MIX_ROTATE, MIX_GROUP = 0, 1
 
 EXPORTS = (
     "b200_rank_create",
@@ -33,6 +34,7 @@ EXPORTS = (
     "b200_rank_merge_certified",
     "b200_rank_topk_pairs",
     "b200_rank_topk_list",
+    "b200_rank_topk_list_mix",
     "b200_rank_peer_export",
     "b200_rank_peer_import",
     "b200_rank_get_snapshot",
@@ -194,6 +196,8 @@ def load() -> C.CDLL:
     lib.b200_rank_topk_pairs.argtypes = [i32, vp, i64, vp, vp, i32, i64, i32, i32, vp, vp, C.POINTER(Stats)]
     lib.b200_rank_topk_list.restype = C.c_int
     lib.b200_rank_topk_list.argtypes = [i32, i64, vp, i64, vp, vp, i32, vp, vp, C.POINTER(Stats)]
+    lib.b200_rank_topk_list_mix.restype = C.c_int
+    lib.b200_rank_topk_list_mix.argtypes = [i32, i32, vp, vp, vp, i32, i64, vp, vp, i32, vp, vp, C.POINTER(Stats)]
     lib.b200_rank_peer_export.restype = C.c_int
     lib.b200_rank_peer_export.argtypes = [vp, i64, vp]
     lib.b200_rank_peer_import.restype = C.c_int

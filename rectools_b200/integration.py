@@ -168,6 +168,7 @@ _FAST_KEY = "VectorModel.recommend"
 _EASE_I2I_KEY = "EASEModel._recommend_i2i"
 _RERANK_KEY = "Reranker.recommend"
 _POPULAR_KEY = "PopularModel._recommend_u2i"
+_POPULAR_IN_CATEGORY_KEY = "PopularInCategoryModel._recommend_u2i"
 # the transformer modules whose module-level `TorchRanker` ranks: u2i (`DistanceSimilarityModule._recommend_u2i`,
 # similarity.py:127-132) and i2i (`TransformerLightningModule._recommend_i2i`, lightning.py:440-442)
 _TRANSFORMER_MODULES = ("rectools.models.nn.transformers.similarity", "rectools.models.nn.transformers.lightning")
@@ -211,7 +212,7 @@ def ease_recommend_i2i(self, target_ids, dataset, k, sorted_item_ids_to_recommen
 
 
 def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = True, rerank: bool = False,
-            popular: bool = False, transformers: bool = False,
+            popular: bool = False, transformers: bool = False, popular_in_category: bool = False,
             ranker_factory: tp.Optional[tp.Callable[..., tp.Any]] = None) -> None:
     """Route `VectorModel` (ALS / PureSVD / LightFM / BPR / DSSM) and `EASEModel` ranking (u2i and i2i) through the B200
     engine.
@@ -231,6 +232,11 @@ def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = T
     `popular`: also rebind `PopularModel._recommend_u2i` (rectools/models/popular.py:229-255), the per-user loop over the
     popularity list, to `rectools_b200.popular.popular_recommend_u2i` on the home device.  `PopularInCategoryModel` ranks
     through its per-category `PopularModel`s, so it is served as well.
+
+    `popular_in_category`: also rebind `PopularInCategoryModel._recommend_u2i` (rectools/models/popular_in_category.py:333-373),
+    one `PopularModel` call per category and the mixing in pandas, to
+    `rectools_b200.popular.popular_in_category_recommend_u2i` on the home device: every category's list and the mixing of
+    each user in one kernel pass.  `popular=True` alone leaves this method as it is.
 
     `transformers`: also rebind the module-level `TorchRanker` of rectools.models.nn.transformers.similarity (u2i of
     `DistanceSimilarityModule`) and of rectools.models.nn.transformers.lightning (item-to-item of
@@ -308,6 +314,19 @@ def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = T
         _popular_recommend_u2i.__doc__ = PopularModel._recommend_u2i.__doc__  # pylint: disable=protected-access
         _ORIGINALS[_POPULAR_KEY] = PopularModel.__dict__["_recommend_u2i"]
         PopularModel._recommend_u2i = _popular_recommend_u2i  # pylint: disable=protected-access
+    if popular_in_category and _POPULAR_IN_CATEGORY_KEY not in _ORIGINALS:
+        from rectools.models.popular_in_category import PopularInCategoryModel
+
+        from .popular import popular_in_category_recommend_u2i
+
+        def _in_category_recommend_u2i(self, user_ids, dataset, k, filter_viewed, sorted_item_ids_to_recommend):
+            home = B200ImplicitRanker.default_device
+            return popular_in_category_recommend_u2i(self, user_ids, dataset, k, filter_viewed, sorted_item_ids_to_recommend,
+                                                     device=home[0] if isinstance(home, tuple) else home)
+
+        _in_category_recommend_u2i.__doc__ = PopularInCategoryModel._recommend_u2i.__doc__  # pylint: disable=protected-access
+        _ORIGINALS[_POPULAR_IN_CATEGORY_KEY] = PopularInCategoryModel.__dict__["_recommend_u2i"]
+        PopularInCategoryModel._recommend_u2i = _in_category_recommend_u2i  # pylint: disable=protected-access
     if transformer_modules:
         bound = transformer_ranker(ranker_factory or B200TorchRanker)
         for mod in transformer_modules:
@@ -336,6 +355,10 @@ def uninstall() -> None:
         from rectools.models.popular import PopularModel
 
         PopularModel._recommend_u2i = _ORIGINALS.pop(_POPULAR_KEY)  # pylint: disable=protected-access
+    if _POPULAR_IN_CATEGORY_KEY in _ORIGINALS:
+        from rectools.models.popular_in_category import PopularInCategoryModel
+
+        PopularInCategoryModel._recommend_u2i = _ORIGINALS.pop(_POPULAR_IN_CATEGORY_KEY)  # pylint: disable=protected-access
     if _EASE_I2I_KEY in _ORIGINALS:
         from rectools.models.ease import EASEModel
 
