@@ -1,6 +1,7 @@
 // Prints the plan of rectools_b200/csrc/plan.h for the calls read from stdin, one per line of `name=value` words:
-// the CallShape fields (n_rows n_pos k d d_pad sm_count tc_dtype n_peers flags sparse) and B200_* hooks, which are set in
-// the environment for that line only and read through read_hooks().  Built and run by tests/test_call_plan_cpu.py.
+// the CallShape fields (n_rows n_pos k d d_pad sm_count tc_dtype n_peers flags sparse rows n_objects cosine) and B200_*
+// hooks, which are set in the environment for that line only and read through read_hooks().  Built and run by
+// tests/test_call_plan_cpu.py and tests/test_call_history_cases_cpu.py.
 #include <iostream>
 #include <map>
 #include <sstream>
@@ -36,9 +37,12 @@ int main() {
         s.n_peers = (int)v["n_peers"];
         s.flags = (int32_t)v["flags"];
         s.sparse = v["sparse"] != 0;
+        s.rows = v["rows"] != 0;
+        s.n_objects = v["n_objects"];
+        s.cosine = v["cosine"] != 0;
         const b200::CallPlan p = b200::plan_call(s, b200::read_hooks());
         for (const std::string& h : hooks) unsetenv(h.c_str());
-        std::cout << "k_out=" << p.k_out << " path=" << (int)p.path << " mode=" << (int)p.mode << " nw=" << p.nw
+        std::cout << "k_out=" << p.k_out << " path=" << (int)p.path << " mode=" << (int)p.mode << " select=" << (int)p.select << " nw=" << p.nw
                   << " k_cand=" << p.k_cand << " peers=" << p.peers << " T=" << p.geom.T << " cand_stride=" << p.geom.cand_stride
                   << " chunk=" << p.chunk << " n_chunks=" << p.n_chunks << " error=" << p.error << " message=" << p.message
                   << std::endl;
