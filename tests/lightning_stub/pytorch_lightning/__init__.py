@@ -7,8 +7,10 @@ installed.  It covers exactly these calls:
 * `LightningModule`: a `torch.nn.Module` whose `save_hyperparameters` and `log` do nothing, with empty hooks
   (`on_train_start`, `on_train_end`, ...) and a `device` property;
 * `Trainer(**kwargs)`: the keyword arguments are kept and ignored except `max_epochs`.  `fit(model, train_dataloader,
-  val_dataloader=None)` calls `model.configure_optimizers()` once and then, for each of `max_epochs` epochs, every batch
-  of the loader moved to the module's device: `zero_grad`, `training_step(batch, batch_idx)`, `backward`, `step`.  The
+  val_dataloader=None)` (or Lightning's keywords `train_dataloaders=` / `val_dataloaders=`, as DSSM passes them) calls
+  `model.configure_optimizers()` once and then, for each of `max_epochs` epochs, every batch of the loader (a dict of
+  tensors, or a sequence of them) moved to the module's device: `zero_grad`, `training_step(batch, batch_idx)`,
+  `backward`, `step`.  The
   hooks `on_train_start` / `on_train_end` run around that; validation loaders are not run.  `fit_loop.max_epochs`,
   `fit_loop.min_epochs` and `fit_loop.epoch_progress.current.ready` are kept as RecTools' `fit_partial` reads and sets them;
   `fit` continues from the ready epochs;
@@ -84,6 +86,8 @@ class Trainer:
         return self.fit_loop.max_epochs
 
     def fit(self, model: LightningModule, train_dataloader: tp.Any = None, val_dataloader: tp.Any = None, **kwargs: tp.Any) -> None:  # pylint: disable=unused-argument
+        if train_dataloader is None:
+            train_dataloader = kwargs.get("train_dataloaders")
         optimizer = model.configure_optimizers()
         if isinstance(optimizer, dict):
             optimizer = optimizer["optimizer"]
@@ -95,7 +99,10 @@ class Trainer:
         progress = self.fit_loop.epoch_progress.current
         while progress.ready < self.fit_loop.max_epochs:
             for batch_idx, batch in enumerate(train_dataloader or ()):
-                batch = {k: v.to(device) if hasattr(v, "to") else v for k, v in batch.items()}
+                if isinstance(batch, dict):
+                    batch = {k: v.to(device) if hasattr(v, "to") else v for k, v in batch.items()}
+                else:
+                    batch = [v.to(device) if hasattr(v, "to") else v for v in batch]
                 optimizer.zero_grad()
                 loss = model.training_step(batch, batch_idx)
                 loss.backward()
