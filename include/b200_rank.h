@@ -169,7 +169,9 @@ typedef struct b200_rank_stats {
     int32_t epi_warps;       /* epilogue warps per CTA of the fused kernel: always 8 */
     int32_t wide;            /* 1: single-pass wide mode (24 < k <= 1024) */
     float ms_select;         /* CUDA-event time of the fp64 re-score / selection kernels */
-    int32_t reserved;
+    float ms_main_pass;      /* the part of ms_main spent in the main pass of the fused tensor-core kernel (one launch per chunk;
+                              * no second-chance or re-rank launches); 0 off path 1.  Takes the slot that was reserved: the
+                              * struct keeps its size and the fields before it their offsets */
 } b200_rank_stats;
 
 typedef struct b200_rank_info {

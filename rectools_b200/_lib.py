@@ -98,7 +98,7 @@ class Stats(C.Structure):
         ("epi_warps", C.c_int32),  # always 8 (one fused-kernel geometry)
         ("wide", C.c_int32),
         ("ms_select", C.c_float),
-        ("reserved", C.c_int32),
+        ("ms_main_pass", C.c_float),  # the main-pass launches of the fused kernel inside ms_main (path 1)
     ]
 
     def as_dict(self) -> tp.Dict[str, tp.Any]:

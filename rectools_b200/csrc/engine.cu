@@ -457,7 +457,7 @@ struct Call {
     bool wl_gathered = false;
     int n_tc = 0;       // fused-kernel launches so far
     size_t n_evt = 0;
-    std::vector<int> evt_kind;  // 0 = fused kernel, 1 = selection
+    std::vector<int> evt_kind;  // 0 = fused kernel, 1 = selection, 2 = fused kernel, main pass
 
     const float* norms() const { return E->distance == B200_DIST_COSINE ? E->obj_norms.as<float>() : nullptr; }
 
@@ -480,9 +480,10 @@ struct Call {
         for (size_t i = 0; i < n_evt; ++i) {
             float ms = 0.f;
             CK(cudaEventElapsedTime(&ms, E->evt[2 * i], E->evt[2 * i + 1]));
-            if (evt_kind[i] == 0) {
+            if (evt_kind[i] != 1) {
                 S.ms_main += ms;
                 S.n_tc_launches++;
+                if (evt_kind[i] == 2) S.ms_main_pass += ms;
             } else {
                 S.ms_select += ms;
             }
@@ -738,7 +739,7 @@ void run_tc(Call& c, const TcPass& t) {
         E->snap_fb.ensure(sizeof(int32_t) * (size_t)(c.n_rows + 2));
         CK(cudaMemcpyAsync(E->snap_fb.p, t.fb_count, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
     }
-    c.time_begin(0);
+    c.time_begin(t.main ? 2 : 0);
     fused_kernel(wide, t.peers && tp.n_peers > 0, bf16).launch(grid, pl.smem_bytes, st, tm_sub, tm_obj, tp);
     CK(cudaGetLastError());
     c.time_end();

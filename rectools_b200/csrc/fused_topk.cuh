@@ -3,7 +3,9 @@
 //   TMA (own 128 subject rows once per work item; every 256-object tile as four quarters of 64 objects, streamed through a
 //   ring of 8 KiB blocks) -> wgmma 64 x 64 x 16 (fp16 / bf16 -> fp32) into the registers of the MMA warp group
 //   -> each finished quarter [128 rows x 64 columns] is staged in shared memory, one m-half of 64 rows at a time, and
-//   read back by the epilogue warps, one row per thread; a staged half is handed back as soon as its rows are in registers
+//   read back by the epilogue warps, one row per thread; a staged half is handed back as soon as its rows are in registers.
+//   Only the 16-row slices (one MMA warp's) with a score above their row's threshold are stored: a flag per slice tells
+//   the epilogue which rows of the buffer hold the current quarter (store_half)
 //   -> threshold scan (3-input max tree), hits extracted into per-thread ring FIFOs in shared memory
 //   -> deferred, bounded steps: filter_pairs_csr lookup through a prefetched 4-entry window, candidate-list insertion.
 // Score rows never reach HBM: only the K' best (score, id) pairs per row and column group are written.
@@ -166,20 +168,50 @@ __device__ __forceinline__ void blocks_landed(uint32_t bar_full, int NS, uint32_
 
 // Hand one m-half of a finished quarter to the epilogue: wait until its two readers have taken the previous one, store
 // this thread's 32 accumulators of it, arrive on the half's `full` barrier.
-__device__ __forceinline__ void store_half(const uint32_t (&d)[32], uint32_t stg, uint32_t qempty, uint32_t parity, uint32_t qfull) {
-    mbar_wait(qempty, parity);
+// The threshold gate: the warp's 16 rows of the half are staged only if one of their 64 scores lies above that row's
+// threshold.  `thr` is the row's exchange slot of the list this quarter feeds (its column group): the list's own rs.thr
+// at some earlier tile of the same work item (the tag says which work item), hence never above the threshold the
+// epilogue scans this quarter with -- a gated row could not have produced a hit.  No other slot may be used: the other
+// list's or the peers' value can lie above anything this list ever adopts (after its last tile, say), and the list's
+// final threshold must bound every score it discarded.  A slot of another work item counts as -inf (stage).  The
+// decision is per warp (one vote over its 32 threads, 16 columns of 2 rows each); the warp's flag tells the epilogue
+// whether its rows of the buffer are this quarter's or still an earlier one's.  Gated or not, the barrier protocol is
+// the same: only the data stores are skipped.
+__device__ __forceinline__ void store_half(const uint32_t (&d)[32], uint32_t stg, uint32_t qempty, uint32_t parity, uint32_t qfull,
+                                           uint32_t thr, uint32_t tag, uint32_t flag) {
+    float m0 = fmaxf(fu(d[0]), fu(d[1])), m1 = fmaxf(fu(d[2]), fu(d[3]));  // this thread's columns of its two rows
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        const uint32_t a = stg + (uint32_t)(8 * j * 4);
-        sts_v2(a, d[4 * j], d[4 * j + 1]);
-        sts_v2(a + 8 * STG_STRIDE * 4, d[4 * j + 2], d[4 * j + 3]);
+    for (int j = 1; j < 8; ++j) {
+        m0 = max3(m0, fu(d[4 * j]), fu(d[4 * j + 1]));
+        m1 = max3(m1, fu(d[4 * j + 2]), fu(d[4 * j + 3]));
     }
+    uint32_t tg0, tg1;
+    float t0, t1;
+    lds_thr(thr, tg0, t0);
+    lds_thr(thr + 8 * 8, tg1, t1);  // the row 8 below
+    const bool hit = (m0 > (tg0 == tag ? t0 : -INFINITY)) | (m1 > (tg1 == tag ? t1 : -INFINITY));
+    const bool staged = __any_sync(B200_FULL_MASK, hit);
+    mbar_wait(qempty, parity);
+    if (staged) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const uint32_t a = stg + (uint32_t)(8 * j * 4);
+            sts_v2(a, d[4 * j], d[4 * j + 1]);
+            sts_v2(a + 8 * STG_STRIDE * 4, d[4 * j + 2], d[4 * j + 3]);
+        }
+    }
+    if ((threadIdx.x & 31) == 0) sts_s32(flag, staged ? 1 : 0);
     mbar_arrive(qfull);
+}
+
+// The staging flags of two MMA warps, read after the half's `full` barrier (ordered after it like the staged data).
+__device__ __forceinline__ void lds_flags2(uint32_t a, uint32_t& f0, uint32_t& f1) {
+    asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(f0), "=r"(f1) : "r"(a) : "memory");
 }
 
 // Shared-memory map (dynamic, 1 KiB aligned): [KB] subject blocks (16 KiB each) | [NS] object blocks (8 KiB each: 64
 // objects of a tile quarter) | accumulator staging [128 rows][STG_STRIDE] fp32 | candidate lists [NLIST][128 rows][SLOTS]
-// scores + ids | FIFOs | thresholds [NLIST + 1][128] | barriers.
+// scores + ids | FIFOs | thresholds [NLIST + 1][128] | barriers, staging flags.
 // WIDE / PEERS compile the wide mode (threshold freeze + global append) and the peer-threshold exchange in; the plain
 // instantiation carries neither in its tile loop.  BF16 selects the MMA operand type.
 template <bool WIDE, bool PEERS, bool BF16>
@@ -204,6 +236,9 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
     // the staging buffer's two m-halves (rows 0-63 / 64-127) are handed over separately
     const uint32_t bar_qfull = smem_u32(bars + MAX_STAGES + 1);   // [4][2] half h of quarter q of the current tile staged
     const uint32_t bar_qempty = smem_u32(bars + MAX_STAGES + 9);  // [2] staged half read by its two epilogue warps
+    // staging flags, u32 [2 halves][4 MMA warps] in the unused tail of the barrier area: 1 = the warp's 16 rows of the half
+    // hold the current quarter, 0 = the threshold gate skipped them (store_half)
+    const uint32_t stg_flags = smem_u32(bars + MAX_STAGES + 11);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int rank = blockIdx.x & 1;  // which 128 rows of the pair's 256 (== the CTA's rank in its cluster)
@@ -278,6 +313,9 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
         // this thread's accumulator rows / columns in the staging buffer (m-half 1: + 64 rows; second row of a fragment: + 8)
         const uint32_t stg_w = smem_u32(sStg) + (uint32_t)(((warp * 16 + (lane >> 2)) * STG_STRIDE + 2 * (lane & 3)) * 4);
         const uint32_t stg_w1 = stg_w + (uint32_t)(64 * STG_STRIDE * 4);
+        // the exchange slot of this thread's first row in list 0 (m-half 1: + 64 rows; list 1: + 128 rows), its warp's flags
+        const uint32_t thr_w = smem_u32(sThr + warp * 16 + (lane >> 2));
+        const uint32_t flag_w = stg_flags + (uint32_t)warp * 4, flag_w1 = flag_w + 16;
         const uint32_t a_lo0 = smem_desc_lo(sA_u), b_lo0 = smem_desc_lo(sB_u);
         // fp32 accumulators of the two m-halves, as bit patterns
         uint32_t acc[2][32];
@@ -318,28 +356,30 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
                 advance();
                 for (int qi = 0; qi + 1 < nq; ++qi, ++n_store) {
                     const uint32_t qf = bar_qfull + 16 * (qi & 3), par = (n_store & 1) ^ 1;
+                    const uint32_t thr_q = thr_w + (uint32_t)(qi & 1) * (TILE_M * 8);  // quarter qi feeds list qi & 1
                     wgmma_wait<1>();  // G0(qi)
                     fence_acc(acc[0]);
-                    store_half(acc[0], stg_w, bar_qempty, par, qf);
+                    store_half(acc[0], stg_w, bar_qempty, par, qf, thr_q, work_it, flag_w);
                     blocks_landed<PKB>(bar_full, NS, stage, ph);
                     mma_half<BF16, PKB>(acc[0], a_lo0, b_lo0, NS, stage);
                     wgmma_wait<1>();  // G1(qi): quarter qi's object blocks are free
                     fence_acc(acc[1]);
                     done += PKB;
                     refill();
-                    store_half(acc[1], stg_w1, bar_qempty + 8, par, qf + 8);
+                    store_half(acc[1], stg_w1, bar_qempty + 8, par, qf + 8, thr_q + 64 * 8, work_it, flag_w1);
                     mma_half<BF16, PKB>(acc[1], a_lo0 + 512, b_lo0, NS, stage);
                     advance();
                 }
                 const uint32_t qf = bar_qfull + 16 * ((nq - 1) & 3), par = (n_store & 1) ^ 1;
+                const uint32_t thr_q = thr_w + (uint32_t)((nq - 1) & 1) * (TILE_M * 8);
                 wgmma_wait<1>();
                 fence_acc(acc[0]);
-                store_half(acc[0], stg_w, bar_qempty, par, qf);
+                store_half(acc[0], stg_w, bar_qempty, par, qf, thr_q, work_it, flag_w);
                 wgmma_wait<0>();  // the work item's last MMAs (the next one reloads the subject blocks)
                 fence_acc(acc[1]);
                 done += PKB;
                 refill();
-                store_half(acc[1], stg_w1, bar_qempty + 8, par, qf + 8);
+                store_half(acc[1], stg_w1, bar_qempty + 8, par, qf + 8, thr_q + 64 * 8, work_it, flag_w1);
                 ++n_store;
             } else {
                 // deeper d: one commit group per k block (both m-halves), its ring slot refilled as soon as the next
@@ -376,8 +416,9 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
                     ++done;
                     refill();
                     const uint32_t qf = bar_qfull + 16 * (qi & 3), par = (n_store & 1) ^ 1;
-                    store_half(acc[0], stg_w, bar_qempty, par, qf);
-                    store_half(acc[1], stg_w1, bar_qempty + 8, par, qf + 8);
+                    const uint32_t thr_q = thr_w + (uint32_t)(qi & 1) * (TILE_M * 8);
+                    store_half(acc[0], stg_w, bar_qempty, par, qf, thr_q, work_it, flag_w);
+                    store_half(acc[1], stg_w1, bar_qempty + 8, par, qf + 8, thr_q + 64 * 8, work_it, flag_w1);
                 }
             }
         }
@@ -396,6 +437,9 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
         // the m-half of the staging buffer that holds this warp's rows: quarters 0, 1 -> half 0; 2, 3 -> half 1
         const uint32_t half = (uint32_t)quarter >> 1;
         const uint32_t qfull0 = pin(bar_qfull + (uint32_t)colg * 16 + half * 8), qempty = pin(bar_qempty + half * 8);
+        // the flags of the two MMA warps that staged this warp's rows: lanes 0-15 / 16-31 are the rows of MMA warps
+        // 2 (quarter & 1) and 2 (quarter & 1) + 1 of the half (not pinned: one register less in the tile loop)
+        const uint32_t flags2 = stg_flags + (half * 4 + 2 * ((uint32_t)quarter & 1)) * 4;
         const bool lane0 = pin((uint32_t)lane) == 0;
         const uint32_t n_pos = (uint32_t)p.n_pos;
         const int kc = p.k_cand;  // (<= SLOTS, guaranteed by the host; a visible bound makes the compiler unroll the list scans fully and spill)
@@ -483,16 +527,22 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
 #pragma unroll
                 for (int s = 0; s < NQ; ++s) {
                     mbar_wait(qfull0 + (uint32_t)(s * NLIST * 16), tpar);
+                    // rows the threshold gate left unstaged cannot hit (store_half); a warp with none staged reads nothing
+                    uint32_t f0, f1;
+                    lds_flags2(flags2, f0, f1);
+                    const bool staged = (lane < 16 ? f0 : f1) != 0;
+                    const bool scan = !dbg_skip && (f0 | f1) != 0;
                     uint32_t r[QUART_N];
-                    if (!dbg_skip) stage_ld(stg_r, r);
+                    if (scan) stage_ld(stg_r, r);
                     __syncwarp();
                     if (lane0) mbar_arrive(qempty);  // staging buffer free again
-                    if (!dbg_skip) {
+                    if (scan) {
                         const uint32_t pos_q = pos_t + (uint32_t)(s * NLIST * QUART_N);
                         const float m0 = chunk_max<0>(r), m1 = chunk_max<32>(r);
                         const float mx = fmaxf(m0, m1);
-                        if (__any_sync(B200_FULL_MASK, mx > rs.thr)) {
-                            const float thr = rs.thr;
+                        // an unstaged row's part of the buffer is an earlier quarter: no hits for its lane
+                        const float thr = staged ? rs.thr : INFINITY;
+                        if (__any_sync(B200_FULL_MASK, mx > thr)) {
                             unsigned h0 = 0, h1 = 0;
                             if (__any_sync(B200_FULL_MASK, m0 > thr)) h0 = chunk_hits<0>(r, thr);
                             if (__any_sync(B200_FULL_MASK, m1 > thr)) h1 = chunk_hits<32>(r, thr);

@@ -80,6 +80,7 @@ void add_stats(b200_rank_stats& acc, const b200_rank_stats& s, bool first) {
     acc.n_chunks += s.n_chunks;
     acc.n_tc_launches += s.n_tc_launches;
     acc.ms_select += s.ms_select;
+    acc.ms_main_pass += s.ms_main_pass;
 }
 
 }  // namespace
@@ -542,6 +543,7 @@ int b200_rank_group_topk(b200_rank_group* g, const b200_rank_query* q, b200_rank
         const float ms_main = std::max(total->ms_main, M.stats.ms_main), ms_total = std::max(total->ms_total, M.stats.ms_total);
         const float ms_h2d = std::max(total->ms_h2d, M.stats.ms_h2d), ms_d2h = std::max(total->ms_d2h, M.stats.ms_d2h);
         const float ms_select = std::max(total->ms_select, M.stats.ms_select);
+        const float ms_main_pass = std::max(total->ms_main_pass, M.stats.ms_main_pass);
         add_stats(*total, M.stats, first);
         first = false;
         total->ms_main = ms_main;
@@ -549,6 +551,7 @@ int b200_rank_group_topk(b200_rank_group* g, const b200_rank_query* q, b200_rank
         total->ms_h2d = ms_h2d;
         total->ms_d2h = ms_d2h;
         total->ms_select = ms_select;
+        total->ms_main_pass = ms_main_pass;
     }
     return B200_OK;
 }
