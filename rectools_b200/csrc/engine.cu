@@ -1540,6 +1540,20 @@ int b200_rank_create_ex(b200_rank_engine** out, const void* objects, int32_t dty
     return create_impl(out, objects, dtype, n_objects, d, distance, device, tc_mode, flags);
 }
 
+#ifdef B200_FUSED_PROFILE
+// Measurement build only (not in b200_rank.h): the fused kernel's cycle counters on `device`, summed over every CTA of
+// every launch since the previous call (tc::PROF_N values in the order of tc::PROF_FULL ...), then cleared.
+int b200_rank_fused_profile(int32_t device, unsigned long long* out) {
+    static const unsigned long long zero[tc::PROF_N] = {};
+    if (!out) return fail(B200_E_INVALID, "b200_rank_fused_profile: NULL argument");
+    if (cudaSetDevice(device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess ||
+        cudaMemcpyFromSymbol(out, tc::fused_prof, sizeof(zero)) != cudaSuccess ||
+        cudaMemcpyToSymbol(tc::fused_prof, zero, sizeof(zero)) != cudaSuccess)
+        return fail(B200_E_CUDA, "b200_rank_fused_profile: CUDA error");
+    return B200_OK;
+}
+#endif
+
 int b200_rank_destroy(b200_rank_engine* E) {
     if (!E) return B200_OK;
     cudaSetDevice(E->device);

@@ -10,8 +10,8 @@
 //   -> deferred, bounded steps: filter_pairs_csr lookup through a prefetched 4-entry window, candidate-list insertion.
 // Score rows never reach HBM: only the K' best (score, id) pairs per row and column group are written.
 //
-// Warps 0-3: the MMA warp group (thread 0 also issues every TMA load); warps 4-11: the eight epilogue warps; with PEERS
-// two more warps poll the other ranks' published thresholds over NVLink and publish this rank's.  Epilogue warp w reads
+// Warps 0-3: the MMA warp group; warps 4-11: the eight epilogue warps; warp 12: the producer (one thread issues every TMA
+// load, and a ring slot returns to it through its `empty` barrier); with PEERS two more warps poll the other ranks' published thresholds over NVLink and publish this rank's.  Epilogue warp w reads
 // the row quarter w & 3 of column group w >> 2: group g of a tile is made of its quarters g and g + 2 (128 columns), and
 // each group has its own candidate list per row (two lists of 32 slots).
 // The two CTAs of a pair work on the same object tiles in the same order; the odd CTA waits for the start tile the even
@@ -38,8 +38,15 @@ constexpr uint32_t TAG_NONE = 0xffffffffu, TAG_DONE = 0xfffffffeu;  // exchange-
 struct FusedCfg {
     static constexpr int EPI0 = 4;                    // first epilogue warp; (warp & 3) is its row quarter
     static constexpr int EPILOGUE_WARPS = 8;          // epilogue warps
-    static constexpr int HELPERS = 2;                 // peer-threshold warps behind the epilogue (PEERS kernels only)
-    static constexpr int threads(bool peers) { return (EPI0 + EPILOGUE_WARPS + (peers ? HELPERS : 0)) * 32; }
+    static constexpr int PRODUCER = EPI0 + EPILOGUE_WARPS;  // the TMA warp
+    static constexpr int HELPERS = 2;                 // peer-threshold warps behind the producer (PEERS kernels only)
+    __host__ __device__ static constexpr int threads(bool peers) { return (PRODUCER + 1 + (peers ? HELPERS : 0)) * 32; }
+    // Registers per thread.  The register file is split over the SM's four sub-partitions (warp w runs on w mod 4); with
+    // 13-15 warps one of them holds four, so a thread gets 128 at launch.  setmaxnreg moves them within the CTA's
+    // allocation: the MMA warp group drops to 96, the two epilogue warp groups rise to 144 (96 + 2 x 144 + 128 = 4 x 128
+    // on the sub-partition with the producer); the producer and helper warps, no whole warp group, keep 128.
+    static constexpr int REGS_LAUNCH = 128, REGS_MMA = 96, REGS_EPILOGUE = 144;
+    static_assert(REGS_MMA + 2 * REGS_EPILOGUE + REGS_LAUNCH <= 4 * REGS_LAUNCH, "register plan of DESIGN section 5");
     static constexpr int COLS = 128;                  // accumulator columns per epilogue thread and tile
     static constexpr int NLIST = 2;                   // column groups = candidate lists per row
     static constexpr int NQ = COLS / QUART_N;         // staged quarters per epilogue thread and tile
@@ -53,6 +60,29 @@ struct FusedCfg {
     static constexpr int THR_BYTES = (NLIST + 1) * TILE_M * 8;     // (tag, threshold) per list + one slot for the peers' maximum
     static constexpr int FIXED_BYTES = STG_BYTES + 2 * LIST_BYTES + QBYTES + THR_BYTES + 1024 /*alignment slack*/ + 512 /*barriers*/;
 };
+
+#ifdef B200_FUSED_PROFILE
+// Measurement build only: clock64() cycles summed over the CTAs of every launch (b200_rank_fused_profile reads and
+// clears them).  Thread 0 of the MMA warp group measures its waits on `full` (TMA / L2), on `qempty` (the hand-off), in
+// wgmma.wait_group (the tensor pipe), and the pass (its first to its last instruction); the producer its waits on
+// `empty` and `aempty` (ring slots and subject blocks still in use); lane 0 of each epilogue warp its waits on `qfull`.
+enum { PROF_FULL, PROF_HANDOFF, PROF_PIPE, PROF_EMPTY, PROF_QFULL, PROF_PASS, PROF_N };
+static __device__ unsigned long long fused_prof[PROF_N];
+#define B200_PROF_ADD(i, v) atomicAdd(&fused_prof[i], (unsigned long long)(v))
+#define B200_TIMED(cyc, stmt)            \
+    do {                                 \
+        const long long t_ = clock64();  \
+        stmt;                            \
+        (cyc) += clock64() - t_;         \
+    } while (0)
+#else
+#define B200_PROF_ADD(i, v) (void)0
+#define B200_TIMED(cyc, stmt) \
+    do {                      \
+        stmt;                 \
+        (void)(cyc);          \
+    } while (0)
+#endif
 
 // Move this thread's pending hits of chunk OFF (ascending column order) into its FIFO (a ring of QN slots).  Returns
 // true when some lane still has hits but no free slot: the caller runs a fifo_step and calls again with the remaining mask.
@@ -178,7 +208,7 @@ __device__ __forceinline__ void blocks_landed(uint32_t bar_full, int NS, uint32_
 // whether its rows of the buffer are this quarter's or still an earlier one's.  Gated or not, the barrier protocol is
 // the same: only the data stores are skipped.
 __device__ __forceinline__ void store_half(const uint32_t (&d)[32], uint32_t stg, uint32_t qempty, uint32_t parity, uint32_t qfull,
-                                           uint32_t thr, uint32_t tag, uint32_t flag) {
+                                           uint32_t thr, uint32_t tag, uint32_t flag, long long& wait_cycles) {
     float m0 = fmaxf(fu(d[0]), fu(d[1])), m1 = fmaxf(fu(d[2]), fu(d[3]));  // this thread's columns of its two rows
 #pragma unroll
     for (int j = 1; j < 8; ++j) {
@@ -191,7 +221,7 @@ __device__ __forceinline__ void store_half(const uint32_t (&d)[32], uint32_t stg
     lds_thr(thr + 8 * 8, tg1, t1);  // the row 8 below
     const bool hit = (m0 > (tg0 == tag ? t0 : -INFINITY)) | (m1 > (tg1 == tag ? t1 : -INFINITY));
     const bool staged = __any_sync(B200_FULL_MASK, hit);
-    mbar_wait(qempty, parity);
+    B200_TIMED(wait_cycles, mbar_wait(qempty, parity));
     if (staged) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
@@ -215,7 +245,7 @@ __device__ __forceinline__ void lds_flags2(uint32_t a, uint32_t& f0, uint32_t& f
 // WIDE / PEERS compile the wide mode (threshold freeze + global append) and the peer-threshold exchange in; the plain
 // instantiation carries neither in its tile loop.  BF16 selects the MMA operand type.
 template <bool WIDE, bool PEERS, bool BF16>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(FusedCfg::threads(PEERS), 1)
+__global__ void __cluster_dims__(2, 1, 1) __maxnreg__(FusedCfg::REGS_LAUNCH)
 fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_constant__ CUtensorMap tm_obj, const TcParams p) {
     using Cfg = FusedCfg;
     constexpr int NLIST = Cfg::NLIST, SLOTS = Cfg::SLOTS, NQ = Cfg::NQ, QN = Cfg::Q, QS = Cfg::QSTRIDE;
@@ -239,14 +269,20 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
     // staging flags, u32 [2 halves][4 MMA warps] in the unused tail of the barrier area: 1 = the warp's 16 rows of the half
     // hold the current quarter, 0 = the threshold gate skipped them (store_half)
     const uint32_t stg_flags = smem_u32(bars + MAX_STAGES + 11);
+    const uint32_t bar_empty = smem_u32(bars + MAX_STAGES + 15);       // [NS] object block read by the MMA warp group
+    const uint32_t bar_aempty = smem_u32(bars + 2 * MAX_STAGES + 15);  // subject blocks no longer read
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int rank = blockIdx.x & 1;  // which 128 rows of the pair's 256 (== the CTA's rank in its cluster)
     const int n_pairs = gridDim.x >> 1, pair = blockIdx.x >> 1;
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < NS; ++i) mbar_init(bar_full + 8 * i, 1);
+        for (int i = 0; i < NS; ++i) {
+            mbar_init(bar_full + 8 * i, 1);
+            mbar_init(bar_empty + 8 * i, 4);  // lane 0 of each MMA warp
+        }
         mbar_init(bar_afull, 1);
+        mbar_init(bar_aempty, 4);
         for (int i = 0; i < 8; ++i) mbar_init(bar_qfull + 8 * i, 128);  // every thread of the MMA warp group
         for (int h = 0; h < 2; ++h) mbar_init(bar_qempty + 8 * h, 2);
         fence_barrier_init();
@@ -260,55 +296,24 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
     constexpr uint32_t BLK16 = BLK_BYTES >> 4, OBJ16 = OBJ_BLK_BYTES >> 4;  // blocks in descriptor address units
 
     if (warp < Cfg::EPI0) {
-        // ===================================================================== MMA warp group (+ TMA issue by thread 0)
-        const bool issuer = threadIdx.x == 0;
+        // ===================================================================== MMA warp group
+        setmaxnreg_dec<Cfg::REGS_MMA>();
+#ifdef B200_FUSED_PROFILE
+        const bool issuer = threadIdx.x == 0;  // the thread that measures
+        const long long t_start = clock64();
+#endif
+        long long full_cycles = 0, handoff_cycles = 0, pipe_cycles = 0;
         const uint32_t sA_u = smem_u32(sA), sB_u = smem_u32(sB);
-        // Object blocks are issued in consumption order (work item, tile, quarter, k block) up to NS blocks ahead of the
-        // MMAs; a ring slot is refilled once the wgmmas that read it have retired in every thread of the warp group
-        // (wgmma.wait_group waits for the executing thread's groups only, hence the warp-group barrier before the refill).
-        int lw = pair, li = 0, lq = 0, lkb = 0, lnt = 0, lts = 0, lt0 = 0, lt1 = 0, lsplit = 0;
-        uint32_t lwork = 0, lstage = 0;
-        bool lnew = true;
-        int64_t issued = 0, done = 0;
-        auto issue_next = [&]() -> bool {
-            if (lw >= n_work) return false;
-            if (lnew) {
-                lsplit = lw / p.n_row_tiles;
-                lt0 = lsplit * p.tiles_per_split;
-                lt1 = min(lt0 + p.tiles_per_split, p.n_obj_tiles);
-                lnt = lt1 - lt0;
-                lts = carousel_start(p, pair, lwork, lsplit, lt0, lt1, rank == 0);
-                lnew = false;
+        // A ring slot goes back to the producer once the wgmmas that read it have retired in every warp of the warp group
+        // (wgmma.wait_group waits for the executing thread's groups only): lane 0 of each warp arrives on its `empty`
+        // barrier after its own wait.  Slots are released in the order they were filled.
+        uint32_t rel = 0;
+        auto release = [&](int n) {
+            for (int i = 0; i < n; ++i) {
+                if (lane == 0) mbar_arrive(bar_empty + 8 * rel);
+                if (++rel == (uint32_t)NS) rel = 0;
             }
-            const int t = lts + li < lt1 ? lts + li : lts + li - lnt;
-            // the front is the position of the reference pair (pair 0 of each split's work items)
-            if (rank == 0 && p.front && pair == 0 && lq == 0 && lkb == 0 && (li & 15) == 0)
-                *reinterpret_cast<volatile int32_t*>(p.front + lsplit) = t;
-            mbar_arrive_expect_tx(bar_full + 8 * lstage, OBJ_BLK_BYTES);
-            tma_load_2d(sB_u + lstage * OBJ_BLK_BYTES, &tm_obj, bar_full + 8 * lstage, lkb * KBLK, t * TILE_N + lq * QUART_N);
-            if (++lstage == (uint32_t)NS) lstage = 0;
-            ++issued;
-            if (++lkb == KB) {
-                lkb = 0;
-                if (++lq == 4) {
-                    lq = 0;
-                    if (++li == lnt) {
-                        li = 0;
-                        lw += n_pairs;
-                        ++lwork;
-                        lnew = true;
-                    }
-                }
-            }
-            return true;
         };
-        auto refill = [&]() {
-            mma_group_sync();
-            if (issuer)
-                while (issued < done + NS && issue_next()) {
-                }
-        };
-        refill();
 
         // this thread's accumulator rows / columns in the staging buffer (m-half 1: + 64 rows; second row of a fragment: + 8)
         const uint32_t stg_w = smem_u32(sStg) + (uint32_t)(((warp * 16 + (lane >> 2)) * STG_STRIDE + 2 * (lane & 3)) * 4);
@@ -337,49 +342,41 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
             }
         };
         for (int w = pair; w < n_work; w += n_pairs, ++work_it) {
-            const int split = w / p.n_row_tiles, rt = w - split * p.n_row_tiles;
+            const int split = w / p.n_row_tiles;
             const int t0 = split * p.tiles_per_split;
             const int t1 = min(t0 + p.tiles_per_split, p.n_obj_tiles);
-            // the previous work item's MMAs have all retired (every work item ends in wgmma.wait_group 0)
-            if (issuer) {
-                mbar_arrive_expect_tx(bar_afull, (uint32_t)(KB * BLK_BYTES));
-                for (int kb = 0; kb < KB; ++kb)
-                    tma_load_2d(sA_u + (uint32_t)kb * BLK_BYTES, &tm_sub, bar_afull, kb * KBLK, (rt * 2 + rank) * TILE_M);
-            }
             mbar_wait(bar_afull, work_it & 1);
             const int nq = 4 * (t1 - t0);  // quarters of the work item, in stream order
             // (rows 64-127 of the subject block start 8 KiB = +512 descriptor units further)
             if (pipelined) {
-                blocks_landed<PKB>(bar_full, NS, stage, ph);
+                B200_TIMED(full_cycles, blocks_landed<PKB>(bar_full, NS, stage, ph));
                 mma_half<BF16, PKB>(acc[0], a_lo0, b_lo0, NS, stage);
                 mma_half<BF16, PKB>(acc[1], a_lo0 + 512, b_lo0, NS, stage);
                 advance();
                 for (int qi = 0; qi + 1 < nq; ++qi, ++n_store) {
                     const uint32_t qf = bar_qfull + 16 * (qi & 3), par = (n_store & 1) ^ 1;
                     const uint32_t thr_q = thr_w + (uint32_t)(qi & 1) * (TILE_M * 8);  // quarter qi feeds list qi & 1
-                    wgmma_wait<1>();  // G0(qi)
+                    B200_TIMED(pipe_cycles, wgmma_wait<1>());  // G0(qi)
                     fence_acc(acc[0]);
-                    store_half(acc[0], stg_w, bar_qempty, par, qf, thr_q, work_it, flag_w);
-                    blocks_landed<PKB>(bar_full, NS, stage, ph);
+                    store_half(acc[0], stg_w, bar_qempty, par, qf, thr_q, work_it, flag_w, handoff_cycles);
+                    B200_TIMED(full_cycles, blocks_landed<PKB>(bar_full, NS, stage, ph));
                     mma_half<BF16, PKB>(acc[0], a_lo0, b_lo0, NS, stage);
-                    wgmma_wait<1>();  // G1(qi): quarter qi's object blocks are free
+                    B200_TIMED(pipe_cycles, wgmma_wait<1>());  // G1(qi): quarter qi's object blocks are free
                     fence_acc(acc[1]);
-                    done += PKB;
-                    refill();
-                    store_half(acc[1], stg_w1, bar_qempty + 8, par, qf + 8, thr_q + 64 * 8, work_it, flag_w1);
+                    release(PKB);
+                    store_half(acc[1], stg_w1, bar_qempty + 8, par, qf + 8, thr_q + 64 * 8, work_it, flag_w1, handoff_cycles);
                     mma_half<BF16, PKB>(acc[1], a_lo0 + 512, b_lo0, NS, stage);
                     advance();
                 }
                 const uint32_t qf = bar_qfull + 16 * ((nq - 1) & 3), par = (n_store & 1) ^ 1;
                 const uint32_t thr_q = thr_w + (uint32_t)((nq - 1) & 1) * (TILE_M * 8);
-                wgmma_wait<1>();
+                B200_TIMED(pipe_cycles, wgmma_wait<1>());
                 fence_acc(acc[0]);
-                store_half(acc[0], stg_w, bar_qempty, par, qf, thr_q, work_it, flag_w);
-                wgmma_wait<0>();  // the work item's last MMAs (the next one reloads the subject blocks)
+                store_half(acc[0], stg_w, bar_qempty, par, qf, thr_q, work_it, flag_w, handoff_cycles);
+                B200_TIMED(pipe_cycles, wgmma_wait<0>());  // the work item's last MMAs (the next one reloads the subject blocks)
                 fence_acc(acc[1]);
-                done += PKB;
-                refill();
-                store_half(acc[1], stg_w1, bar_qempty + 8, par, qf + 8, thr_q + 64 * 8, work_it, flag_w1);
+                release(PKB);
+                store_half(acc[1], stg_w1, bar_qempty + 8, par, qf + 8, thr_q + 64 * 8, work_it, flag_w1, handoff_cycles);
                 ++n_store;
             } else {
                 // deeper d: one commit group per k block (both m-halves), its ring slot refilled as soon as the next
@@ -389,7 +386,7 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
                     fence_acc(acc[0]);
                     fence_acc(acc[1]);
                     for (int kb = 0; kb < KB; ++kb, a_lo += BLK16) {
-                        mbar_wait(bar_full + 8 * stage, ph);
+                        B200_TIMED(full_cycles, mbar_wait(bar_full + 8 * stage, ph));
                         wgmma_fence();
                         const uint32_t b_lo = b_lo0 + stage * OBJ16;
                         // +32 B per K = 16 step inside the 128 B swizzle atom = +2 in descriptor address units
@@ -405,25 +402,35 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
                             ph ^= 1;
                         }
                         if (kb > 0) {
-                            wgmma_wait<1>();  // the previous k block's MMAs have read their ring slot
-                            ++done;
-                            refill();
+                            B200_TIMED(pipe_cycles, wgmma_wait<1>());  // the previous k block's MMAs have read their ring slot
+                            release(1);
                         }
                     }
-                    wgmma_wait<0>();
+                    B200_TIMED(pipe_cycles, wgmma_wait<0>());
                     fence_acc(acc[0]);
                     fence_acc(acc[1]);
-                    ++done;
-                    refill();
+                    release(1);
                     const uint32_t qf = bar_qfull + 16 * (qi & 3), par = (n_store & 1) ^ 1;
                     const uint32_t thr_q = thr_w + (uint32_t)(qi & 1) * (TILE_M * 8);
-                    store_half(acc[0], stg_w, bar_qempty, par, qf, thr_q, work_it, flag_w);
-                    store_half(acc[1], stg_w1, bar_qempty + 8, par, qf + 8, thr_q + 64 * 8, work_it, flag_w1);
+                    store_half(acc[0], stg_w, bar_qempty, par, qf, thr_q, work_it, flag_w, handoff_cycles);
+                    store_half(acc[1], stg_w1, bar_qempty + 8, par, qf + 8, thr_q + 64 * 8, work_it, flag_w1, handoff_cycles);
                 }
             }
+            // every work item ends in wgmma.wait_group 0: the subject blocks may be reloaded
+            if (lane == 0) mbar_arrive(bar_aempty);
         }
-    } else if (warp < Cfg::EPI0 + Cfg::EPILOGUE_WARPS) {
+#ifdef B200_FUSED_PROFILE
+        if (issuer) {
+            B200_PROF_ADD(PROF_FULL, full_cycles);
+            B200_PROF_ADD(PROF_HANDOFF, handoff_cycles);
+            B200_PROF_ADD(PROF_PIPE, pipe_cycles);
+            B200_PROF_ADD(PROF_PASS, clock64() - t_start);
+        }
+#endif
+    } else if (warp < Cfg::PRODUCER) {
         // ===================================================================== epilogue: select candidates
+        setmaxnreg_inc<Cfg::REGS_EPILOGUE>();
+        long long qfull_cycles = 0;
         const int ew = warp - Cfg::EPI0;
         const int colg = ew >> 2, quarter = warp & 3;  // column group of the tile / row quarter of the CTA's 128 rows
         const int wrow0 = quarter * 32;                // first CTA-local subject row of this warp
@@ -526,7 +533,7 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
                 const bool last = (it + 1 == nt);
 #pragma unroll
                 for (int s = 0; s < NQ; ++s) {
-                    mbar_wait(qfull0 + (uint32_t)(s * NLIST * 16), tpar);
+                    B200_TIMED(qfull_cycles, mbar_wait(qfull0 + (uint32_t)(s * NLIST * 16), tpar));
                     // rows the threshold gate left unstaged cannot hit (store_half); a warp with none staged reads nothing
                     uint32_t f0, f1;
                     lds_flags2(flags2, f0, f1);
@@ -592,13 +599,52 @@ fused_topk_kernel(const __grid_constant__ CUtensorMap tm_sub, const __grid_const
             if (PEERS && peers && w + n_pairs >= n_work) sts_thr(my_thr, TAG_DONE, INFINITY);
         }
 #undef B200_STEP
+        if (lane == 0) B200_PROF_ADD(PROF_QFULL, qfull_cycles);
+    } else if (warp == Cfg::PRODUCER) {
+        // ===================================================================== producer: every TMA load of the CTA
+        // Object blocks in consumption order (work item, tile, quarter, k block), up to NS blocks ahead of the MMAs; a
+        // slot is refilled once its `empty` barrier says every MMA warp has retired the wgmmas that read it.
+        if (lane == 0) {
+            const uint32_t sA_u = smem_u32(sA), sB_u = smem_u32(sB);
+            long long empty_cycles = 0;
+            uint32_t stage = 0, ph = 0, work_it = 0;
+            for (int w = pair; w < n_work; w += n_pairs, ++work_it) {
+                const int split = w / p.n_row_tiles, rt = w - split * p.n_row_tiles;
+                const int t0 = split * p.tiles_per_split;
+                const int t1 = min(t0 + p.tiles_per_split, p.n_obj_tiles);
+                const int nt = t1 - t0;
+                // the subject blocks are reloaded once the previous work item's MMAs have all retired
+                if (work_it > 0) B200_TIMED(empty_cycles, mbar_wait(bar_aempty, (work_it - 1) & 1));
+                mbar_arrive_expect_tx(bar_afull, (uint32_t)(KB * BLK_BYTES));
+                for (int kb = 0; kb < KB; ++kb)
+                    tma_load_2d(sA_u + (uint32_t)kb * BLK_BYTES, &tm_sub, bar_afull, kb * KBLK, (rt * 2 + rank) * TILE_M);
+                const int ts = carousel_start(p, pair, work_it, split, t0, t1, rank == 0);
+                for (int i = 0; i < nt; ++i) {
+                    const int t = ts + i < t1 ? ts + i : ts + i - nt;
+                    // the front is the position of the reference pair (pair 0 of each split's work items)
+                    if (rank == 0 && p.front && pair == 0 && (i & 15) == 0) *reinterpret_cast<volatile int32_t*>(p.front + split) = t;
+                    for (int q = 0; q < 4; ++q)
+                        for (int kb = 0; kb < KB; ++kb) {
+                            // (a fresh barrier passes the wait for parity 1: the first round finds every slot free)
+                            B200_TIMED(empty_cycles, mbar_wait(bar_empty + 8 * stage, ph ^ 1));
+                            mbar_arrive_expect_tx(bar_full + 8 * stage, OBJ_BLK_BYTES);
+                            tma_load_2d(sB_u + stage * OBJ_BLK_BYTES, &tm_obj, bar_full + 8 * stage, kb * KBLK, t * TILE_N + q * QUART_N);
+                            if (++stage == (uint32_t)NS) {
+                                stage = 0;
+                                ph ^= 1;
+                            }
+                        }
+                }
+            }
+            B200_PROF_ADD(PROF_EMPTY, empty_cycles);
+        }
     } else if (PEERS && p.n_peers > 0) {
         // ===================================================================== peer-threshold helpers (two warps)
         // Thread h serves CTA-local rows h and h + 64.  Per round and row: read the row's own thresholds from the exchange
         // slots, publish their maximum to this rank's global array, read the other ranks' published values (NVLink peer
         // loads, latency irrelevant here), leave their maximum in the row's extra exchange slot.  All values are monotone
         // lower bounds of the row's final threshold: a stale one is only weaker, never wrong.
-        const int h = (warp - Cfg::EPI0 - Cfg::EPILOGUE_WARPS) * 32 + lane;
+        const int h = (warp - Cfg::PRODUCER - 1) * 32 + lane;
         float published[2] = {-INFINITY, -INFINITY};
         uint32_t pub_tag[2] = {0xffffffffu, 0xffffffffu};
         bool done[2] = {false, false};

@@ -120,8 +120,11 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* m, 
 __device__ __forceinline__ uint32_t smem_desc_lo(uint32_t saddr) { return ((saddr & 0x3FFFF) >> 4) | (1u << 16); }
 constexpr uint32_t SMEM_DESC_HI = (1024u >> 4) | (1u << 30);
 
-// Barrier of the 128 threads of the MMA warp group only (named barrier 1; barrier 0 is __syncthreads).
-__device__ __forceinline__ void mma_group_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+// Hand registers of this warp group back to the CTA / take them (all four warps execute it together).
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 // Pin the accumulator registers at this point of the instruction stream (before wgmma.fence, after wgmma.wait_group:

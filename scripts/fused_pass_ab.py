@@ -14,6 +14,15 @@ a minute per million rows on an H100): so the debug arms rank the first --debug-
 that size too, next to the full config-2 batch.  Each library runs in its own process (the library is chosen by
 B200_RANK_LIB when the package loads); the two alternate --reps times, each arm takes the median of --calls calls after
 one warm-up call.  Prints the card name, power limit and max SM clock, writes DIR/fused_pass_ab.json.
+
+    python scripts/fused_pass_ab.py --profile rectools_b200/libb200rank_profile.so --out DIR
+
+runs the measurement build instead (`python -m rectools_b200.build --variant profile -DB200_FUSED_PROFILE`): one call of
+the normal arm at --users rows and one of debug1, each after a warm-up, and prints where the fused kernel waits, as shares
+of the pass (the MMA warp group's thread 0 from start to end, per CTA): that thread on `full` (TMA / L2), on `qempty`
+(the hand-off) and in `wgmma.wait_group` (the tensor pipe); the producer on `empty` / `aempty` (slots still in use);
+the epilogue warps on `qfull` (mean over the eight).
+Writes DIR/fused_profile.json.
 """
 from __future__ import annotations
 
@@ -27,6 +36,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FIELDS = ("ms_main_pass", "ms_main", "ms_total", "n_tc_launches", "n_fallback_rows")
+PROF_FIELDS = ("full", "handoff", "pipe", "empty", "qfull", "pass")  # the counters of fused_topk.cuh, in its order
 
 
 def worker(a) -> None:
@@ -60,6 +70,32 @@ def worker(a) -> None:
         return {f: st[f] for f in FIELDS}
 
     out = {}
+    if a.profile_worker:
+        import ctypes
+
+        lib = _lib.load()
+        lib.b200_rank_fused_profile.restype = ctypes.c_int
+        lib.b200_rank_fused_profile.argtypes = [ctypes.c_int32, ctypes.POINTER(ctypes.c_ulonglong)]
+        cnt = (ctypes.c_ulonglong * len(PROF_FIELDS))()
+        for name, dbg, n_rows in [("normal", 0, n_users), ("debug1", 1, a.debug_users)]:
+            if dbg:
+                os.environ["B200_TC_DEBUG"] = str(dbg)
+            else:
+                os.environ.pop("B200_TC_DEBUG", None)
+            call(n_rows)  # warm-up
+            _lib.check(lib.b200_rank_fused_profile(0, cnt))
+            st = call(n_rows)
+            _lib.check(lib.b200_rank_fused_profile(0, cnt))
+            c = dict(zip(PROF_FIELDS, (int(v) for v in cnt)))
+            pas = max(c["pass"], 1)
+            out[name] = {"rows": n_rows, "ms_main_pass": st["ms_main_pass"], "cycles": c,
+                         "shares": {"mma_full": c["full"] / pas, "mma_handoff": c["handoff"] / pas,
+                                    "mma_wgmma_wait": c["pipe"] / pas, "producer_empty": c["empty"] / pas,
+                                    "epilogue_qfull": c["qfull"] / (8 * pas)}}
+        os.environ.pop("B200_TC_DEBUG", None)
+        eng.close()
+        print("RESULT " + json.dumps(out), flush=True)
+        return
     arms = [("normal", 0, n_users), ("normal_small", 0, a.debug_users), ("debug2", 2, a.debug_users), ("debug1", 1, a.debug_users)]
     for name, dbg, n_rows in arms:
         if dbg:
@@ -74,11 +110,11 @@ def worker(a) -> None:
     print("RESULT " + json.dumps(out), flush=True)
 
 
-def run_worker(lib: str, a) -> dict:
+def run_worker(lib: str, a, profile: bool = False) -> dict:
     env = dict(os.environ, B200_RANK_LIB=os.path.abspath(lib))
     env.pop("B200_TC_DEBUG", None)
     cmd = [sys.executable, os.path.abspath(__file__), "--worker", "--users", str(a.users), "--debug-users", str(a.debug_users),
-           "--calls", str(a.calls)]
+           "--calls", str(a.calls)] + (["--profile-worker"] if profile else [])
     res = subprocess.run(cmd, env=env, capture_output=True, text=True, cwd=ROOT)
     lines = [ln for ln in res.stdout.splitlines() if ln.startswith("RESULT ")]
     if res.returncode != 0 or not lines:
@@ -97,7 +133,9 @@ def main() -> None:
     ap.add_argument("--calls", type=int, default=5)
     ap.add_argument("--users", type=int, default=1_000_000, help="rows of the normal arm (config 2: 1M)")
     ap.add_argument("--debug-users", type=int, default=65_536, help="rows of the debug arms and of normal_small")
+    ap.add_argument("--profile", help="a B200_FUSED_PROFILE build: report the kernel's wait shares instead of the A/B")
     ap.add_argument("--worker", action="store_true", help=argparse.SUPPRESS)
+    ap.add_argument("--profile-worker", action="store_true", help=argparse.SUPPRESS)
     a = ap.parse_args()
     if a.worker:
         worker(a)
@@ -107,6 +145,15 @@ def main() -> None:
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                           capture_output=True, text=True).stdout.strip()
     print("card:", card, flush=True)
+    if a.profile:
+        r = run_worker(a.profile, a, profile=True)
+        print("wait shares of the pass:", json.dumps({m: {"rows": v["rows"], "ms_main_pass": round(v["ms_main_pass"], 2),
+                                                          **{k: round(x, 3) for k, x in v["shares"].items()}}
+                                                      for m, v in r.items()}, indent=1), flush=True)
+        os.makedirs(a.out, exist_ok=True)
+        with open(os.path.join(a.out, "fused_profile.json"), "w") as f:
+            json.dump({"card": card, "users": a.users, "debug_users": a.debug_users, "profile": r}, f, indent=1)
+        return
     arms = {"base": a.base, "new": a.new}
     if a.only:
         arms = {a.only: arms[a.only]}
