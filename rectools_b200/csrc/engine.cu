@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "../../include/b200_rank.h"
+#include "cuda_call.h"
 #include "engine_internal.h"
 #include "plan.h"
 #include "common.cuh"
@@ -45,46 +46,6 @@ int fail(int code, const char* fmt, ...) {
     g_last_error = buf;
     return code;
 }
-
-struct CudaError {
-    cudaError_t e;
-    const char* what;
-    int line;
-};
-
-#define CK(call)                                               \
-    do {                                                       \
-        cudaError_t e__ = (call);                              \
-        if (e__ != cudaSuccess) throw CudaError{e__, #call, __LINE__}; \
-    } while (0)
-
-struct DevBuf {
-    void* p = nullptr;
-    size_t cap = 0;
-    void ensure(size_t bytes) {
-        if (bytes <= cap) return;
-        if (p) CK(cudaFree(p));
-        p = nullptr;
-        cap = 0;
-        size_t want = bytes + bytes / 8 + 256;
-        CK(cudaMalloc(&p, want));
-        cap = want;
-    }
-    void ensure_exact(size_t bytes) {  // buffers that never grow (the resident objects): no slack
-        release();
-        CK(cudaMalloc(&p, bytes));
-        cap = bytes;
-    }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
-    template <typename T>
-    T* as() const {
-        return reinterpret_cast<T*>(p);
-    }
-};
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -419,11 +380,9 @@ int create_impl(b200_rank_engine** out, const void* objects, int32_t dtype, int6
         CK(cudaFuncSetAttribute(cand_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lk_smem_bytes(LK_SMEM_PAIRS)));
         CK(cudaFuncSetAttribute(cand_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lk_smem_bytes(LK_SMEM_PAIRS)));
     } catch (const CudaError& ce) {
-        int rc = fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_create: %s failed at line %d: %s",
-                      ce.what, ce.line, cudaGetErrorString(ce.e));
         E->free_all();
         delete E;
-        return rc;
+        return cuda_fail("b200_rank_create", ce);
     }
     *out = E;
     return B200_OK;
@@ -1598,8 +1557,7 @@ int b200_rank_set_subjects(b200_rank_engine* E, const float* subjects, int64_t n
         E->n_sub_res = n_subjects;
         E->sub_res_on_device = on_device != 0;
     } catch (const CudaError& ce) {
-        return fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_set_subjects: %s failed: %s", ce.what,
-                    cudaGetErrorString(ce.e));
+        return cuda_fail("b200_rank_set_subjects", ce);
     }
     return B200_OK;
 }
@@ -1629,7 +1587,7 @@ int b200_rank_peer_export(b200_rank_engine* E, int64_t max_rows, void* handle_ou
         CK(cudaIpcGetMemHandle(&h, E->peer_pub.p));
         memcpy(handle_out, &h, sizeof(h));
     } catch (const CudaError& ce) {
-        return fail(B200_E_CUDA, "b200_rank_peer_export: %s failed: %s", ce.what, cudaGetErrorString(ce.e));
+        return cuda_fail("b200_rank_peer_export", ce);
     }
     return B200_OK;
 }
@@ -1651,7 +1609,7 @@ int b200_rank_peer_import(b200_rank_engine* E, int32_t n_ranks, int32_t self, co
         }
         E->n_peers = n;
     } catch (const CudaError& ce) {
-        return fail(B200_E_CUDA, "b200_rank_peer_import: %s failed: %s", ce.what, cudaGetErrorString(ce.e));
+        return cuda_fail("b200_rank_peer_import", ce);
     }
     return B200_OK;
 }
@@ -1673,7 +1631,7 @@ int b200_rank_peer_attach(b200_rank_engine* E, int64_t max_rows, void* pub, int3
             }
         }
     } catch (const CudaError& ce) {
-        return fail(B200_E_CUDA, "b200_rank_peer_attach: %s failed: %s", ce.what, cudaGetErrorString(ce.e));
+        return cuda_fail("b200_rank_peer_attach", ce);
     }
     E->peer_attached = true;
     E->peer_out = reinterpret_cast<unsigned long long*>(pub);
@@ -1785,8 +1743,7 @@ int b200_rank_topk(b200_rank_engine* E, const b200_rank_query* q, b200_rank_stat
         CK(cudaEventElapsedTime(&S.ms_d2h, E->ev_ranked, E->ev_end));    // exposed part: the last chunk's results (+ re-ranked rows)
         c.collect_times();
     } catch (const CudaError& ce) {
-        return fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_topk: %s failed at line %d: %s", ce.what,
-                    ce.line, cudaGetErrorString(ce.e));
+        return cuda_fail("b200_rank_topk", ce);
     }
     if (stats) *stats = c.S;
     return B200_OK;
@@ -1884,8 +1841,7 @@ int b200_rank_topk_candidates(b200_rank_engine* E, const b200_rank_query* q, con
         c.collect_times();
         c.S.n_tc_launches = 0;  // (collect_times counts the scoring launches there)
     } catch (const CudaError& ce) {
-        return fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_topk_candidates: %s failed at line %d: %s",
-                    ce.what, ce.line, cudaGetErrorString(ce.e));
+        return cuda_fail("b200_rank_topk_candidates", ce);
     }
     if (stats) *stats = c.S;
     return B200_OK;
@@ -1997,8 +1953,7 @@ int b200_rank_topk_candidates_device(b200_rank_engine* E, const b200_rank_query*
         c.collect_times();
         c.S.n_tc_launches = 0;  // (collect_times counts the preparation + scoring spans there)
     } catch (const CudaError& ce) {
-        return fail(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, "b200_rank_topk_candidates_device: %s failed at line %d: %s",
-                    ce.what, ce.line, cudaGetErrorString(ce.e));
+        return cuda_fail("b200_rank_topk_candidates_device", ce);
     }
     if (stats) *stats = c.S;
     return B200_OK;
@@ -2037,7 +1992,7 @@ int b200_rank_get_snapshot(b200_rank_engine* E, b200_rank_snapshot* meta, float*
         }
         CK(cudaStreamSynchronize(st));
     } catch (const CudaError& ce) {
-        return fail(B200_E_CUDA, "b200_rank_get_snapshot: %s failed: %s", ce.what, cudaGetErrorString(ce.e));
+        return cuda_fail("b200_rank_get_snapshot", ce);
     }
     return B200_OK;
 }
@@ -2078,7 +2033,7 @@ static int merge_impl(int32_t device, void* stream, int32_t n_lists, int64_t n_r
             CK(cudaGetLastError());
         }
     } catch (const CudaError& ce) {
-        return fail(B200_E_CUDA, "b200_rank_merge: %s failed: %s", ce.what, cudaGetErrorString(ce.e));
+        return cuda_fail("b200_rank_merge", ce);
     }
     return B200_OK;
 }

@@ -21,40 +21,11 @@
 #include <vector>
 
 #include "../../include/b200_rank.h"
+#include "cuda_call.h"
 #include "engine_internal.h"
 #include "group_plan.h"
 
 namespace {
-
-struct CudaError {
-    cudaError_t e;
-    const char* what;
-};
-
-#define GCK(call)                                   \
-    do {                                            \
-        cudaError_t e__ = (call);                   \
-        if (e__ != cudaSuccess) throw CudaError{e__, #call}; \
-    } while (0)
-
-// device memory of one member's device
-struct DBuf {
-    void* p = nullptr;
-    size_t cap = 0;
-    void* ensure(size_t bytes) {
-        if (bytes > cap) {
-            release();
-            GCK(cudaMalloc(&p, bytes));
-            cap = bytes;
-        }
-        return p;
-    }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
-};
 
 size_t dtype_bytes(int32_t dtype) { return dtype == B200_DT_F32 ? 4 : 2; }
 
@@ -89,13 +60,13 @@ struct GroupMember {
     b200_rank_engine* E = nullptr;
     int device = 0;
     bool home = true;
-    DBuf objects;   // peer copy of a device object matrix (members off the home device)
-    DBuf subjects;  // peer copy of device resident subjects (members off the home device)
+    DevBuf objects;   // peer copy of a device object matrix (members off the home device)
+    DevBuf subjects;  // peer copy of device resident subjects (members off the home device)
     // staging of device inputs / outputs (members off the home device)
     cudaStream_t st = nullptr;
     cudaEvent_t ev_done = nullptr;
-    DBuf in_sub, in_ids, in_rows, in_f_indptr, in_f_indices, in_wl, in_s_indptr, in_s_indices, in_s_data;
-    DBuf out_ids, out_scores, out_counts;
+    DevBuf in_sub, in_ids, in_rows, in_f_indptr, in_f_indices, in_wl, in_s_indptr, in_s_indices, in_s_data;
+    DevBuf out_ids, out_scores, out_counts;
     std::vector<int64_t> f_indptr, s_indptr;  // rebased host CSR rows of the current slice
     // result of the current call
     int rc = B200_OK;
@@ -104,7 +75,7 @@ struct GroupMember {
     b200_rank_stats stats{};
     std::thread worker;
 
-    std::vector<DBuf*> bufs() {
+    std::vector<DevBuf*> bufs() {
         return {&objects, &subjects, &in_sub, &in_ids, &in_rows, &in_f_indptr, &in_f_indices, &in_wl, &in_s_indptr, &in_s_indices,
                 &in_s_data, &out_ids, &out_scores, &out_counts};
     }
@@ -145,17 +116,17 @@ using b200_group = b200_rank_group;
 void stage_inputs_remote(b200_group* g, GroupMember& M, b200_rank_query& base) {
     const b200_rank_query& q = *g->q;
     const int64_t n = q.n_rows;
-    auto copy = [&](DBuf& buf, const void* src, size_t bytes) -> void* {
+    auto copy = [&](DevBuf& buf, const void* src, size_t bytes) -> void* {
         if (!src) return nullptr;
-        void* dst = buf.ensure(std::max<size_t>(bytes, 16));
-        if (bytes) GCK(cudaMemcpyPeerAsync(dst, M.device, src, g->home, bytes, M.st));
+        void* dst = buf.ensure_exact(std::max<size_t>(bytes, 16));
+        if (bytes) CK(cudaMemcpyPeerAsync(dst, M.device, src, g->home, bytes, M.st));
         return dst;
     };
     auto read_last = [&](const int64_t* indptr) {  // indptr[n_rows] of a home-device array, after the caller's stream
         int64_t v = 0;
-        GCK(cudaMemcpyPeerAsync(M.in_rows.ensure(16), M.device, indptr + n, g->home, sizeof(int64_t), M.st));
-        GCK(cudaMemcpyAsync(&v, M.in_rows.p, sizeof(int64_t), cudaMemcpyDeviceToHost, M.st));
-        GCK(cudaStreamSynchronize(M.st));
+        CK(cudaMemcpyPeerAsync(M.in_rows.ensure_exact(16), M.device, indptr + n, g->home, sizeof(int64_t), M.st));
+        CK(cudaMemcpyAsync(&v, M.in_rows.p, sizeof(int64_t), cudaMemcpyDeviceToHost, M.st));
+        CK(cudaStreamSynchronize(M.st));
         return std::max<int64_t>(v, 0);
     };
     if (q.subjects) {
@@ -230,17 +201,17 @@ void run_member(b200_group* g, int i) {
     M.n_slices = 0;
     memset(&M.stats, 0, sizeof(M.stats));
     try {
-        GCK(cudaSetDevice(M.device));
+        CK(cudaSetDevice(M.device));
         b200_rank_query base = q;
         if (remote) {
             base.stream = M.st;  // the member's calls are ordered after M.st, which follows the caller's stream
-            if (g->from_user) GCK(cudaStreamWaitEvent(M.st, g->ev_user, 0));
+            if (g->from_user) CK(cudaStreamWaitEvent(M.st, g->ev_user, 0));
             if (q.flags & B200_Q_INPUTS_ON_DEVICE) stage_inputs_remote(g, M, base);
             if (out_dev) {
                 const size_t nk = (size_t)q.n_rows * g->k_out;
-                base.out_ids = (int32_t*)M.out_ids.ensure(std::max<size_t>(4 * nk, 16));
-                base.out_scores = (float*)M.out_scores.ensure(std::max<size_t>(4 * nk, 16));
-                base.out_counts = (int32_t*)M.out_counts.ensure(std::max<size_t>(4 * q.n_rows, 16));
+                base.out_ids = (int32_t*)M.out_ids.ensure_exact(std::max<size_t>(4 * nk, 16));
+                base.out_scores = (float*)M.out_scores.ensure_exact(std::max<size_t>(4 * nk, 16));
+                base.out_counts = (int32_t*)M.out_counts.ensure_exact(std::max<size_t>(4 * q.n_rows, 16));
             }
         }
         for (;;) {
@@ -261,18 +232,17 @@ void run_member(b200_group* g, int i) {
             ++M.n_slices;
             if (remote && out_dev) {  // the slice's results into the caller's buffers, after the engine (M.st waits for it)
                 const int64_t k = g->k_out, nr = sl.r1 - sl.r0;
-                GCK(cudaMemcpyPeerAsync(q.out_ids + sl.r0 * k, g->home, sq.out_ids, M.device, sizeof(int32_t) * nr * k, M.st));
-                GCK(cudaMemcpyPeerAsync(q.out_scores + sl.r0 * k, g->home, sq.out_scores, M.device, sizeof(float) * nr * k, M.st));
-                GCK(cudaMemcpyPeerAsync(q.out_counts + sl.r0, g->home, sq.out_counts, M.device, sizeof(int32_t) * nr, M.st));
+                CK(cudaMemcpyPeerAsync(q.out_ids + sl.r0 * k, g->home, sq.out_ids, M.device, sizeof(int32_t) * nr * k, M.st));
+                CK(cudaMemcpyPeerAsync(q.out_scores + sl.r0 * k, g->home, sq.out_scores, M.device, sizeof(float) * nr * k, M.st));
+                CK(cudaMemcpyPeerAsync(q.out_counts + sl.r0, g->home, sq.out_counts, M.device, sizeof(int32_t) * nr, M.st));
             }
         }
         if (remote) {
-            GCK(cudaEventRecord(M.ev_done, M.st));
-            GCK(cudaStreamSynchronize(M.st));  // the staging buffers are reused by the next call
+            CK(cudaEventRecord(M.ev_done, M.st));
+            CK(cudaStreamSynchronize(M.st));  // the staging buffers are reused by the next call
         }
     } catch (const CudaError& ce) {
-        M.rc = ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA;
-        M.message = std::string(ce.what) + " failed: " + cudaGetErrorString(ce.e);
+        M.rc = cuda_failure(ce, M.message);
         g->failed.store(true);
     }
 }
@@ -305,7 +275,7 @@ void destroy_group(b200_group* g) {
     for (GroupMember& M : g->m) {
         if (M.E) b200_rank_destroy(M.E);  // before the peer copy an fp32 (or kept 16-bit) member references
         cudaSetDevice(M.device);
-        for (DBuf* b : M.bufs()) b->release();
+        for (DevBuf* b : M.bufs()) b->release();
         if (M.st) cudaStreamDestroy(M.st);
         if (M.ev_done) cudaEventDestroy(M.ev_done);
     }
@@ -346,22 +316,22 @@ int group_create(b200_group** out, const void* objects, int32_t dtype, int64_t n
     g->d = d;
     const bool obj_dev = flags & B200_F_OBJECTS_ON_DEVICE;
     try {
-        GCK(cudaSetDevice(g->home));
-        GCK(cudaEventCreateWithFlags(&g->ev_user, cudaEventDisableTiming));
-        if (obj_dev) GCK(cudaDeviceSynchronize());  // the peer copies read the matrix after the work queued on the home device
+        CK(cudaSetDevice(g->home));
+        CK(cudaEventCreateWithFlags(&g->ev_user, cudaEventDisableTiming));
+        if (obj_dev) CK(cudaDeviceSynchronize());  // the peer copies read the matrix after the work queued on the home device
         for (int i = 0; i < n_devices; ++i) {
             GroupMember& M = g->m[i];
             M.device = devices[i];
             M.home = M.device == g->home;
             const void* obj = objects;
             if (!M.home) {
-                GCK(cudaSetDevice(M.device));
-                GCK(cudaStreamCreateWithFlags(&M.st, cudaStreamNonBlocking));
-                GCK(cudaEventCreateWithFlags(&M.ev_done, cudaEventDisableTiming));
+                CK(cudaSetDevice(M.device));
+                CK(cudaStreamCreateWithFlags(&M.st, cudaStreamNonBlocking));
+                CK(cudaEventCreateWithFlags(&M.ev_done, cudaEventDisableTiming));
                 if (obj_dev && n_objects > 0 && d > 0) {
                     const size_t bytes = (size_t)n_objects * d * dtype_bytes(dtype);
-                    obj = M.objects.ensure(bytes);
-                    GCK(cudaMemcpyPeer(M.objects.p, M.device, objects, g->home, bytes));
+                    obj = M.objects.ensure_exact(bytes);
+                    CK(cudaMemcpyPeer(M.objects.p, M.device, objects, g->home, bytes));
                 }
             }
             const int rc = b200_rank_create_ex(&M.E, obj, dtype, n_objects, d, distance, M.device, tc_mode, flags);
@@ -373,16 +343,14 @@ int group_create(b200_group** out, const void* objects, int32_t dtype, int64_t n
                 return ret;
             }
             if (!M.home && dtype != B200_DT_F32 && !(flags & B200_F_OBJECTS_16BIT)) {  // widened into the engine's own master copy
-                GCK(cudaSetDevice(M.device));
+                CK(cudaSetDevice(M.device));
                 M.objects.release();
             }
         }
         for (int i = 0; i < n_devices; ++i) g->m[i].worker = std::thread(worker_loop, g, i);
     } catch (const CudaError& ce) {
-        char buf[512];
-        snprintf(buf, sizeof(buf), "b200_rank_group_create: %s failed: %s", ce.what, cudaGetErrorString(ce.e));
         destroy_group(g);
-        return b200_set_error(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, buf);
+        return cuda_fail("b200_rank_group_create", ce);
     } catch (const std::system_error&) {
         destroy_group(g);
         return b200_set_error(B200_E_NOMEM, "b200_rank_group_create: cannot start the worker threads");
@@ -422,7 +390,7 @@ int b200_rank_group_get_info(b200_rank_group* g, b200_rank_info* infos, int64_t*
         GroupMember& M = g->m[i];
         if (const int rc = b200_rank_get_info(M.E, &infos[i])) return rc;
         total += infos[i].hbm_bytes;
-        for (DBuf* b : M.bufs()) total += (int64_t)b->cap;
+        for (DevBuf* b : M.bufs()) total += (int64_t)b->cap;
     }
     if (hbm_bytes) *hbm_bytes = total;
     return B200_OK;
@@ -434,17 +402,17 @@ int b200_rank_group_set_subjects(b200_rank_group* g, const float* subjects, int6
     std::lock_guard<std::mutex> lock(g->mu);
     try {
         if (on_device) {
-            GCK(cudaSetDevice(g->home));
-            GCK(cudaDeviceSynchronize());  // the peer copies read the matrix after the work queued on the home device
+            CK(cudaSetDevice(g->home));
+            CK(cudaDeviceSynchronize());  // the peer copies read the matrix after the work queued on the home device
         }
         for (size_t i = 0; i < g->m.size(); ++i) {
             GroupMember& M = g->m[i];
             const float* src = subjects;
             if (on_device && !M.home) {
-                GCK(cudaSetDevice(M.device));
+                CK(cudaSetDevice(M.device));
                 const size_t bytes = sizeof(float) * (size_t)n_subjects * g->d;
-                src = (const float*)M.subjects.ensure(std::max<size_t>(bytes, 16));
-                if (bytes) GCK(cudaMemcpyPeer(M.subjects.p, M.device, subjects, g->home, bytes));
+                src = (const float*)M.subjects.ensure_exact(std::max<size_t>(bytes, 16));
+                if (bytes) CK(cudaMemcpyPeer(M.subjects.p, M.device, subjects, g->home, bytes));
             }
             if (const int rc = b200_rank_set_subjects(M.E, src, n_subjects, on_device)) {
                 M.rc = rc;
@@ -453,9 +421,7 @@ int b200_rank_group_set_subjects(b200_rank_group* g, const float* subjects, int6
             }
         }
     } catch (const CudaError& ce) {
-        char buf[512];
-        snprintf(buf, sizeof(buf), "b200_rank_group_set_subjects: %s failed: %s", ce.what, cudaGetErrorString(ce.e));
-        return b200_set_error(ce.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, buf);
+        return cuda_fail("b200_rank_group_set_subjects", ce);
     }
     g->n_sub_res = n_subjects;
     g->sub_res_on_device = on_device != 0;
@@ -503,13 +469,11 @@ int b200_rank_group_topk(b200_rank_group* g, const b200_rank_query* q, b200_rank
     if (!user) user = cudaStreamLegacy;
     try {
         if (any_remote && g->from_user) {
-            GCK(cudaSetDevice(g->home));
-            GCK(cudaEventRecord(g->ev_user, user));
+            CK(cudaSetDevice(g->home));
+            CK(cudaEventRecord(g->ev_user, user));
         }
     } catch (const CudaError& ce) {
-        char buf[512];
-        snprintf(buf, sizeof(buf), "b200_rank_group_topk: %s failed: %s", ce.what, cudaGetErrorString(ce.e));
-        return b200_set_error(B200_E_CUDA, buf);
+        return cuda_fail("b200_rank_group_topk", ce);
     }
     {
         std::lock_guard<std::mutex> lk(g->wmu);
@@ -526,14 +490,12 @@ int b200_rank_group_topk(b200_rank_group* g, const b200_rank_query* q, b200_rank
         if (g->m[i].rc != B200_OK) return member_error(g, i, "b200_rank_group_topk");
     try {
         if (any_remote && out_dev) {  // the caller's stream sees the copies back from the other devices
-            GCK(cudaSetDevice(g->home));
+            CK(cudaSetDevice(g->home));
             for (const GroupMember& M : g->m)
-                if (!M.home) GCK(cudaStreamWaitEvent(user, M.ev_done, 0));
+                if (!M.home) CK(cudaStreamWaitEvent(user, M.ev_done, 0));
         }
     } catch (const CudaError& ce) {
-        char buf[512];
-        snprintf(buf, sizeof(buf), "b200_rank_group_topk: %s failed: %s", ce.what, cudaGetErrorString(ce.e));
-        return b200_set_error(B200_E_CUDA, buf);
+        return cuda_fail("b200_rank_group_topk", ce);
     }
     bool first = true;
     for (int i = 0; i < n_mem; ++i) {

@@ -9,59 +9,14 @@
 #include <algorithm>
 #include <climits>
 #include <cstdint>
-#include <cstdio>
 #include <vector>
 
 #include "../../include/b200_rank.h"
+#include "cuda_call.h"
 #include "engine_internal.h"
 #include "pairs_select.cuh"
 
 namespace {
-
-struct PairsError {
-    cudaError_t e;
-    const char* what;
-    int line;
-};
-
-#define PCK(call)                                                     \
-    do {                                                              \
-        cudaError_t e__ = (call);                                     \
-        if (e__ != cudaSuccess) throw PairsError{e__, #call, __LINE__}; \
-    } while (0)
-
-// device allocations of one call, freed when it returns
-struct Scratch {
-    std::vector<void*> bufs;
-    template <typename T>
-    T* get(size_t count) {
-        void* p = nullptr;
-        PCK(cudaMalloc(&p, std::max<size_t>(count * sizeof(T), 16)));
-        bufs.push_back(p);
-        return static_cast<T*>(p);
-    }
-    ~Scratch() {
-        for (void* p : bufs) cudaFree(p);
-    }
-};
-
-struct Events {
-    cudaEvent_t e[7] = {};
-    Events() {
-        for (auto& x : e) PCK(cudaEventCreate(&x));
-    }
-    ~Events() {
-        for (auto& x : e)
-            if (x) cudaEventDestroy(x);
-    }
-    float ms(int a, int b) const {
-        float t = 0.f;
-        PCK(cudaEventElapsedTime(&t, e[a], e[b]));
-        return t;
-    }
-};
-
-int pairs_fail(int code, const char* msg) { return b200_set_error(code, msg); }
 
 size_t score_bytes(int32_t type) { return type == B200_PAIRS_F64 || type == B200_PAIRS_I64 ? 8 : 4; }
 
@@ -76,15 +31,15 @@ extern "C" int b200_rank_topk_pairs(int32_t device, void* stream, int64_t n, con
                                     int32_t score_type, int64_t n_groups, int32_t k, int32_t flags, int64_t* out_pos,
                                     int64_t* out_offsets, b200_rank_stats* stats) {
     using namespace b200;
-    if (n < 0 || n_groups < 0) return pairs_fail(B200_E_INVALID, "b200_rank_topk_pairs: n and n_groups must be >= 0");
-    if (k < 1) return pairs_fail(B200_E_INVALID, "b200_rank_topk_pairs: k must be >= 1");
+    if (n < 0 || n_groups < 0) return b200_set_error(B200_E_INVALID, "b200_rank_topk_pairs: n and n_groups must be >= 0");
+    if (k < 1) return b200_set_error(B200_E_INVALID, "b200_rank_topk_pairs: k must be >= 1");
     if (score_type < B200_PAIRS_F64 || score_type > B200_PAIRS_I32)
-        return pairs_fail(B200_E_INVALID, "b200_rank_topk_pairs: unknown score type");
+        return b200_set_error(B200_E_INVALID, "b200_rank_topk_pairs: unknown score type");
     if (flags & ~(B200_Q_INPUTS_ON_DEVICE | B200_Q_OUTPUTS_ON_DEVICE))
-        return pairs_fail(B200_E_INVALID, "b200_rank_topk_pairs: only B200_Q_INPUTS_ON_DEVICE / B200_Q_OUTPUTS_ON_DEVICE are accepted");
-    if (!out_offsets) return pairs_fail(B200_E_INVALID, "b200_rank_topk_pairs: out_offsets is NULL");
-    if (n > 0 && (!group_codes || !scores)) return pairs_fail(B200_E_INVALID, "b200_rank_topk_pairs: group_codes / scores are NULL");
-    if (n > 0 && n_groups > 0 && !out_pos) return pairs_fail(B200_E_INVALID, "b200_rank_topk_pairs: out_pos is NULL");
+        return b200_set_error(B200_E_INVALID, "b200_rank_topk_pairs: only B200_Q_INPUTS_ON_DEVICE / B200_Q_OUTPUTS_ON_DEVICE are accepted");
+    if (!out_offsets) return b200_set_error(B200_E_INVALID, "b200_rank_topk_pairs: out_offsets is NULL");
+    if (n > 0 && (!group_codes || !scores)) return b200_set_error(B200_E_INVALID, "b200_rank_topk_pairs: group_codes / scores are NULL");
+    if (n > 0 && n_groups > 0 && !out_pos) return b200_set_error(B200_E_INVALID, "b200_rank_topk_pairs: out_pos is NULL");
     const bool in_dev = flags & B200_Q_INPUTS_ON_DEVICE, out_dev = flags & B200_Q_OUTPUTS_ON_DEVICE;
     const int64_t G = n_groups;
     b200_rank_stats S{};
@@ -92,28 +47,27 @@ extern "C" int b200_rank_topk_pairs(int32_t device, void* stream, int64_t n, con
     S.k_out = k;
     S.n_chunks = 1;
     try {
-        PCK(cudaSetDevice(device));
+        CK(cudaSetDevice(device));
         int sms = 0;
-        PCK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+        CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
         cudaStream_t st = stream ? reinterpret_cast<cudaStream_t>(stream) : cudaStreamLegacy;
-        Scratch mem;
-        Events ev;
+        CallScratch<7> mem(st);
         int launches = 0;
 
         // ---- order keys and grouping
-        PCK(cudaEventRecord(ev.e[0], st));
+        CK(cudaEventRecord(mem.ev[0], st));
         const int64_t* codes = group_codes;
         const void* sc = scores;
         if (!in_dev && n > 0) {
             int64_t* d_codes = mem.get<int64_t>(n);
             void* d_sc = mem.get<uint8_t>(score_bytes(score_type) * n);
-            PCK(cudaMemcpyAsync(d_codes, group_codes, sizeof(int64_t) * n, cudaMemcpyHostToDevice, st));
-            PCK(cudaMemcpyAsync(d_sc, scores, score_bytes(score_type) * n, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(d_codes, group_codes, sizeof(int64_t) * n, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(d_sc, scores, score_bytes(score_type) * n, cudaMemcpyHostToDevice, st));
             S.h2d_bytes = (int64_t)((sizeof(int64_t) + score_bytes(score_type)) * n);
             codes = d_codes;
             sc = d_sc;
         }
-        PCK(cudaEventRecord(ev.e[1], st));
+        CK(cudaEventRecord(mem.ev[1], st));
         int64_t* count = mem.get<int64_t>(G + 1);  // rows per group, then the scatter's cursors
         int64_t* seg_off = mem.get<int64_t>(G + 1);
         int64_t* kept = mem.get<int64_t>(G + 1);
@@ -123,38 +77,38 @@ extern "C" int b200_rank_topk_pairs(int32_t device, void* stream, int64_t n, con
         int64_t* class_off = small + PAIRS_N_CLASSES;
         int64_t* class_cursor = small + 2 * PAIRS_N_CLASSES;
         int* bad = reinterpret_cast<int*>(small + 3 * PAIRS_N_CLASSES);
-        PCK(cudaMemsetAsync(count, 0, sizeof(int64_t) * (G + 1), st));
-        PCK(cudaMemsetAsync(kept, 0, sizeof(int64_t) * (G + 1), st));
-        PCK(cudaMemsetAsync(small, 0, sizeof(int64_t) * (3 * PAIRS_N_CLASSES + 1), st));
+        CK(cudaMemsetAsync(count, 0, sizeof(int64_t) * (G + 1), st));
+        CK(cudaMemsetAsync(kept, 0, sizeof(int64_t) * (G + 1), st));
+        CK(cudaMemsetAsync(small, 0, sizeof(int64_t) * (3 * PAIRS_N_CLASSES + 1), st));
         if (n > 0) {
             pairs_count_kernel<<<grid_stride(n, sms), 256, 0, st>>>(n, codes, G, reinterpret_cast<unsigned long long*>(count), bad);
-            PCK(cudaGetLastError());
+            CK(cudaGetLastError());
             ++launches;
         }
         if (G > 0) {
             pairs_group_kernel<<<grid_stride(G, sms), 256, 0, st>>>(G, k, reinterpret_cast<const unsigned long long*>(count), kept,
                                                                     reinterpret_cast<unsigned long long*>(class_count));
-            PCK(cudaGetLastError());
+            CK(cudaGetLastError());
             ++launches;
         }
         size_t scan_bytes = 0;
-        PCK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, count, seg_off, G + 1, st));
+        CK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, count, seg_off, G + 1, st));
         void* scan_tmp = mem.get<uint8_t>(scan_bytes);
-        PCK(cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, count, seg_off, G + 1, st));
-        PCK(cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, kept, out_off, G + 1, st));
+        CK(cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, count, seg_off, G + 1, st));
+        CK(cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, kept, out_off, G + 1, st));
         launches += 2;
         int64_t h_small[PAIRS_N_CLASSES + 1] = {};
         int h_bad = 0;
         int64_t total_out = 0;
-        PCK(cudaMemcpyAsync(h_small, class_count, sizeof(int64_t) * PAIRS_N_CLASSES, cudaMemcpyDeviceToHost, st));
-        PCK(cudaMemcpyAsync(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
-        PCK(cudaMemcpyAsync(&total_out, out_off + G, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-        PCK(cudaEventRecord(ev.e[2], st));
-        PCK(cudaStreamSynchronize(st));
-        if (h_bad) return pairs_fail(B200_E_INVALID, "b200_rank_topk_pairs: a group code lies outside [-1, n_groups)");
+        CK(cudaMemcpyAsync(h_small, class_count, sizeof(int64_t) * PAIRS_N_CLASSES, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(&total_out, out_off + G, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+        CK(cudaEventRecord(mem.ev[2], st));
+        CK(cudaStreamSynchronize(st));
+        if (h_bad) return b200_set_error(B200_E_INVALID, "b200_rank_topk_pairs: a group code lies outside [-1, n_groups)");
         const int64_t n_large = h_small[PAIRS_N_CLASSES - 1];
         if (n_large > 0 && total_out > INT_MAX)
-            return pairs_fail(B200_E_NOMEM, "b200_rank_topk_pairs: more than 2^31 - 1 output rows with groups beyond shared memory");
+            return b200_set_error(B200_E_NOMEM, "b200_rank_topk_pairs: more than 2^31 - 1 output rows with groups beyond shared memory");
         int64_t h_class_off[PAIRS_N_CLASSES];
         for (int64_t c = 0, run = 0; c < PAIRS_N_CLASSES; run += h_small[c++]) h_class_off[c] = run;
         // every allocation before the first output write: a refusal leaves the outputs untouched
@@ -174,42 +128,42 @@ extern "C" int b200_rank_topk_pairs(int32_t device, void* stream, int64_t n, con
             lbeg = mem.get<int64_t>(n_large);
             lend = mem.get<int64_t>(n_large);
             size_t a = 0, b = 0;
-            PCK(cub::DeviceSegmentedSort::SortPairs(nullptr, a, sp0, sp1, sk0, sk1, (int)total_out, (int)n_large, lbeg, lend, st));
-            PCK(cub::DeviceSegmentedSort::StableSortPairsDescending(nullptr, b, sk1, sk0, sp1, sp0, (int)total_out, (int)n_large, lbeg, lend, st));
+            CK(cub::DeviceSegmentedSort::SortPairs(nullptr, a, sp0, sp1, sk0, sk1, (int)total_out, (int)n_large, lbeg, lend, st));
+            CK(cub::DeviceSegmentedSort::StableSortPairsDescending(nullptr, b, sk1, sk0, sp1, sp0, (int)total_out, (int)n_large, lbeg, lend, st));
             sort_bytes = std::max(a, b);
             sort_tmp = mem.get<uint8_t>(sort_bytes);
         }
 
-        PCK(cudaEventRecord(ev.e[3], st));
-        PCK(cudaMemcpyAsync(class_off, h_class_off, sizeof(h_class_off), cudaMemcpyHostToDevice, st));
-        PCK(cudaMemsetAsync(count, 0, sizeof(int64_t) * (G + 1), st));
+        CK(cudaEventRecord(mem.ev[3], st));
+        CK(cudaMemcpyAsync(class_off, h_class_off, sizeof(h_class_off), cudaMemcpyHostToDevice, st));
+        CK(cudaMemsetAsync(count, 0, sizeof(int64_t) * (G + 1), st));
         if (G > 0) {
             pairs_classify_kernel<<<grid_stride(G, sms), 256, 0, st>>>(G, seg_off, class_off, reinterpret_cast<unsigned long long*>(class_cursor),
                                                                        class_list);
-            PCK(cudaGetLastError());
+            CK(cudaGetLastError());
             ++launches;
         }
         if (n > 0) {
             pairs_scatter_kernel<<<grid_stride(n, sms), 256, 0, st>>>(n, codes, sc, score_type, seg_off,
                                                                       reinterpret_cast<unsigned long long*>(count), seg_key, seg_pos);
-            PCK(cudaGetLastError());
+            CK(cudaGetLastError());
             ++launches;
         }
-        PCK(cudaEventRecord(ev.e[4], st));
+        CK(cudaEventRecord(mem.ev[4], st));
 
         // ---- per-group selection, one launch per size class
         if (h_small[0] > 0) {
             pairs_warp_kernel<<<(unsigned)((h_small[0] + 7) / 8), 256, 0, st>>>(h_small[0], class_list + h_class_off[0], seg_off, out_off,
                                                                                 seg_key, seg_pos, dpos);
-            PCK(cudaGetLastError());
+            CK(cudaGetLastError());
             ++launches;
         }
         auto cta = [&](int c, auto kernel, int cap, int threads) {
             if (h_small[c] == 0) return;
             const int smem = cap * 16;
-            PCK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+            CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
             kernel<<<(unsigned)h_small[c], threads, smem, st>>>(class_list + h_class_off[c], seg_off, out_off, seg_key, seg_pos, dpos);
-            PCK(cudaGetLastError());
+            CK(cudaGetLastError());
             ++launches;
         };
         cta(1, pairs_cta_kernel<256, 128>, 256, 128);
@@ -219,38 +173,35 @@ extern "C" int b200_rank_topk_pairs(int32_t device, void* stream, int64_t n, con
             const int64_t* list = class_list + h_class_off[4];
             pairs_select_kernel<<<(unsigned)n_large, PAIRS_SELECT_THREADS, 0, st>>>(list, seg_off, out_off, seg_key, seg_pos, sk0, sp0,
                                                                                     lbeg, lend);
-            PCK(cudaGetLastError());
+            CK(cudaGetLastError());
             // position ascending (positions are unique), then key descending, stable: (key desc, position asc)
-            PCK(cub::DeviceSegmentedSort::SortPairs(sort_tmp, sort_bytes, sp0, sp1, sk0, sk1, (int)total_out, (int)n_large, lbeg, lend, st));
-            PCK(cub::DeviceSegmentedSort::StableSortPairsDescending(sort_tmp, sort_bytes, sk1, sk0, sp1, sp0, (int)total_out, (int)n_large,
-                                                                    lbeg, lend, st));
+            CK(cub::DeviceSegmentedSort::SortPairs(sort_tmp, sort_bytes, sp0, sp1, sk0, sk1, (int)total_out, (int)n_large, lbeg, lend, st));
+            CK(cub::DeviceSegmentedSort::StableSortPairsDescending(sort_tmp, sort_bytes, sk1, sk0, sp1, sp0, (int)total_out, (int)n_large,
+                                                                   lbeg, lend, st));
             pairs_copy_kernel<<<(unsigned)n_large, 256, 0, st>>>(list, out_off, sp0, dpos);
-            PCK(cudaGetLastError());
+            CK(cudaGetLastError());
             launches += 4;
         }
-        PCK(cudaEventRecord(ev.e[5], st));
+        CK(cudaEventRecord(mem.ev[5], st));
 
         // ---- outputs
         if (out_dev) {
-            PCK(cudaMemcpyAsync(out_offsets, out_off, sizeof(int64_t) * (G + 1), cudaMemcpyDeviceToDevice, st));
+            CK(cudaMemcpyAsync(out_offsets, out_off, sizeof(int64_t) * (G + 1), cudaMemcpyDeviceToDevice, st));
         } else {
-            PCK(cudaMemcpyAsync(out_offsets, out_off, sizeof(int64_t) * (G + 1), cudaMemcpyDeviceToHost, st));
-            if (total_out > 0) PCK(cudaMemcpyAsync(out_pos, dpos, sizeof(int64_t) * total_out, cudaMemcpyDeviceToHost, st));
+            CK(cudaMemcpyAsync(out_offsets, out_off, sizeof(int64_t) * (G + 1), cudaMemcpyDeviceToHost, st));
+            if (total_out > 0) CK(cudaMemcpyAsync(out_pos, dpos, sizeof(int64_t) * total_out, cudaMemcpyDeviceToHost, st));
             S.d2h_bytes = (int64_t)sizeof(int64_t) * (G + 1 + total_out);
         }
-        PCK(cudaEventRecord(ev.e[6], st));
-        PCK(cudaStreamSynchronize(st));
-        S.ms_h2d = ev.ms(0, 1);
-        S.ms_main = ev.ms(1, 2) + ev.ms(3, 4);
-        S.ms_select = ev.ms(4, 5);
-        S.ms_d2h = out_dev ? 0.f : ev.ms(5, 6);
-        S.ms_total = ev.ms(0, 6);
+        CK(cudaEventRecord(mem.ev[6], st));
+        CK(cudaStreamSynchronize(st));
+        S.ms_h2d = mem.ms(0, 1);
+        S.ms_main = mem.ms(1, 2) + mem.ms(3, 4);
+        S.ms_select = mem.ms(4, 5);
+        S.ms_d2h = out_dev ? 0.f : mem.ms(5, 6);
+        S.ms_total = mem.ms(0, 6);
         S.n_launches = launches;
-    } catch (const PairsError& pe) {
-        cudaGetLastError();  // a failed allocation must not surface in a later call
-        char msg[512];
-        snprintf(msg, sizeof(msg), "b200_rank_topk_pairs: %s failed at line %d: %s", pe.what, pe.line, cudaGetErrorString(pe.e));
-        return pairs_fail(pe.e == cudaErrorMemoryAllocation ? B200_E_NOMEM : B200_E_CUDA, msg);
+    } catch (const CudaError& ce) {
+        return cuda_fail("b200_rank_topk_pairs", ce);
     }
     if (stats) *stats = S;
     return B200_OK;
