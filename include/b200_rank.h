@@ -149,7 +149,8 @@ typedef struct b200_rank_stats {
                               * rows (object_rows): one radix-select launch per row chunk over the rows in place, 5 = candidate
                               * sets (b200_rank_topk_candidates): ms_main = scoring, ms_select = selection, 6 = scored pairs
                               * (b200_rank_topk_pairs), 7 = a shared list minus viewed ids (b200_rank_topk_list),
-                              * 8 = per-category lists minus viewed ids, mixed (b200_rank_topk_list_mix) */
+                              * 8 = per-category lists minus viewed ids, mixed (b200_rank_topk_list_mix), 9 = ItemKNN user
+                              * scores from a neighbour matrix (b200_rank_topk_knn): ms_main = scoring, ms_select = selection */
     int32_t tc_dtype;        /* B200_TC_FP16 / B200_TC_BF16 when path == 1 */
     int32_t k_out;           /* columns of the output arrays */
     int32_t k_cand;          /* candidates kept per row and item split by the tensor-core pass */
@@ -349,6 +350,40 @@ int b200_rank_topk_list_mix(int32_t device, int32_t n_lists, const int64_t* list
                             const int32_t* quota, int32_t mixing, int64_t n_rows, const int64_t* csr_indptr,
                             const int32_t* csr_indices, int32_t k, int32_t* out_pos, int32_t* out_counts,
                             b200_rank_stats* stats /* nullable */);
+
+/* ItemKNN user scores (stats.path = 9; no engine): for each row, the k best items of the user scores implicit's
+ * `ItemItemRecommender.recommend` accumulates from the neighbour matrix S, as `ImplicitItemKNNWrapperModel._recommend_u2i`
+ * (rectools/models/implicit_knn.py:152-211) ranks them per user.
+ *   s_*        S, n_items x n_items CSR: s_indptr[0] = 0, monotone; ids in [0, n_items), each at most once per row, in any
+ *              order; finite fp64 values.
+ *   u_*        row r's weighted entries (j_e, w_e), e = u_indptr[r] .. u_indptr[r+1]), in that order: ids in [0, n_items),
+ *              finite fp32 weights, repeats allowed.
+ *   f_*        row r's filter ids f_indices[f_indptr[r] .. f_indptr[r+1]), ascending within the row, any int32 value;
+ *              f_indptr NULL: no filter.
+ *   whitelist  [n_whitelist] strictly ascending ids in [0, n_items); n_whitelist < 0: no whitelist (0: nothing is kept).
+ *   Row r touches T_r, the union of the S rows of its entries, and item i of T_r scores
+ *   s_r(i) = (((0 + p_1) + p_2) + ...) over the entries whose S row holds i, in entry order, p = S[j_e, i] * (double)w_e,
+ *   each product and each sum rounded to fp64 (no fused multiply-add).  A zero or negative score still counts.  The
+ *   candidates are T_r minus the row's filter ids, within the whitelist; the row keeps min(k, their count), ordered by
+ *   (score desc, id asc) on the fp64 value.
+ *   out_ids    [n_rows, k] int32, unfilled slots -1; out_scores [n_rows, k] fp64, unfilled slots 0; out_counts [n_rows].
+ * Host buffers only.  S and the whitelist are uploaded once per call; rows are ranked in chunks of whole rows within
+ * 1 GiB of device memory (B200_KNN_CHUNK_ROWS=n caps a chunk's rows), on a stream the call creates and destroys.  A row
+ * whose S rows hold at most 3072 entries in all accumulates in shared memory; a larger one in a dense fp64 row of
+ * n_items in global scratch (at most 256 MiB for the call).  Each chunk's selection is b200_rank_topk_pairs (path 6) on
+ * the device buffers.  n_rows = 0 writes nothing and does not touch the device.
+ * Refused, with every output untouched:
+ *   B200_E_INVALID  n_items or n_rows < 0, n_items > 2^31 - 1, k < 1, NULL arrays that have entries, an indptr that does
+ *                   not start at 0 or is not monotone, ids out of range, an item twice in one S row, a non-finite S value
+ *                   or weight, filter ids not ascending within a row, a whitelist not strictly ascending;
+ *   B200_E_NOMEM    a row that alone needs more than a chunk's 1 GiB, or a failed device allocation.
+ * stats: ms_main = the scoring kernels, ms_select = path 6 and the gather into the outputs, ms_h2d / ms_d2h = the
+ * copies, summed over chunks; ms_total = their sum. */
+int b200_rank_topk_knn(int32_t device, int64_t n_items, const int64_t* s_indptr, const int32_t* s_indices,
+                       const double* s_data, int64_t n_rows, const int64_t* u_indptr, const int32_t* u_indices,
+                       const float* u_data, const int64_t* f_indptr, const int32_t* f_indices, const int32_t* whitelist,
+                       int64_t n_whitelist, int32_t k, int32_t* out_ids, double* out_scores, int32_t* out_counts,
+                       b200_rank_stats* stats /* nullable */);
 
 /* Merge `n_lists` per-shard results (device pointers, each [n_rows, k] / [n_rows], list l at base + l * stride) into
  * the global top-k ordered by (score desc, id asc).  Runs on `stream` of `device`. */

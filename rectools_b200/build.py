@@ -13,8 +13,8 @@ import typing as tp
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200rank.so")
-SOURCES = ["engine.cu", "group.cu", "pairs.cu", "list.cu", "list_mix.cu"]
-HEADERS = ["cuda_call.h", "common.cuh", "sizes.h", "plan.h", "group_plan.h", "engine_internal.h", "order_key.h", "large_k_select.cuh", "row_select.cuh", "cand_select.cuh", "cand_prep.cuh", "prep.cuh", "select.cuh", "sparse.cuh", "tc_common.cuh", "fused_topk.cuh", "pairs_select.cuh", "list_plan.h", "list_select.cuh", "list_call.h", "list_mix_plan.h", "list_mix.cuh", os.path.join("..", "..", "include", "b200_rank.h")]
+SOURCES = ["engine.cu", "group.cu", "pairs.cu", "list.cu", "list_mix.cu", "knn.cu"]
+HEADERS = ["cuda_call.h", "common.cuh", "sizes.h", "plan.h", "group_plan.h", "engine_internal.h", "order_key.h", "large_k_select.cuh", "row_select.cuh", "cand_select.cuh", "cand_prep.cuh", "prep.cuh", "select.cuh", "sparse.cuh", "tc_common.cuh", "fused_topk.cuh", "pairs_select.cuh", "list_plan.h", "list_select.cuh", "list_call.h", "list_mix_plan.h", "list_mix.cuh", "knn.cuh", "knn_plan.h", os.path.join("..", "..", "include", "b200_rank.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -169,6 +169,7 @@ _EASE_I2I_KEY = "EASEModel._recommend_i2i"
 _RERANK_KEY = "Reranker.recommend"
 _POPULAR_KEY = "PopularModel._recommend_u2i"
 _POPULAR_IN_CATEGORY_KEY = "PopularInCategoryModel._recommend_u2i"
+_ITEM_KNN_KEY = "ImplicitItemKNNWrapperModel._recommend_u2i/_recommend_i2i"
 # the transformer modules whose module-level `TorchRanker` ranks: u2i (`DistanceSimilarityModule._recommend_u2i`,
 # similarity.py:127-132) and i2i (`TransformerLightningModule._recommend_i2i`, lightning.py:440-442)
 _TRANSFORMER_MODULES = ("rectools.models.nn.transformers.similarity", "rectools.models.nn.transformers.lightning")
@@ -212,7 +213,7 @@ def ease_recommend_i2i(self, target_ids, dataset, k, sorted_item_ids_to_recommen
 
 
 def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = True, rerank: bool = False,
-            popular: bool = False, transformers: bool = False, popular_in_category: bool = False,
+            popular: bool = False, transformers: bool = False, popular_in_category: bool = False, item_knn: bool = False,
             ranker_factory: tp.Optional[tp.Callable[..., tp.Any]] = None) -> None:
     """Route `VectorModel` (ALS / PureSVD / LightFM / BPR / DSSM) and `EASEModel` ranking (u2i and i2i) through the B200
     engine.
@@ -237,6 +238,11 @@ def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = T
     one `PopularModel` call per category and the mixing in pandas, to
     `rectools_b200.popular.popular_in_category_recommend_u2i` on the home device: every category's list and the mixing of
     each user in one kernel pass.  `popular=True` alone leaves this method as it is.
+
+    `item_knn`: also rebind `ImplicitItemKNNWrapperModel._recommend_u2i` and `._recommend_i2i`
+    (rectools/models/implicit_knn.py:152-255), one implicit `recommend` call or one numpy selection per target, to
+    `rectools_b200.item_knn.item_knn_recommend_u2i` / `item_knn_recommend_i2i` on the home device: every user's scores
+    accumulated from `model.similarity` in one sparse pass, and every target's neighbour row selected in one call.
 
     `transformers`: also rebind the module-level `TorchRanker` of rectools.models.nn.transformers.similarity (u2i of
     `DistanceSimilarityModule`) and of rectools.models.nn.transformers.lightning (item-to-item of
@@ -327,6 +333,27 @@ def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = T
         _in_category_recommend_u2i.__doc__ = PopularInCategoryModel._recommend_u2i.__doc__  # pylint: disable=protected-access
         _ORIGINALS[_POPULAR_IN_CATEGORY_KEY] = PopularInCategoryModel.__dict__["_recommend_u2i"]
         PopularInCategoryModel._recommend_u2i = _in_category_recommend_u2i  # pylint: disable=protected-access
+    if item_knn and _ITEM_KNN_KEY not in _ORIGINALS:
+        from rectools.models.implicit_knn import ImplicitItemKNNWrapperModel
+
+        from .item_knn import item_knn_recommend_i2i, item_knn_recommend_u2i
+
+        def _knn_recommend_u2i(self, user_ids, dataset, k, filter_viewed, sorted_item_ids_to_recommend):
+            home = B200ImplicitRanker.default_device
+            return item_knn_recommend_u2i(self, user_ids, dataset, k, filter_viewed, sorted_item_ids_to_recommend,
+                                          device=home[0] if isinstance(home, tuple) else home)
+
+        def _knn_recommend_i2i(self, target_ids, dataset, k, sorted_item_ids_to_recommend):
+            home = B200ImplicitRanker.default_device
+            return item_knn_recommend_i2i(self, target_ids, dataset, k, sorted_item_ids_to_recommend,
+                                          device=home[0] if isinstance(home, tuple) else home)
+
+        cls = ImplicitItemKNNWrapperModel
+        _knn_recommend_u2i.__doc__ = cls._recommend_u2i.__doc__  # pylint: disable=protected-access
+        _knn_recommend_i2i.__doc__ = cls._recommend_i2i.__doc__  # pylint: disable=protected-access
+        _ORIGINALS[_ITEM_KNN_KEY] = {name: cls.__dict__[name] for name in ("_recommend_u2i", "_recommend_i2i")}
+        cls._recommend_u2i = _knn_recommend_u2i  # pylint: disable=protected-access
+        cls._recommend_i2i = _knn_recommend_i2i  # pylint: disable=protected-access
     if transformer_modules:
         bound = transformer_ranker(ranker_factory or B200TorchRanker)
         for mod in transformer_modules:
@@ -359,6 +386,11 @@ def uninstall() -> None:
         from rectools.models.popular_in_category import PopularInCategoryModel
 
         PopularInCategoryModel._recommend_u2i = _ORIGINALS.pop(_POPULAR_IN_CATEGORY_KEY)  # pylint: disable=protected-access
+    if _ITEM_KNN_KEY in _ORIGINALS:
+        from rectools.models.implicit_knn import ImplicitItemKNNWrapperModel
+
+        for name, orig in _ORIGINALS.pop(_ITEM_KNN_KEY).items():
+            setattr(ImplicitItemKNNWrapperModel, name, orig)
     if _EASE_I2I_KEY in _ORIGINALS:
         from rectools.models.ease import EASEModel
 
