@@ -150,7 +150,9 @@ typedef struct b200_rank_stats {
                               * sets (b200_rank_topk_candidates): ms_main = scoring, ms_select = selection, 6 = scored pairs
                               * (b200_rank_topk_pairs), 7 = a shared list minus viewed ids (b200_rank_topk_list),
                               * 8 = per-category lists minus viewed ids, mixed (b200_rank_topk_list_mix), 9 = ItemKNN user
-                              * scores from a neighbour matrix (b200_rank_topk_knn): ms_main = scoring, ms_select = selection */
+                              * scores from a neighbour matrix (b200_rank_topk_knn): ms_main = scoring, ms_select = selection,
+                              * 10 = classification and ranking metrics of a reco table (b200_rank_metrics): ms_main = the join
+                              * and the per-user reductions */
     int32_t tc_dtype;        /* B200_TC_FP16 / B200_TC_BF16 when path == 1 */
     int32_t k_out;           /* columns of the output arrays */
     int32_t k_cand;          /* candidates kept per row and item split by the tensor-core pass */
@@ -384,6 +386,47 @@ int b200_rank_topk_knn(int32_t device, int64_t n_items, const int64_t* s_indptr,
                        const float* u_data, const int64_t* f_indptr, const int32_t* f_indices, const int32_t* whitelist,
                        int64_t n_whitelist, int32_t k, int32_t* out_ids, double* out_scores, int32_t* out_counts,
                        b200_rank_stats* stats /* nullable */);
+
+/* Classification and ranking metrics of a reco table (stats.path = 10; no engine): the per-user counts and sums from which
+ * RecTools' `calc_metrics` (rectools/metrics/scoring.py:37-223) computes Precision, Recall, F1Beta, HitRate, Accuracy, MCC,
+ * NDCG, MRR and MAP, without its pandas join (`merge_reco`, rectools/metrics/base.py:81-103) and groupbys.
+ *   inter_*     [n_inter] the test interactions (user, item), int64, in their row order; repeats allowed.
+ *   reco_*      [n_reco] the reco table (user, item, rank), int64; each (user, item) pair at most once, ranks >= 1.
+ *   ks          [n_k] strictly ascending k values in [1, 2^31 - 1].
+ *   ndcg_*      n_ndcg term tables: table t is ndcg_terms[ndcg_offsets[t] .. ndcg_offsets[t + 1]), at least one term, the
+ *               term of rank r = 1, 2, ...; a rank past the table's end has the term 0.0.
+ *   Interaction row j is a hit of rank r when the reco table holds its pair with rank r, else a miss.  The U distinct test
+ *   users come out in ascending id (out_users), each with:
+ *     out_liked       its interaction rows;
+ *     out_min_rank    the smallest rank of its hits, 0 with none;
+ *     out_tp          [n_k] per k its hits of rank <= k (rows counted with repeats);
+ *     out_ndcg        [n_ndcg] per table, pandas' compensated group sum (Kahan: y = v - c, t = s + y, c = (t - s) - y, a NaN
+ *                     c reset to 0, s = t; NaN terms skipped) of the terms of its hits in row order, each fp64 operation
+ *                     rounded (no contraction); a user with no hit gets 0.0;
+ *     out_map         [n_k] (nullable: no MAP stage) per k the sum over its distinct hit ranks r <= k, ascending, of
+ *                     C(r) / r, C(r) = its hits of rank <= r with repeats; summed as np.add.reduceat does (the first
+ *                     precision plus numpy's pairwise sum of the others), 0.0 with none;
+ *   and out_first_order [U]: the positions in out_users of the users in order of their first interaction row.
+ *   Per-k and per-table outputs are rows of stride n_inter (out_tp[q * n_inter + s]); every output holds n_inter entries
+ *   per row, of which the first U = *out_n_users are written.
+ *   out_flags   bit 0: a (user, item) pair twice in the reco table; bit 1: a rank below 1.  With a flag set nothing else is
+ *               computed and *out_n_users = 0.
+ * Host buffers only, on `stream` (NULL: a stream of the call's own), all device memory allocated per call (the bytes of
+ * metrics_plan.h: about 100 B per interaction row plus 16 B per k and 8 B per table, and 24 B per reco row plus 8 B per
+ * table slot, as a hash table of the smallest power of two >= 2 x n_reco slots).  n_inter = 0 writes the count (0) and
+ * the flags without touching the device.
+ * Refused, with every output untouched:
+ *   B200_E_INVALID  n_inter, n_reco, n_k or n_ndcg < 0, n_inter or n_reco > 2^31 - 1, NULL arrays that have entries, a k
+ *                   outside [1, 2^31 - 1] or ks not strictly ascending, out_map with n_k = 0, an NDCG table with no term or
+ *                   ndcg_offsets[0] != 0;
+ *   B200_E_NOMEM    a failed device allocation.
+ * stats: ms_h2d / ms_main / ms_d2h = the uploads, the kernels and CUB passes, the copies back; ms_total = their sum. */
+int b200_rank_metrics(int32_t device, void* stream, int64_t n_inter, const int64_t* inter_users, const int64_t* inter_items,
+                      int64_t n_reco, const int64_t* reco_users, const int64_t* reco_items, const int64_t* reco_ranks,
+                      int32_t n_k, const int64_t* ks, int32_t n_ndcg, const int64_t* ndcg_offsets, const double* ndcg_terms,
+                      int64_t* out_n_users, int64_t* out_users, int64_t* out_first_order, int64_t* out_liked,
+                      int64_t* out_min_rank, int64_t* out_tp, double* out_map, double* out_ndcg, int32_t* out_flags,
+                      b200_rank_stats* stats /* nullable */);
 
 /* Merge `n_lists` per-shard results (device pointers, each [n_rows, k] / [n_rows], list l at base + l * stride) into
  * the global top-k ordered by (score desc, id asc).  Runs on `stream` of `device`. */

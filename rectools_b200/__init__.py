@@ -10,6 +10,8 @@ Public surface (host-side mirror of `rectools.models.rank`):
   * `rank_list()`                         -- a shared ordered list minus each row's viewed ids (`PopularModel`, install(popular=True))
   * `rank_list_mix()`                     -- per-category lists minus viewed ids, mixed (`PopularInCategoryModel`,
                                              install(popular_in_category=True))
+  * `calc_metrics()`                      -- RecTools' `calc_metrics` with classification and ranking metrics from one device
+                                             join (install(metrics=True))
   * `ShardedB200Ranker`                   -- item-sharded multi-GPU ranking (one process per GPU, NCCL all-gather + merge)
 The CUDA library is `rectools_b200/libb200rank.so` (C ABI: include/b200_rank.h); build it with
 `python -m rectools_b200.build`.  There is no CPU fallback.
@@ -19,11 +21,13 @@ from .integration import B200ImplicitRanker, B200TorchRanker, install, uninstall
 from .recommend import recommend, recommend_to_items  # noqa: F401
 from .rerank import rank_pairs, reranker_recommend  # noqa: F401
 from .popular import rank_list, rank_list_mix  # noqa: F401
+from .metrics import calc_metrics  # noqa: F401
 
 __all__ = [
     "B200Ranker",
     "B200ImplicitRanker",
     "B200TorchRanker",
+    "calc_metrics",
     "Distance",
     "Engine",
     "EngineGroup",

@@ -36,6 +36,7 @@ EXPORTS = (
     "b200_rank_topk_list",
     "b200_rank_topk_list_mix",
     "b200_rank_topk_knn",
+    "b200_rank_metrics",
     "b200_rank_peer_export",
     "b200_rank_peer_import",
     "b200_rank_get_snapshot",
@@ -201,6 +202,9 @@ def load() -> C.CDLL:
     lib.b200_rank_topk_list_mix.argtypes = [i32, i32, vp, vp, vp, i32, i64, vp, vp, i32, vp, vp, C.POINTER(Stats)]
     lib.b200_rank_topk_knn.restype = C.c_int
     lib.b200_rank_topk_knn.argtypes = [i32, i64, vp, vp, vp, i64, vp, vp, vp, vp, vp, vp, i64, i32, vp, vp, vp, C.POINTER(Stats)]
+    lib.b200_rank_metrics.restype = C.c_int
+    lib.b200_rank_metrics.argtypes = [i32, vp, i64, vp, vp, i64, vp, vp, vp, i32, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,
+                                      C.POINTER(Stats)]
     lib.b200_rank_peer_export.restype = C.c_int
     lib.b200_rank_peer_export.argtypes = [vp, i64, vp]
     lib.b200_rank_peer_import.restype = C.c_int

@@ -170,6 +170,10 @@ _RERANK_KEY = "Reranker.recommend"
 _POPULAR_KEY = "PopularModel._recommend_u2i"
 _POPULAR_IN_CATEGORY_KEY = "PopularInCategoryModel._recommend_u2i"
 _ITEM_KNN_KEY = "ImplicitItemKNNWrapperModel._recommend_u2i/_recommend_i2i"
+_METRICS_KEY = "calc_metrics"
+# the modules whose attribute `calc_metrics` install(metrics=True) rebinds: the definition, the package's re-export and
+# `cross_validate`'s import (rectools/model_selection/cross_validate.py:20)
+_METRICS_MODULES = ("rectools.metrics.scoring", "rectools.metrics", "rectools.model_selection.cross_validate")
 # the transformer modules whose module-level `TorchRanker` ranks: u2i (`DistanceSimilarityModule._recommend_u2i`,
 # similarity.py:127-132) and i2i (`TransformerLightningModule._recommend_i2i`, lightning.py:440-442)
 _TRANSFORMER_MODULES = ("rectools.models.nn.transformers.similarity", "rectools.models.nn.transformers.lightning")
@@ -214,7 +218,7 @@ def ease_recommend_i2i(self, target_ids, dataset, k, sorted_item_ids_to_recommen
 
 def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = True, rerank: bool = False,
             popular: bool = False, transformers: bool = False, popular_in_category: bool = False, item_knn: bool = False,
-            ranker_factory: tp.Optional[tp.Callable[..., tp.Any]] = None) -> None:
+            metrics: bool = False, ranker_factory: tp.Optional[tp.Callable[..., tp.Any]] = None) -> None:
     """Route `VectorModel` (ALS / PureSVD / LightFM / BPR / DSSM) and `EASEModel` ranking (u2i and i2i) through the B200
     engine.
 
@@ -243,6 +247,12 @@ def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = T
     (rectools/models/implicit_knn.py:152-255), one implicit `recommend` call or one numpy selection per target, to
     `rectools_b200.item_knn.item_knn_recommend_u2i` / `item_knn_recommend_i2i` on the home device: every user's scores
     accumulated from `model.similarity` in one sparse pass, and every target's neighbour row selected in one call.
+
+    `metrics`: also rebind the module attribute `calc_metrics` of rectools.metrics.scoring, rectools.metrics and
+    rectools.model_selection.cross_validate (so `cross_validate` scores each fold through it) to
+    `rectools_b200.metrics.calc_metrics` on the home device: the classification and ranking metrics from one device join
+    of the test interactions with the reco table, every value equal to the stock one.  A name imported before `install()`
+    (`from rectools.metrics import calc_metrics`) keeps the stock function, as with the other rebound names.
 
     `transformers`: also rebind the module-level `TorchRanker` of rectools.models.nn.transformers.similarity (u2i of
     `DistanceSimilarityModule`) and of rectools.models.nn.transformers.lightning (item-to-item of
@@ -354,6 +364,20 @@ def install(device: Devices = 0, tc_mode: str = "auto", fast_recommend: bool = T
         _ORIGINALS[_ITEM_KNN_KEY] = {name: cls.__dict__[name] for name in ("_recommend_u2i", "_recommend_i2i")}
         cls._recommend_u2i = _knn_recommend_u2i  # pylint: disable=protected-access
         cls._recommend_i2i = _knn_recommend_i2i  # pylint: disable=protected-access
+    if metrics and _METRICS_KEY not in _ORIGINALS:
+        from .metrics import calc_metrics as device_calc_metrics
+
+        modules = [importlib.import_module(modname) for modname in _METRICS_MODULES]
+
+        def _calc_metrics(metrics, reco, interactions=None, prev_interactions=None, catalog=None, ref_reco=None):  # pylint: disable=redefined-outer-name
+            home = B200ImplicitRanker.default_device
+            return device_calc_metrics(metrics, reco, interactions, prev_interactions, catalog, ref_reco,
+                                       device=home[0] if isinstance(home, tuple) else home)
+
+        _calc_metrics.__doc__ = modules[0].calc_metrics.__doc__
+        _ORIGINALS[_METRICS_KEY] = {mod.__name__: mod.calc_metrics for mod in modules}
+        for mod in modules:
+            mod.calc_metrics = _calc_metrics
     if transformer_modules:
         bound = transformer_ranker(ranker_factory or B200TorchRanker)
         for mod in transformer_modules:
@@ -391,6 +415,9 @@ def uninstall() -> None:
 
         for name, orig in _ORIGINALS.pop(_ITEM_KNN_KEY).items():
             setattr(ImplicitItemKNNWrapperModel, name, orig)
+    if _METRICS_KEY in _ORIGINALS:
+        for modname, orig in _ORIGINALS.pop(_METRICS_KEY).items():
+            importlib.import_module(modname).calc_metrics = orig
     if _EASE_I2I_KEY in _ORIGINALS:
         from rectools.models.ease import EASEModel
 
